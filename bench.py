@@ -2,11 +2,12 @@
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--precision fp16x3|bf16x3|fp16|bf16]
                     [--config cfg2|cfg3|cfg5] [--scaling weak|strong] [--gather maps|labels|none]
+                    [--dump-outputs DIR]
 
 A step = one pass of the hot path over one frame of rays (default: config 2 of BASELINE.json, 376 x 1408 rays,
 64 samples/ray, 8 x 256 MLP, rgb + sigma, 64 bounding primitives) through the public API - Renderer.render, i.e.
 ONE pnr_render_fused call: scene near/far -> ray/box intersection -> stratified depths + ids -> fused PE + MLP
-(tcgen05) -> alpha compositing.
+(wgmma) -> alpha compositing.
   --scaling weak   (default; config 4): every rank renders its own frame, one NCCL all-gather of the rendered tiles
                    (libpnr's pnr_allgather_outputs) rebuilds all of them on every rank inside the step;
   --scaling strong : ONE frame is ray-sharded over the ranks (config 5's layout), same gather;
@@ -15,7 +16,12 @@ ONE pnr_render_fused call: scene near/far -> ray/box intersection -> stratified 
 
 value  : rays/s with inputs resident in HBM (CUDA events per step, L2 flushed between steps, max over ranks)
 e2e    : the same through Renderer.render from pinned HOST rays, H2D + D2H inside the timed region
-roofline: dominant kernel (fused MLP) algorithmic FLOP/s vs the measured dense bf16 tensor peak
+roofline: dominant kernel (fused MLP) algorithmic FLOP/s vs the dense bf16 tensor peak (MEASURED_PEAKS.json when
+         present, else the H100 SXM data sheet)
+--dump-outputs DIR: after the timed steps, what the last timed step returned (Renderer.render's output dict; the
+         oracle's on its strip with --impl reference) as DIR/<name>.npy in float32 (float64 for integer outputs),
+         per-ray outputs on a fixed seeded sample of rays (DIR/sample_rays.npy) sized so that the files stay under
+         64 MB; the inputs depend on the arguments only.
 cpu_baseline / --impl reference: the CPU oracle (port of the spec; the reference source is not in the
          mount) timed on the box's host cores on a bounded strip of the same frame.
 """
@@ -48,7 +54,7 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
 UNIT = "rays/s"
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}   # H100 SXM data sheet, dense
 WORKLOADS = {
     "cfg2": "cfg2: KITTI-360 perspective 376x1408, 64 samples/ray, 8x256 MLP, rgb+sigma, 64 boxes",
     "cfg3": "cfg3: the cfg2 frame + semantic (45) and instance (64) heads, coarse 64 + fine 128 samples/ray (fine pass: 192)",
@@ -70,7 +76,7 @@ def peaks():
         d["_src"] = "measured (MEASURED_PEAKS.json)"
         return d
     d = dict(FALLBACK_PEAKS)
-    d["_src"] = "fallback (B200_PROFILING.md)"
+    d["_src"] = "H100 SXM data sheet (700 W); not a measured rate"
     return d
 
 
@@ -110,7 +116,7 @@ def host_threads() -> int:
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md).  Uses NVML in-process
+    """SM clock / throttle reasons sampled DURING the timed region.  Uses NVML in-process
     (nvidia_ml_py) - spawning nvidia-smi every 100 ms perturbs the GPU - with nvidia-smi as the fallback.
     Created (NVML initialised) before the warm-up so no first-call cost lands in the timed steps."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -215,9 +221,12 @@ def run_reference(args, cfg, rank, world):
     for _ in range(max(args.warmup - 2, 0) if not args.ref_rows else args.warmup):
         orc.run(rows)
     secs = []
+    out = None
     for _ in range(args.steps):
-        _, dt, _, _ = orc.run(rows)
+        _, dt, _, out = orc.run(rows)
         secs.append(dt)
+    if args.dump_outputs and out is not None:
+        dump_outputs(out, Path(args.dump_outputs))
     rays = rows * cfg.W_img
     value = rays * len(secs) / sum(secs)
     sample = (f"{rows}-row strip ({rays} rays) of the {cfg.H}x{cfg.W_img} frame per step; median step "
@@ -227,7 +236,7 @@ def run_reference(args, cfg, rank, world):
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * sum(secs) / len(secs),
         "higher_is_better": True, "scaling": args.scaling, "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOADS[cfg.preset], "sample": sample,
-                   "note": "CPU oracle port; reference source unavailable in /root/reference"},
+                   "note": "CPU oracle port; the reference source is not available"},
         "cpu_baseline": {"value": value, "unit": UNIT, "cores": threads, "kind": "port", "sample": sample,
                          "median_rays_per_s": rays / statistics.median(secs), "os_cpu_count": os.cpu_count()},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -255,6 +264,45 @@ def parity_on_strip(ref_out, gpu_out, far: float) -> dict:
     return rep
 
 
+DUMP_BYTES = 64 << 20
+DUMP_RAYS = 32768
+
+
+def dump_outputs(out: dict, d: Path) -> None:
+    """Renderer.render's outputs -> d/<name>.npy: floating outputs as float32, integer / mask outputs as float64 (exact).
+    Per-ray tensors (first dimension = rays) are cut to a fixed sample of rays (torch.Generator seed 0, ascending;
+    written as sample_rays.npy): at most DUMP_RAYS, fewer when the outputs' bytes per ray would take the files past
+    DUMP_BYTES.  The sample depends on the output shapes only, so every run with the same arguments writes the same
+    rays."""
+    import numpy as np
+    R = out["rgb_map"].shape[0]
+    tensors = {k: v.detach() for k, v in out.items() if torch.is_tensor(v)}
+
+    def nbytes(v, per_ray):   # bytes of v as dumped: 4 per float32 value, 8 per float64 (integer outputs)
+        n = v[0].numel() if per_ray else v.numel()
+        return n * (4 if (v.is_floating_point() or v.is_complex()) else 8)
+
+    per_ray = {k for k, v in tensors.items() if v.dim() >= 1 and v.shape[0] == R}
+    ray_bytes = 8 + sum(nbytes(tensors[k], True) for k in per_ray)          # 8: the ray's index in sample_rays
+    fixed = sum(nbytes(v, False) for k, v in tensors.items() if k not in per_ray)
+    fixed += 256 * (len(tensors) + 1)                                          # .npy headers (128 bytes each)
+    n = min(R, DUMP_RAYS, (DUMP_BYTES - fixed) // ray_bytes)
+    assert n >= 1, f"--dump-outputs: {fixed} bytes of outputs that are not per ray exceed {DUMP_BYTES}"
+    g = torch.Generator().manual_seed(0)
+    rows = torch.sort(torch.randperm(R, generator=g)[:n]).values if n < R else torch.arange(R)
+    arrays = {"sample_rays": rows.numpy().astype(np.float64)}
+    for k in sorted(tensors):
+        v = tensors[k]
+        if k in per_ray:
+            v = v[rows.to(v.device)]
+        v = v.cpu()
+        arrays[k] = v.double().numpy() if not (v.is_floating_point() or v.is_complex()) else v.float().numpy()
+    assert sum(a.nbytes + 256 for a in arrays.values()) <= DUMP_BYTES
+    d.mkdir(parents=True, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(d / f"{k}.npy", a)
+
+
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -270,6 +318,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-fast-mode", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the cfg3 block under 'extra'")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else max(args.warmup, 1)
 
@@ -313,7 +363,7 @@ def main():
     batch = {k: v.to(dev) for k, v in cpu_batch.items()}
     R = batch["rays"].shape[0]
     N = cfg.N_samples
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)     # > 50 MB L2
     tg = parallel.TileGather(dev) if (dist is not None and args.gather != "none") else None
     R_gather = R_frame if args.scaling == "strong" else R * world       # rows of the gathered image(s)
     # weak scaling gathers `world` whole frames: rank r's tile = its frame (per = R rays each)
@@ -350,6 +400,8 @@ def main():
     barrier()
     t_wall = time.perf_counter() - t_wall0
     launches = int(L.pnr_launch_count(0))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, Path(args.dump_outputs))
     step_ms = [a.elapsed_time(b) for a, b in evs]
     total_ms = torch.tensor([sum(step_ms)], dtype=torch.float64, device=dev)
     if dist is not None:
@@ -387,13 +439,6 @@ def main():
     achieved = alg_flop / (mlp_t / 1e3) / 1e12
     peak = float(pk["bf16_tflops_sustained"])
     traffic, traffic_src = None, None
-    prof = ROOT / "profiles" / "mlp_ncu_summary.json"
-    if prof.exists() and args.config == "cfg2" and R == R_frame:
-        try:
-            ent = json.loads(prof.read_text()).get(args.precision, {})
-            traffic, traffic_src = ent.get("dram_bytes_per_launch"), ent.get("source")
-        except Exception:
-            traffic = None
     mlp_per_step = mlp_t * (1.0 + (N / Nz if cfg.N_importance else 0.0))    # coarse launch scaled by its samples
     roofline = {"bound": "tensor", "kernel": "mlp_fused_kernel", "achieved": achieved, "peak": peak,
                 "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,

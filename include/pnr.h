@@ -1,4 +1,4 @@
-/* pnr.h — C ABI of libpnr (PanopticNeRF render hot path, sm_100a).
+/* pnr.h — C ABI of libpnr (PanopticNeRF render hot path, sm_90a).
  *
  * The reference exposes this path only as a Python plugin surface in lib/networks
  * (make_network, Renderer.render, batchify_rays, raw2outputs, sample_pdf; SURVEY.md 8(b)); it has
@@ -279,7 +279,7 @@ int pnr_mlp_trunk_forward(pnr_ctx* ctx, const float* pts, const float* rays, con
  * sums of dZ (NULL: skipped), for dZ [S, No] (row stride ld_dz) and X [S, Ni] (row stride ld_x), fp32, No, Ni <= 256
  * (wider layers - the skip layer's [gamma(x), h], the view layer's [feature, gamma(d)] - are split by columns into
  * two calls on the same dZ).  A split-K GEMM over the samples on the tensor cores: every CTA accumulates its share of
- * the samples in tensor memory (operands split into 16-bit hi / lo parts on the fly, hi.hi + lo.hi + hi.lo, fp32
+ * the samples in registers (operands split into 16-bit hi / lo parts on the fly, hi.hi + lo.hi + hi.lo, fp32
  * accumulation), the partial products are added in a fixed order by a second kernel (deterministic).
  * precision = PNR_PREC_BF16X3 (~2^-17 per product, fp32 exponent range: gradients need no scaling) or PNR_PREC_FP16X3
  * (~2^-21 per product; dz_scale - DEVICE scalar or NULL - is a power of two dZ is multiplied by on load and dW divided
@@ -296,7 +296,7 @@ int pnr_wgrad(const float* dz, int64_t ld_dz, int32_t No, const float* x, int64_
 /* a8 on the training path, the layers AFTER the trunk (alpha / feature / view / rgb / heads; SURVEY 8(f) rank 2):
  * y [S, N] (row stride ld_y) = act(x W^T + bias) for x [S, K] (row stride ld_x), fp32, N <= 256, K <= 512, on the
  * tensor cores with the 3-product 16-bit operand split of the fused MLP kernel (precision = PNR_PREC_FP16X3 or
- * PNR_PREC_BF16X3), fp32 accumulation in tensor memory.  W is [N, K] (row stride ld_w), or with transposed != 0 a
+ * PNR_PREC_BF16X3), fp32 accumulation in registers.  W is [N, K] (row stride ld_w), or with transposed != 0 a
  * [K, N] matrix read transposed: dL/dx = g W of a layer y = x W^T is pnr_linear(g, W, transposed = 1).  bias [N] or
  * NULL; relu != 0 applies max(., 0).  in_scale: DEVICE scalar or NULL - a power of two the rows of x are multiplied
  * by on load, the result divided by it (exact): gradients of a mean-reduced loss are ~1e-6 and their fp16 parts would

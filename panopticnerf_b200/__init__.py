@@ -1,4 +1,4 @@
-"""panopticnerf_b200 — B200-native (sm_100a) implementation of the PanopticNeRF per-ray render path
+"""panopticnerf_b200 — H100-native (sm_90a) implementation of the PanopticNeRF per-ray render path
 behind the reference's lib/networks plugin surface (make_network, make_renderer, Renderer.render,
 batchify_rays, raw2outputs, sample_pdf).  All compute is hand-written CUDA in libpnr.so (C ABI,
 include/pnr.h); there is no CPU or PyTorch fallback."""

@@ -12,7 +12,7 @@ from typing import Optional
 
 import torch
 
-# PNR_LIB: load a development variant of the library (tools/timeline.py: the -DPNR_TIMELINE build)
+# PNR_LIB: load a development variant of the library (a build with extra flags, _build.build(out=...))
 _LIB_PATH = Path(os.environ.get("PNR_LIB") or Path(__file__).resolve().parent / "libpnr.so")
 _lib: Optional[C.CDLL] = None
 
@@ -128,7 +128,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not _LIB_PATH.exists():
             raise PnrError(f"{_LIB_PATH} is missing - run `python -c 'import __graft_entry__ as g; g.build()'` "
-                           "(nvcc, sm_100a).  panopticnerf_b200 has no CPU or PyTorch fallback.")
+                           "(nvcc, sm_90a).  panopticnerf_b200 has no CPU or PyTorch fallback.")
         L = C.CDLL(str(_LIB_PATH))
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(L, name)          # AttributeError here = header/library mismatch

@@ -42,11 +42,11 @@ constexpr int kMaxDevices = 64;
 // SM count of device `dev` (cached per device; every per-device fact in this library is indexed by ordinal).
 inline int num_sms(int dev) {
   static int n[kMaxDevices] = {0};
-  if (dev < 0 || dev >= kMaxDevices) return 148;
+  if (dev < 0 || dev >= kMaxDevices) return 132;
   if (n[dev] == 0) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[dev] = v > 0 ? v : 148;
+    n[dev] = v > 0 ? v : 132;
   }
   return n[dev];
 }

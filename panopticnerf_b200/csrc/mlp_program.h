@@ -1,75 +1,80 @@
 // mlp_program.h — the per-tile "program" the fused MLP kernel interprets (built once on the host when
-// weights are loaded, see pnr_api.cu) and the shared-memory / tensor-memory maps both sides agree on.
+// weights are loaded, see pnr_api.cu) and the shared-memory map of the sm_90 kernel (mlp_wgmma.cu).
 //
-// A tile (128 samples) runs a fixed sequence of STEPS (one GEMM + epilogue each: trunk layers, heads,
-// view branch with the feature layer folded in).  Every step is issued as two N-HALVES (h0, h1) with separate
-// accumulator column ranges, so that the epilogue of h0 (E0) overlaps the MMAs of h1, and the epilogue of h1 (E1)
-// overlaps the first K-chunks of the next step's h0 (which only need what E0 wrote).  Each half is a
-// list of weight STAGES (<= 32 KB: up to 128 rows x 64 K, hi image then lo image), streamed by TMA.
+// A tile runs a fixed sequence of STEPS (one GEMM + epilogue each: trunk layers, heads, view branch with the feature
+// layer folded in).  Every step is issued as two N-HALVES (h0, h1) with separate accumulator column ranges; each half
+// is a list of weight STAGES (<= 32 KB: up to 128 rows x 64 K, hi image then lo image), streamed by TMA.  A operands
+// are addressed as packed operand columns (see the column map below).  The sm_90 kernel runs the steps in order and
+// reads the stage list (st) and the epilogue table (ep).
+//
+// UNUSED ON SM_90.  The program also carries a finer-grained schedule, written for a kernel in which a step's
+// epilogue overlaps the next step's MMAs: per stage the epilogue hand-offs it waits for and the commits it makes
+// (flags other than F_FIRST / F_COMMIT_ACC1 / F_COMMIT_VIEW, IssueDesc, acc_flip, view_step), placed on the host from the
+// operand-column footprints of every stage and epilogue part (Builder::finalize; its consistency is checked by
+// tests/test_cpu_hazards.py).  The sm_90 kernel executes none of it: it runs each step's epilogue after all of that
+// step's MMAs have retired, and reads F_FIRST (first MMA of a half overwrites) and F_COMMIT_ACC1 / F_COMMIT_VIEW (last
+// stage of a step) only.  The parts of that schedule:
 //
 // E1 works in two PARTS (column blocks a, b; part b may be empty) that are SIGNALLED separately, so the next step's
-// third K-chunk can start when half of E1 is done (timeline r2: 75.4 k -> 71.5 k cycles per tile).  (Releasing E0's
-// stores in two blocks with two write-after-read barriers was measured as well: no gain, removed.)
-// Epilogue -> MMA hand-offs are three monotonic shared-memory counters (E0 done, E1 part a done, E1 done), bumped
-// once per epilogue warp and watched by the scout thread: every stage carries the counts it needs.
+// first K-chunks can start when half of E1 is done.  Epilogue -> MMA hand-offs are three monotonic counters (E0 done,
+// E1 part a done, E1 done): every stage carries the counts it needs.
 //
-// ACCUMULATOR FLIP.  A tile's last step (view or logits, N <= 128) accumulates in the lower 128 accumulator columns, and
-// so does the first half of the next tile's first layer - which therefore had to wait until the last step's epilogue
-// had drained them, at the one place where the epilogue warps have more work than the tensor pipe.  With acc_flip set,
-// odd tiles address every accumulator column XOR 128 (MMA destinations and epilogue loads alike; no accumulator
-// range straddles column 128): the first half of layer 0 then lands in the half the previous tile's last step does
-// not use and is issued right behind it.  Everything else (K order, activation columns) is unchanged.
+// ACCUMULATOR FLIP.  With acc_flip set, odd tiles address every accumulator column XOR 128 (no accumulator range
+// straddles column 128), so that the first half of a tile's layer 0 does not wait for the previous tile's last
+// epilogue.
 //
-// VIEW ON PRODUCERS (networks without heads, forward).  The view step is the tile's last; its epilogue (ReLU, the
-// 3 x W/2 rgb dot products on CUDA cores, the raw store) sits in front of the next tile's layer-0 epilogue on the
-// epilogue warps - the one resource the tile boundary is bound by (timeline r2: ~3.5 k of a 70 k-cycle tile).  In such
-// programs (view_step >= 0) the four positional-encoding warps - one thread per row, idle most of the tile - run it
-// instead: the view step's last stage commits to its own mbarrier (F_COMMIT_VIEW), the epilogue warps skip the step
-// (it is not part of the E0 / E1 counts), the producer warp of a lane quarter reads its 32 rows' accumulators, and a
-// fourth counter (+1 per producer warp and tile) gates the first stage of the next tile that reuses those columns.
+// VIEW ON PRODUCERS (networks without heads, forward).  view_step >= 0: the view step is the tile's last and may run its
+// epilogue apart from the other steps (on sm_90 such a program runs exactly like the plain one); its last stage is flagged F_COMMIT_VIEW and the first stage of the next tile
+// that reuses its accumulator columns waits for it.
 //
-// BACKWARD (first slice of the training path: dL/d(embedded input) through the trunk, on the same tiles).  A backward
-// program is the trunk's forward steps - whose EPI_RELU_TO_A epilogues also save the 16-column sign patterns of their
-// activations in shared memory (slot n_valid-1; the view-direction embedding's region, unused here) - followed by one
+// BACKWARD (dL/d(embedded input) through the trunk, on the same tiles).  A backward program is the trunk's forward
+// steps - whose EPI_RELU_TO_A epilogues also save the 16-column sign patterns of their activations - followed by one
 // step per layer in reverse order with the TRANSPOSED weights streamed the same way: the A operand is the gradient
-// w.r.t. the layer's pre-activation (tensor-memory activation columns, hi/lo split like any activation), the
-// accumulator receives the gradient w.r.t. the layer's input, and the epilogue gates it with the saved pattern of the
-// layer below.  The last forward layer's epilogue does not keep its activation: it loads the incoming gradient from
-// global memory and gates it with its own sign pattern.  The embedded-input columns (layer 0, and the skip layer's
-// first columns) are written / accumulated to the output rows by EPI_GRAD_OUT steps.
+// w.r.t. the layer's pre-activation (hi/lo split like any activation), the accumulator receives the gradient w.r.t.
+// the layer's input, and the epilogue gates it with the saved pattern of the layer below.  The last forward layer's
+// epilogue does not keep its activation: it loads the incoming gradient from global memory and gates it with its own
+// sign pattern.  The embedded-input columns (layer 0, and the skip layer's first columns) are written / accumulated
+// to the output rows by EPI_GRAD_OUT steps.
 //
-// The program travels as a __grid_constant__ kernel parameter (constant bank, uniform datapath for the issuing
-// thread; nothing shared between contexts, streams, devices or graph replays).
+// The program travels as a __grid_constant__ kernel parameter (constant bank; nothing shared between contexts,
+// streams, devices or graph replays).
 #pragma once
 #include <stdint.h>
 
 namespace pnr {
 
-constexpr int kTileM = 128;               // samples per tile = TMEM lanes = UMMA M
-constexpr int kRing = 4;                  // weight stages in flight
+constexpr int kTileM = 128;               // M of the program's instruction descriptors (IssueDesc::idesc)
+constexpr int kRows = 64;                 // samples per tile of the sm_90 kernel = wgmma M of one warpgroup
+constexpr int kRing = 2;                  // weight stages in flight
 constexpr int kStageBytes = 32768;        // max stage: N=128 rows x 64 K x 2 bytes x (hi + lo images)
-constexpr int kEpiWarps = 8;              // TMEM->reg->TMEM activation warps (2 per lane quarter; 12 and 16 measured slower)
-constexpr int kProWarps = 4;              // positional-encoding producer warps (one thread per row)
-constexpr int kMlpThreads = (kEpiWarps + kProWarps + 4) * 32;   // + TMA warp, MMA issuer, scout, second MMA issuer = 512
-constexpr int kClusterSize = 2;           // CTAs sharing one weight stream by TMA multicast
+constexpr int kConsumerThreads = 128;     // one warpgroup: MMAs, positional encoding and epilogues
+constexpr int kMlpThreads = kConsumerThreads + 32;   // + the weight-stream warp
 constexpr int kMaxStages = 256;
 constexpr int kMaxSteps = 24;
 constexpr int kMaxConsts = 4096;          // floats: biases + sigma / rgb weights
 
-// Tensor-memory column map (512 x 32-bit columns, 128 lanes).
+// Operand column map.  The program addresses its A operands as "packed columns" of 32 bits (two 16-bit values of
+// consecutive K) - 512 of them per row, the first 256 being accumulator space.
 constexpr int kColAcc = 0;                // fp32 accumulators, up to 256 columns
 constexpr int kColAHi = 256;              // activations, 16-bit hi parts, 2 per column (K <= 256)
 constexpr int kColALo = 384;              // activations, 16-bit lo parts
 constexpr int kColHeadHi = 128;           // head hidden activations (K <= 128) live in the upper
 constexpr int kColHeadLo = 192;           //   half of the accumulator region while it is free
+// The sm_90 kernel keeps accumulators in registers and the operand columns [kColOpBase, 512) in shared memory, in
+// the no-swizzle K-major layout of wgmma: packed column c of row r is K-core (c - kColOpBase) / 4, i.e. the bytes
+// ((c - kColOpBase) / 4 * kRows + r) * 16 + (c % 4) * 4.
+constexpr int kColOpBase = 128;
 
-// Shared-memory map (bytes from the 1024-aligned dynamic base).
+// Shared-memory map of the sm_90 kernel (bytes from the 1024-aligned dynamic base).
 constexpr int kSmemRing = 0;
-constexpr int kSmemEmb = kRing * kStageBytes;          // xyz embedding, UMMA no-swizzle K-major: hi 16K, lo 16K
-constexpr int kEmbPartBytes = kTileM * 64 * 2;         // 16 KB
-constexpr int kSmemDir = kSmemEmb + 2 * kEmbPartBytes; // view-dir embedding, 2 buffers x (hi 8K, lo 8K)
-constexpr int kDirPartBytes = kTileM * 32 * 2;         // 8 KB
-constexpr int kSmemProg = kSmemDir + 4 * kDirPartBytes;
+constexpr int kSmemOp = kRing * kStageBytes;           // operand columns [128, 512): 96 K-cores x kRows x 16 B
+constexpr int kOpKCoreBytes = kRows * 16;
+constexpr int kSmemEmb = kSmemOp + (512 - kColOpBase) / 4 * kOpKCoreBytes;   // xyz embedding: hi 8K, lo 8K
+constexpr int kEmbPartBytes = kRows * 64 * 2;
+constexpr int kSmemDir = kSmemEmb + 2 * kEmbPartBytes; // view-dir embedding: hi 4K, lo 4K
+constexpr int kDirPartBytes = kRows * 32 * 2;
+constexpr int kSmemStage = kSmemDir + 2 * kDirPartBytes;   // fp32 accumulators of one 128-column window
+constexpr int kStageLd = 128 + 4;                      // floats per staged row (padding: conflict-free 16-byte reads)
 
 enum : uint8_t { A_TMEM = 0, A_EMB = 1, A_DIR = 2 };
 enum : uint16_t {
@@ -97,7 +102,7 @@ constexpr bool epi_writes_a(uint8_t kind) { return kind == EPI_RELU_TO_A || kind
 struct StageDesc {     // one weight stage = one bulk copy + its MMAs
   uint32_t gofs;       // byte offset into the packed weight stream
   uint32_t bytes;
-  uint16_t n;          // UMMA N (rows of the weight tile = width of this half)
+  uint16_t n;          // MMA N (rows of the weight tile = width of this half)
   uint16_t acc_col;    // accumulator column of this half
   uint16_t a_off;      // A_TMEM: packed column of the first K16 step (hi part)
   uint16_t a_lo_off;   //         and of the lo part
@@ -108,7 +113,7 @@ struct StageDesc {     // one weight stage = one bulk copy + its MMAs
 };
 
 struct IssueDesc {     // the same stage, pre-digested for the MMA-issuing warp: every word is used as it is
-  uint32_t idesc;      // tcgen05 instruction descriptor (M=128, N=n, operand format)
+  uint32_t idesc;      // instruction-descriptor word (M=128, N=n, operand format); not read on sm_90
   uint32_t b_lo_base;  // low word of the weight-tile descriptor without its address: (n*16 >> 4) << 16
   uint32_t b_inc;      // address-field step per K16: 2 * n*16 >> 4
   uint32_t lo_off16;
@@ -201,22 +206,25 @@ struct MlpLaunch {
 };
 static_assert(sizeof(MlpLaunch) <= 32764, "kernel parameter space is 32764 bytes");
 
-// backward kernels: ReLU sign patterns, uint16 [slot][16-column group][row], in the view-direction region
-constexpr int kSmemMask = kSmemDir;
-constexpr int kMaskSlotU16 = 16 * kTileM;                     // one layer of up to 256 columns
-constexpr int kMaxMaskSlots = 4 * kDirPartBytes / (kMaskSlotU16 * 2);   // 8
-constexpr int kSmemConsts = kSmemProg;   // (the program itself is in the kernel's parameter bank)
-constexpr int kSmemPart = kSmemConsts + kMaxConsts * 4;      // [kEpiWarps/4][128][4] floats
-constexpr int kSmemBars = kSmemPart + (kEpiWarps / 4) * kTileM * 4 * 4;
+// backward kernels: ReLU sign patterns, uint16 [slot][16-column group][row], in the head operand columns (unused by
+// backward programs)
+constexpr int kSmemMask = kSmemOp;
+constexpr int kMaskSlotU16 = 16 * kRows;                      // one layer of up to 256 columns
+constexpr int kMaxMaskSlots = 8;
+static_assert(kMaxMaskSlots * kMaskSlotU16 * 2 <= (kColAHi - kColOpBase) / 4 * kOpKCoreBytes, "sign patterns overflow");
+constexpr int kSmemPart = kSmemStage + kRows * kStageLd * 4;   // [2 column shares][kRows][4] floats
+constexpr int kSmemBars = kSmemPart + 2 * kRows * 4 * 4;
 constexpr int kSmemTotal = kSmemBars + 256;
 // compositing epilogue: weights of the tile's rows, per-quarter transmittance products and the carried transmittance
-// (double-buffered by tile parity), per-quarter partial sums of every composited channel (double-buffered)
+// (double-buffered by tile parity), per-quarter partial sums of every composited channel (double-buffered); a
+// "quarter" is an aligned group of 32 samples, kRows / 32 of them per tile
+constexpr int kQuarters = kRows / 32;
 constexpr int kCompMaxCh = 5 + 128 + 128;                       // rgb(3) depth acc + C + K
 constexpr int kCompChPad = (kCompMaxCh + 31) / 32 * 32;         // 288
-constexpr int kSmemCompW = kSmemTotal;                          // float w_row[128]
-constexpr int kSmemCompQ = kSmemCompW + kTileM * 4;             // float qprod[2][4]; float carry[2]; (64 bytes)
-constexpr int kSmemCompS = kSmemCompQ + 64;                     // float qsum[2][4][kCompChPad]
-constexpr int kSmemCompR = kSmemCompS + 2 * 4 * kCompChPad * 4; // float racc[kCompChPad]: running sums of the open ray
+constexpr int kSmemCompW = kSmemTotal;                          // float w_row[kRows]
+constexpr int kSmemCompQ = kSmemCompW + kRows * 4;              // float qprod[2][kQuarters]; float carry[2]; (64 bytes)
+constexpr int kSmemCompS = kSmemCompQ + 64;                     // float qsum[2][kQuarters][kCompChPad]
+constexpr int kSmemCompR = kSmemCompS + 2 * kQuarters * kCompChPad * 4; // float racc[kCompChPad]: running sums of the open ray
 constexpr int kSmemTotalComp = kSmemCompR + kCompChPad * 4;
 static_assert(kSmemTotalComp <= 232448, "shared-memory map exceeds the 227 KB per-CTA limit");
 

@@ -7,7 +7,7 @@
 #include <vector>
 #include "common.cuh"
 #include "mlp_program.h"
-#include "tc05.cuh"
+#include "sm90.cuh"
 
 namespace pnr {
 
@@ -24,7 +24,7 @@ int set_error(int code, const char* fmt, ...) {
 }
 void count_launch(int n) { g_launches += n; }
 
-int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream);  // mlp_tc05.cu
+int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream);  // mlp_wgmma.cu
 
 }  // namespace pnr
 
@@ -96,6 +96,13 @@ static inline float bf2f(uint16_t h) {
 }
 
 namespace {
+
+// Instruction-descriptor word of the program's issue table (IssueDesc::idesc): M, N and operand-format fields of a
+// 16-bit-operand MMA with fp32 accumulators.  Part of the overlapped schedule the sm_90 kernel does not execute
+// (mlp_program.h, "UNUSED ON SM_90").
+constexpr uint32_t make_idesc_f32acc(int M, int N, int fmt) {
+  return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
+}
 
 struct Mat { const float* w; int out, in; };  // row-major [out, in]
 
@@ -195,6 +202,8 @@ struct Builder {
       const int mrow0 = (h == 1 && segs_h1) ? 0 : r0;     // first row of the half in its weight matrix
       const int half_first = prog.n_stages;
       if (h == 1) info.n0_stage = prog.n_stages;
+      // the kernel issues one wgmma m64nNk16 per K step of a half: N a multiple of 8, at most 128
+      if ((r1 - r0) % 8 != 0 || r1 - r0 > 128 || r1 <= r0) { err = "half of a step is not an MMA width (multiple of 8, <= 128)"; return false; }
       for (size_t si = 0; si < hsegs.size(); ++si) {
         const Seg& sg = hsegs[si];
         // K per stage: 64 with hi+lo images (x3), 128 with the hi image only (1-pass): <= 32 KB either way
@@ -406,8 +415,8 @@ extern "C" int pnr_create(const pnr_config* cfg, pnr_ctx** out) {
   PNR_CHECK_ARG(cfg->device >= 0 && cfg->device < ndev, "pnr_create: device %d of %d", cfg->device, ndev);
   cudaDeviceProp prop;
   PNR_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10)
-    return set_error(PNR_ERR_UNSUPPORTED, "pnr_create: device %d is sm_%d%d; libpnr is sm_100a only (no fallback path)",
+  if (prop.major != 9 || prop.minor != 0)
+    return set_error(PNR_ERR_UNSUPPORTED, "pnr_create: device %d is sm_%d%d; libpnr is sm_90a only (no fallback path)",
                      cfg->device, prop.major, prop.minor);
   PNR_CHECK_ARG(cfg->device < kMaxDevices, "pnr_create: device ordinal %d >= %d", cfg->device, kMaxDevices);
   DeviceGuard guard(cfg->device);   // the caller's current device is restored on return

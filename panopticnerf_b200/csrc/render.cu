@@ -4,6 +4,7 @@
 // (~1.5 GB at the default workspace) instead of being materialised for the whole frame (46 GB at config 3).
 #include <cstring>
 #include "common.cuh"
+#include "mlp_program.h"   // kRows
 #include "ray_math.h"   // PNR_MAX_HITS
 
 struct pnr_ctx;
@@ -102,14 +103,13 @@ __global__ void __launch_bounds__(256) fill2_kernel(float* __restrict__ a, float
   if (i < n) { a[i] = va; b[i] = vb; }
 }
 
-// Rays per chunk by default: raw of ~1.5 GB, never below ~64 tiles of the fused MLP per SM and pass.  (Measured,
-// B200: chunks small enough to keep raw L2-resident - 96 MB, ~1 200 rays of config 3 - leave the persistent MLP
-// kernel 4-12 tiles per SM and launch, and its ramp-up / tail then costs far more than the HBM round trip of raw
-// saves: 633 ms per config-3 frame against ~430.)
+// Rays per chunk by default: raw of ~1.5 GB, never below ~64 tiles of the fused MLP per SM and pass (chunks small
+// enough to keep raw L2-resident leave the persistent MLP kernel a few tiles per SM and launch, and its ramp-up / tail
+// then costs more than the HBM round trip of raw saves).
 int64_t default_chunk_rays(int Nt, int CH) {
   const size_t raw_per_ray = (size_t)Nt * CH * 4;
   int64_t by_bytes = (int64_t)((1536ull << 20) / raw_per_ray);
-  const int64_t by_tiles = ((int64_t)148 * 64 * 128 + Nt - 1) / Nt;
+  const int64_t by_tiles = ((int64_t)num_sms() * 64 * kRows + Nt - 1) / Nt;
   return by_bytes > by_tiles ? by_bytes : by_tiles;
 }
 

@@ -6,8 +6,8 @@ Parameter names follow nerf-pytorch, which the reference is recalled to inherit,
     pts_linears.{i}, alpha_linear, feature_linear, views_linears.0, rgb_linear,
     semantic_linears.{0,1}, instance_linears.{0,1}
 
-``forward(pts, viewdirs)`` runs the fused sm_100a kernel (positional encoding + all layers + heads in one
-launch, activations resident in tensor memory) through the libpnr C ABI.  There is no PyTorch forward:
+``forward(pts, viewdirs)`` runs the fused sm_90a kernel (positional encoding + all layers + heads in one
+launch, activations kept in shared memory) through the libpnr C ABI.  There is no PyTorch forward:
 CPU tensors raise.
 """
 from __future__ import annotations

@@ -39,7 +39,7 @@ def wgrad(dz: torch.Tensor, x: torch.Tensor, bias: bool = True, precision: str =
           scale: Optional[torch.Tensor] = None):
     """(dW [No, Ni], db [No] or None) = (dz^T @ x, dz.sum(0)) for dz [S, No], x [S, Ni] (fp32, No <= 256): the weight
     and bias gradient of y = x W^T + b from dz = dL/dy, on the tensor cores (pnr_wgrad: 16-bit hi / lo operand parts,
-    fp32 accumulation in tensor memory, deterministic).  Ni > 256 (the skip and view layers' concatenated inputs) is
+    fp32 accumulation in registers, deterministic).  Ni > 256 (the skip and view layers' concatenated inputs) is
     covered by one call per 256-column block of x; neither dz^T nor a split copy of an operand is materialised.
     precision "bf16x3": ~2^-17 per product, no scaling needed; "fp16x3": ~2^-21 per product with `scale`, a device
     scalar power of two (`_pow2_scale(dz)`) that keeps the fp16 parts of tiny gradients normal."""

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds (cross-compiled for sm_100a), loads, and exports every symbol that
+"""CPU: the C-ABI library builds (cross-compiled for sm_90a), loads, and exports every symbol that
 include/pnr.h declares; the ctypes table mirrors the header; the product refuses CPU tensors loudly.
 No compute call is made (there is no GPU here)."""
 import ctypes as C
@@ -43,15 +43,15 @@ def test_ctypes_argument_counts_match_header():
         assert n == len(_capi.SIGNATURES[name][1]), f"{name}: header has {n} parameters, ctypes {len(_capi.SIGNATURES[name][1])}"
 
 
-def test_sass_is_blackwell_native():
-    """cuobjdump evidence (B200_PROFILING.md): tcgen05.mma -> UTC*MMA, tcgen05.ld/st -> LDTM/STTM,
-    bulk TMA -> UBLKCP; and only sm_100a code is embedded."""
+def test_sass_is_hopper_native():
+    """cuobjdump evidence: wgmma -> HGMMA (fp16 and bf16 operands), bulk TMA -> UBLKCP, mbarrier waits -> SYNCS;
+    and only sm_90a code is embedded."""
     import subprocess
     so = ROOT / "panopticnerf_b200" / "libpnr.so"
     sass = subprocess.run(["cuobjdump", "-sass", str(so)], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    assert not re.search(r"arch = sm_(?!100a)", sass)
-    for mnem in ("UTCHMMA", "LDTM", "STTM", "UBLKCP"):
+    assert "sm_90a" in sass
+    assert not re.search(r"arch = sm_(?!90a)", sass)
+    for mnem in ("HGMMA.64x128x16.F32 ", "HGMMA.64x128x16.F32.BF16", "UBLKCP", "SYNCS"):
         assert mnem in sass, mnem
 
 

@@ -1,8 +1,10 @@
-"""CPU tier: tensor-memory hazard check of the fused MLP program (Builder::finalize in csrc/pnr_api.cu).
+"""CPU tier: hazard check of the fused MLP program's overlapped schedule (Builder::finalize in csrc/pnr_api.cu).
+The sm_90 kernel does not execute this schedule (it runs a step's epilogue after all of the step's MMAs; see
+"UNUSED ON SM_90" in csrc/mlp_program.h); the test pins that the program's flags stay self-consistent.
 
-The kernel keeps accumulators, activations (16-bit hi / lo parts) and head activations in overlapping tensor-memory
-column ranges and orders the MMA stages against the epilogue parts of every step with
-  * tcgen05.commit -> mbarrier:  acc_full[0/1] (F_COMMIT_ACC0/1), war_ok (F_COMMIT_WAR),
+The program keeps accumulators, activations (16-bit hi / lo parts) and head activations in overlapping operand-column
+ranges and orders the MMA stages against the epilogue parts of every step with
+  * MMA commit -> mbarrier:  acc_full[0/1] (F_COMMIT_ACC0/1), war_ok (F_COMMIT_WAR),
   * three monotonic counters epilogue -> MMA issuer (E0 done, E1 part a done, E1 done): every stage of the issue
     table carries the counts it needs (IssueDesc.needs).
 Their placement is computed on the host.  This test rebuilds the happens-before graph they imply, over two
@@ -93,7 +95,7 @@ def events_and_edges(prog, tiles=3):
                 g = t * n_esteps + ((needs >> shift) & 0xFF) - 2      # global index of the last step required
                 if g >= 0:
                     edges.append(((name,) + order[g], ev))
-        if s == vs:      # the producer warps read the whole accumulator of the step and write nothing to tensor memory
+        if s == vs:      # the producer warps read the whole accumulator of the step and write no operand column
             reads[("EV", t)], writes[("EV", t)] = cols(t, ed, 0, ed.n, False)[0], []
             reads[("DV", t)], writes[("DV", t)] = [], []
             edges.append((("EV", t), ("DV", t)))

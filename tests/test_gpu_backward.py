@@ -399,7 +399,7 @@ def test_backward_trunk_collects_the_stash_maxima():
 
 
 # ------------------------------------------------------------------------------------------------
-# pnr_wgrad: the weight-gradient GEMM over the samples (csrc/wgrad_tc05.cu) vs float64 on the CPU
+# pnr_wgrad: the weight-gradient GEMM over the samples (csrc/wgrad_wgmma.cu) vs float64 on the CPU
 # ------------------------------------------------------------------------------------------------
 def _wgrad_case(S_, No, Ni, seed, gscale=1e-6):
     g = torch.Generator().manual_seed(seed)
@@ -411,7 +411,8 @@ def _wgrad_case(S_, No, Ni, seed, gscale=1e-6):
 
 @pytest.mark.parametrize("prec", ["fp16x3", "bf16x3"])
 @pytest.mark.parametrize("S_,No,Ni", [(4096, 256, 256), (5000, 256, 63), (777, 128, 283), (33, 1, 256), (1, 3, 128),
-                                      (20011, 45, 128), (148 * 32 * 3 + 5, 64, 319), (31, 256, 16), (200, 130, 17)])
+                                      (20011, 45, 128), (148 * 32 * 3 + 5, 64, 319), (132 * 64 * 3 + 5, 64, 319),
+                                      (31, 256, 16), (200, 130, 17)])
 def test_wgrad_matches_float64(S_, No, Ni, prec):
     from panopticnerf_b200.lib.train.mlp_backward import wgrad, _pow2_scale
     dz, x = _wgrad_case(S_, No, Ni, seed=S_ + No + Ni)
@@ -463,11 +464,12 @@ def test_wgrad_views_determinism_and_errors():
 
 
 # ------------------------------------------------------------------------------------------------
-# pnr_linear: y = act(x W^T + b) of the layers after the trunk on the training path (csrc/linear_tc05.cu)
+# pnr_linear: y = act(x W^T + b) of the layers after the trunk on the training path (csrc/linear_wgmma.cu)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("S_,K,N,relu,prec", [(4096, 256, 256, False, "fp16x3"), (1000, 283, 128, True, "fp16x3"),
                                              (130, 256, 1, False, "fp16x3"), (5000, 128, 45, False, "bf16x3"),
                                              (129, 128, 3, False, "fp16x3"), (148 * 128 * 2 + 77, 256, 128, True, "bf16x3"),
+                                             (132 * 128 * 2 + 77, 256, 128, True, "bf16x3"),
                                              (7, 27, 64, False, "fp16x3"), (300, 512, 256, False, "fp16x3")])
 def test_linear3x_matches_float64(S_, K, N, relu, prec):
     from panopticnerf_b200.lib.train.mlp_backward import linear3x

@@ -1,4 +1,4 @@
-"""GPU parity of the fused tcgen05 MLP (Network.forward, SURVEY 8(a) a7+a8) and of the end-to-end
+"""GPU parity of the fused wgmma MLP (Network.forward, SURVEY 8(a) a7+a8) and of the end-to-end
 Renderer.render, against the CPU oracle with identical weights and inputs."""
 import pytest
 import torch

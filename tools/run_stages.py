@@ -1,4 +1,4 @@
-"""One launch of every HBM-bound stage at the cfg2 frame size (for ncu captures of achieved DRAM throughput)."""
+"""One launch of every HBM-bound stage at the cfg2 frame size (for captures of achieved DRAM throughput with torch.profiler)."""
 import sys
 from pathlib import Path
 import torch
