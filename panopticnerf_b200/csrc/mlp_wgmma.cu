@@ -6,7 +6,8 @@
 //     one row each) and gamma(d) (threads 64-127), splits them into 16-bit hi/lo parts and writes them into shared
 //     memory in the no-swizzle K-major operand layout;
 //   * one weight-stream warp copies the pre-packed weight stages (<= 32 KB: hi image then lo image of an N-row x 64-K
-//     tile) from L2 into a 2-deep shared-memory ring with cp.async.bulk + mbarrier complete_tx;
+//     tile) from L2 into a 4-slot shared-memory ring, one K-half of a stage per 16 KB slot, with cp.async.bulk +
+//     mbarrier complete_tx;
 //   * the consumer warpgroup issues wgmma m64nNk16 (N <= 128 per half of a step), both operands in shared memory:
 //     A = an embedding or the previous layer's activations, B = the weight stage; fp32 accumulators in registers;
 //   * once a step's MMAs have retired, its accumulators pass through a 64 x 128 fp32 staging tile in shared memory
@@ -298,14 +299,121 @@ __device__ __forceinline__ constexpr uint32_t inf_bits16() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// MMA issue: one weight stage = ksteps K16 steps of wgmma m64nNk16 (x3: three products each, mma_run).  PTX spells
-// out the accumulator registers, so N is a template argument and mma_stage dispatches on the stage's N.
+// Weight ring.  The ring region (kRing program stages of kStageBytes) is run as kSlots slots of half a stage: a stage
+// arrives as one slot per K-half, slot j holding the K16 steps [k0, k0 + kn) of the stage's hi image and then (x3) the
+// same steps of its lo image.  The images keep K-cores outermost, so each part is one contiguous range of the packed
+// stream.  Four slots keep two stages in flight while one is consumed.
 // ------------------------------------------------------------------------------------------------
+constexpr int kSlots = 4;
+constexpr int kSlotBytes = kRing * kStageBytes / kSlots;
+static_assert(2 * kSlotBytes == kStageBytes, "a program stage is two ring slots");
+
+__device__ __forceinline__ int stage_slots(const StageDesc& sd) { return sd.ksteps > 1 ? 2 : 1; }
+// the K16 steps [k0, k0 + kn) of slot j of the stage (the first K-half is the larger one)
+__device__ __forceinline__ void slot_ksteps(const StageDesc& sd, int j, int& k0, int& kn) {
+  const int h = (sd.ksteps + 1) >> 1;
+  k0 = j ? h : 0;
+  kn = j ? sd.ksteps - h : h;
+}
+
+// The slot's MMAs have retired: one arrival per consumer warp (lane 0) on its empty barrier; slot < 0: none.
+__device__ __forceinline__ void release_slot(uint32_t bar_empty, int slot, bool leader) {
+  mbar_arrive_if(bar_empty + 8u * (uint32_t)(slot & (kSlots - 1)), leader && slot >= 0);
+}
+
+// ------------------------------------------------------------------------------------------------
+// MMA issue.  PTX spells out the accumulator registers, so N is a template argument, and ptxas keeps wgmmas in flight
+// only where N and the accumulator array are fixed and nothing between a wgmma and the wait that retires it is a call
+// or a divergent branch.  So the issue code is dispatched on N once per half of a step (mma_half_n), and within it
+// every slot is one straight-line run of wgmmas.
+// ------------------------------------------------------------------------------------------------
+// Ring position of the consumer warpgroup: gs = slots consumed so far, prev = the slot whose MMAs are still in flight.
+struct RingPos {
+  uint32_t gs;
+  int prev;
+};
+
+// KN K16 steps of D (+)= A * B^T, each PASSES products in the order hi*hi, lo*hi, hi*lo (acc = 0: the first product
+// overwrites D), as one committed group.
+template <int N, int PASSES, int FMT, int KN>
+__device__ __forceinline__ void mma_issue(float (&d)[64], uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
+                                          uint32_t acc) {
+  constexpr uint32_t a_inc16 = (2u * kOpKCoreBytes) >> 4, b_inc16 = (2u * N * 16u) >> 4;   // 16-byte units
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < KN; ++ks) {
+    const uint64_t ao = (uint64_t)(ks * a_inc16), bo = (uint64_t)(ks * b_inc16);
+    Wgmma<N, FMT>::run(d, a_hi + ao, b_hi + bo, ks == 0 ? acc : 1u);
+    if (PASSES == 3) {
+      Wgmma<N, FMT>::run(d, a_lo + ao, b_hi + bo, 1u);
+      Wgmma<N, FMT>::run(d, a_hi + ao, b_lo + bo, 1u);
+    }
+  }
+  wgmma_commit();
+}
+
+// Slot j of stage sd into the accumulator d: wait for it to land, issue its kn (<= KMAX) K16 steps and release the
+// previous slot once they are issued (wait_group 1: the previous slot's MMAs are done).
+template <int N, int PASSES, int FMT>
+__device__ __forceinline__ void mma_slot(float (&d)[64], const StageDesc& sd, int j, uint32_t acc, uint32_t ring_s,
+                                         uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
+                                         uint32_t op_s, RingPos& rp, bool leader) {
+  constexpr int KMAX = PASSES == 3 ? 2 : 4;   // half of a stage's 64 (x3) or 128 (1-pass) K
+  constexpr uint32_t a_inc16 = (2u * kOpKCoreBytes) >> 4;
+  uint32_t a_hi, a_lo;
+  if (sd.a_kind == A_EMB) {
+    a_hi = emb_s; a_lo = emb_s + kEmbPartBytes;
+  } else if (sd.a_kind == A_DIR) {
+    a_hi = dir_s; a_lo = dir_s + kDirPartBytes;
+  } else {
+    a_hi = op_s + (uint32_t)((sd.a_off - kColOpBase) / 4) * kOpKCoreBytes;
+    a_lo = op_s + (uint32_t)((sd.a_lo_off - kColOpBase) / 4) * kOpKCoreBytes;
+  }
+  int k0, kn;
+  slot_ksteps(sd, j, k0, kn);
+  const uint32_t slot = rp.gs % kSlots, ph = (rp.gs / kSlots) & 1;
+  const uint32_t b = ring_s + slot * (uint32_t)kSlotBytes;
+  const uint64_t ad_hi = make_smem_desc_noswz(a_hi, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
+  const uint64_t ad_lo = make_smem_desc_noswz(a_lo, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
+  const uint64_t b_hi = make_smem_desc_noswz(b, N * 16u, 128);
+  const uint64_t b_lo = make_smem_desc_noswz(b + (uint32_t)kn * N * 32u, N * 16u, 128);
+  mbar_wait(bar_full + 8 * slot, ph);
+  // one straight-line branch per K-step count, fence to commit: no join between the wgmmas and their commit
+  if (kn == 1) mma_issue<N, PASSES, FMT, 1>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
+  else if (KMAX == 2 || kn == 2) mma_issue<N, PASSES, FMT, 2>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
+  else if (kn == 3) mma_issue<N, PASSES, FMT, (KMAX < 3 ? KMAX : 3)>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
+  else mma_issue<N, PASSES, FMT, KMAX>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
+  wgmma_wait<1>();
+  release_slot(bar_empty, rp.prev, leader);
+  rp.prev = (int)slot;
+  ++rp.gs;
+}
+
+// The stages [si, si_end) of one half of a step (all of width N) into d.
+template <int N, int PASSES, int FMT>
+__device__ __forceinline__ void mma_half(float (&d)[64], const MlpProgram& prog, int si, int si_end, uint32_t ring_s,
+                                         uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
+                                         uint32_t op_s, RingPos& rp, bool leader) {
+#pragma unroll 1
+  for (; si < si_end; ++si) {
+    const StageDesc& sd = prog.st[si];
+    const uint32_t acc = (sd.flags & F_FIRST) ? 0u : 1u;
+#pragma unroll 1
+    for (int j = 0; j < stage_slots(sd); ++j)
+      mma_slot<N, PASSES, FMT>(d, sd, j, j == 0 ? acc : 1u, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+  }
+  // retire the half here: no wgmma may be in flight where the N-dispatch merges (the compiler may move accumulators)
+  wgmma_wait<0>();
+  release_slot(bar_empty, rp.prev, leader);
+  rp.prev = -1;
+}
+
 template <int PASSES, int FMT>
-__device__ __forceinline__ void mma_stage(float (&d)[64], int n, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi, uint64_t b_lo,
-                                          int ksteps, uint32_t a_inc16, uint32_t b_inc16, uint32_t acc) {
+__device__ __forceinline__ void mma_half_n(float (&d)[64], int n, const MlpProgram& prog, int si, int si_end, uint32_t ring_s,
+                                           uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
+                                           uint32_t op_s, RingPos& rp, bool leader) {
 #define PNR_MMA_N(NN) \
-  case NN / 8: mma_run<NN, PASSES, FMT>(d, a_hi, a_lo, b_hi, b_lo, ksteps, a_inc16, b_inc16, acc); break;
+  case NN / 8: mma_half<NN, PASSES, FMT>(d, prog, si, si_end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader); break;
   switch (n >> 3) {
     PNR_MMA_N(8) PNR_MMA_N(16) PNR_MMA_N(24) PNR_MMA_N(32) PNR_MMA_N(40) PNR_MMA_N(48) PNR_MMA_N(56) PNR_MMA_N(64)
     PNR_MMA_N(72) PNR_MMA_N(80) PNR_MMA_N(88) PNR_MMA_N(96) PNR_MMA_N(104) PNR_MMA_N(112) PNR_MMA_N(120) PNR_MMA_N(128)
@@ -361,14 +469,15 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
   const float* consts = p.consts;   // (read through L1: a few KB, the same words for every tile)
   float* part = reinterpret_cast<float*>(smem + kSmemPart);   // [2 column shares][kRows][4]: partial sigma / rgb sums
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSmemBars);
-  const uint32_t bar_full = smem_u32(&bars[0]);         // [kRing] weight stage landed
-  const uint32_t bar_empty = smem_u32(&bars[kRing]);    // [kRing] its MMAs retired (one arrival per consumer warp)
-  uint32_t* absmax = reinterpret_cast<uint32_t*>(bars + 2 * kRing);   // BWD: [kMaxSteps] this CTA's stash maxima
-  static_assert(2 * kRing * 8 + kMaxSteps * 4 <= 256, "barrier area");
+  const uint32_t bar_full = smem_u32(&bars[0]);          // [kSlots] weight slot landed
+  const uint32_t bar_empty = smem_u32(&bars[kSlots]);    // [kSlots] its MMAs retired (one arrival per consumer warp)
+  uint32_t* absmax = reinterpret_cast<uint32_t*>(bars + 2 * kSlots);   // BWD: [kMaxSteps] this CTA's stash maxima
+  static_assert(2 * kSlots * 8 + kMaxSteps * 4 <= 256, "barrier area");
+  const uint32_t ring_s = smem_u32(smem + kSmemRing);
 
   if (BWD) for (int i = threadIdx.x; i < kMaxSteps; i += blockDim.x) absmax[i] = 0u;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kRing; ++s) {
+    for (int s = 0; s < kSlots; ++s) {
       mbar_init(bar_full + 8 * s, 1);
       mbar_init(bar_empty + 8 * s, kConsumerThreads / 32);
     }
@@ -380,14 +489,25 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
   if (warp == kConsumerThreads / 32) {
     // =============================================================== weight stream (one elected thread)
     if (elect_one()) {
-      uint32_t gs = 0;  // global stage counter
+      uint32_t gs = 0;  // global slot counter
       for (int it = 0; it < n_iter; ++it) {
-        for (int si = 0; si < n_stages; ++si, ++gs) {
-          const uint32_t slot = gs % kRing, ph = (gs / kRing) & 1;
-          const uint32_t bytes = prog.st[si].bytes;
-          mbar_wait_backoff(bar_empty + 8 * slot, ph ^ 1);
-          mbar_arrive_expect_tx(bar_full + 8 * slot, bytes);
-          bulk_g2s(smem_u32(smem + kSmemRing + slot * kStageBytes), p.wpacked + prog.st[si].gofs, bytes, bar_full + 8 * slot);
+        for (int si = 0; si < n_stages; ++si) {
+          const StageDesc& sd = prog.st[si];
+          const uint32_t step_bytes = (uint32_t)sd.n * 32u;   // one K16 step of one image
+          const int nslots = stage_slots(sd);
+          for (int j = 0; j < nslots; ++j, ++gs) {
+            int k0, kn;
+            slot_ksteps(sd, j, k0, kn);
+            const uint32_t slot = gs % kSlots, ph = (gs / kSlots) & 1;
+            const uint32_t part = (uint32_t)kn * step_bytes;   // bytes of one image in this slot
+            const uint32_t dst = ring_s + slot * (uint32_t)kSlotBytes, bar = bar_full + 8 * slot;
+            const uint8_t* hi = p.wpacked + sd.gofs + (uint32_t)k0 * step_bytes;
+            const uint8_t* lo = p.wpacked + sd.gofs + (uint32_t)sd.lo_off16 * 16u + (uint32_t)k0 * step_bytes;
+            mbar_wait_backoff(bar_empty + 8 * slot, ph ^ 1);
+            mbar_arrive_expect_tx(bar, PASSES == 3 ? 2 * part : part);
+            bulk_g2s(dst, hi, part, bar);
+            if (PASSES == 3) bulk_g2s(dst + part, lo, part, bar);
+          }
         }
       }
     }
@@ -398,9 +518,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
     uint8_t* op = smem + kSmemOp;
     float* stg = reinterpret_cast<float*>(smem + kSmemStage);
     const uint32_t op_s = smem_u32(op), emb_s = smem_u32(smem + kSmemEmb), dir_s = smem_u32(smem + kSmemDir);
-    const uint32_t ring_s = smem_u32(smem + kSmemRing);
-    uint32_t gs = 0;
-    uint32_t vmax = 0;                          // largest hi-part bit patterns this thread produced (16x2)
+    RingPos rp{0u, -1};
+    uint32_t vmax = 0;                         // largest hi-part bit patterns this thread produced (16x2)
     float acc0[64], acc1[64];                   // the step's two N-halves
     // compositing state (COMP): see mlp_program.h for the shared-memory map
     float* w_row = reinterpret_cast<float*>(smem + kSmemCompW);
@@ -418,6 +537,23 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       const int64_t s = s_base + row;
       const int64_t s_end = cta_end();
       const bool valid = s < s_end;
+#ifdef PNR_ABL_STREAM_ONLY
+      constexpr bool kStreamOnly = true;    // ablation (timing only, garbage outputs): the weight stream alone
+#else
+      constexpr bool kStreamOnly = false;
+#endif
+      if (kStreamOnly || s_base >= s_end) {
+        // no sample of this CTA in the tile: take the weight slots, compute nothing
+#pragma unroll 1
+        for (int si = 0; si < n_stages; ++si) {
+#pragma unroll 1
+          for (int j = 0; j < stage_slots(prog.st[si]); ++j, ++rp.gs) {
+            mbar_wait(bar_full + 8 * (rp.gs % kSlots), (rp.gs / kSlots) & 1);
+            release_slot(bar_empty, (int)(rp.gs % kSlots), lane == 0);
+          }
+        }
+        continue;
+      }
       const int par = it & 1;
       float* qsum_q = qsum + (par * kQuarters + q) * kCompChPad;     // this quarter's partial sums of this tile
       float w_mine = 0.f;                                            // this row's compositing weight (COMP)
@@ -464,43 +600,24 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       int si = 0;
       for (int st = 0; st < n_steps; ++st) {
         const EpiDesc ed = prog.ep[st];
-        // ---- the step's MMAs: its stages, up to the one that closes it; a ring slot is released when the MMAs
-        // that read it have retired (wait_group 1 after the next stage's MMAs are issued)
-        int prev_slot = -1;
+        // ---- the step's MMAs: its stages up to the one that closes it, those of the first half (accumulator column
+        // ed.acc_col) into acc0, the rest into acc1; a ring slot is released when the MMAs that read it have retired
+        int h1 = si, end = si;
         for (;;) {
-          const StageDesc& sd = prog.st[si];
-          const uint32_t flags = sd.flags;
-          const uint32_t slot = gs % kRing, ph = (gs / kRing) & 1;
-          const int n = sd.n;
-          const uint32_t b = ring_s + slot * (uint32_t)kStageBytes;
-          const uint64_t b_hi = make_smem_desc_noswz(b, (uint32_t)n * 16u, 128);
-          const uint64_t b_lo = make_smem_desc_noswz(b + (uint32_t)sd.lo_off16 * 16u, (uint32_t)n * 16u, 128);
-          uint32_t a_hi, a_lo;
-          if (sd.a_kind == A_EMB) {
-            a_hi = emb_s; a_lo = emb_s + kEmbPartBytes;
-          } else if (sd.a_kind == A_DIR) {
-            a_hi = dir_s; a_lo = dir_s + kDirPartBytes;
-          } else {
-            a_hi = op_s + (uint32_t)((sd.a_off - kColOpBase) / 4) * kOpKCoreBytes;
-            a_lo = op_s + (uint32_t)((sd.a_lo_off - kColOpBase) / 4) * kOpKCoreBytes;
-          }
-          const uint64_t ad_hi = make_smem_desc_noswz(a_hi, kOpKCoreBytes, 128), ad_lo = make_smem_desc_noswz(a_lo, kOpKCoreBytes, 128);
-          const uint32_t a_inc16 = (2u * kOpKCoreBytes) >> 4, b_inc16 = (2u * (uint32_t)n * 16u) >> 4;
-          const uint32_t acc = (flags & F_FIRST) ? 0u : 1u;
-          mbar_wait(bar_full + 8 * slot, ph);
-          wgmma_fence();
-          if (sd.acc_col == ed.acc_col) mma_stage<PASSES, FMT>(acc0, n, ad_hi, ad_lo, b_hi, b_lo, sd.ksteps, a_inc16, b_inc16, acc);
-          else mma_stage<PASSES, FMT>(acc1, n, ad_hi, ad_lo, b_hi, b_lo, sd.ksteps, a_inc16, b_inc16, acc);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (prev_slot >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev_slot);
-          prev_slot = (int)slot;
-          ++gs;
-          ++si;
+          const uint32_t flags = prog.st[end].flags;
+          if (prog.st[end].acc_col == ed.acc_col) h1 = end + 1;
+          ++end;
           if (flags & (F_COMMIT_ACC1 | F_COMMIT_VIEW)) break;
         }
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(bar_empty + 8 * prev_slot);
+        // each half's first stage (F_FIRST) overwrites its accumulator, so the old values are dead: clearing them
+        // (before any of the step's wgmmas) says so to the compiler, which can then use those registers between
+        // steps without moving live accumulators - a move in a divergent path would serialize every wgmma
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
+        mma_half_n<PASSES, FMT>(acc0, prog.st[si].n, prog, si, h1, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
+        if (h1 < end)
+          mma_half_n<PASSES, FMT>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
+        si = end;
 
         // ---- epilogue: accumulator columns [0, n0) are in acc0, [n0, n) in acc1
         const float* bias = consts + ed.bias_off;

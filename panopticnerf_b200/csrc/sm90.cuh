@@ -54,31 +54,33 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// The MMA-issuing warps wait here while earlier wgmmas are in flight: no call (printf) in the loop, or ptxas
+// serializes every wgmma of the kernel.  The watchdog traps without a message.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
-  long long t0 = clock64();
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 0x3FFu) == 0 && (clock64() - t0) > PNR_WATCHDOG_CYCLES) {
-      printf("pnr: mbarrier watchdog: block %d thread %d bar 0x%x parity %u\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
-  }
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > PNR_WATCHDOG_CYCLES) __trap();
 }
-// Same, for warps whose waits are long (the weight-stream warp): back off between polls so the spinning warp
-// does not take issue slots from the MMA-issuing warpgroup that shares its scheduler.
+// One arrival on `bar` if `pred` (a predicated instruction, not a branch: safe next to in-flight wgmmas).
+__device__ __forceinline__ void mbar_arrive_if(uint32_t bar, bool pred) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %1, 0;\n\t"
+      "@p mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(bar),
+      "r"((uint32_t)pred)
+      : "memory");
+}
+// mbar_wait for warps whose waits are long (the weight-stream warp): back off between polls so the spinning warp
+// does not take issue slots from the MMA-issuing warpgroup that shares its scheduler.  No printf either: ptxas
+// serializes the wgmmas of a kernel that contains a call, on whichever warp it runs.
 __device__ __forceinline__ void mbar_wait_backoff(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
-  long long t0 = clock64();
+  const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     __nanosleep(40);
-    if ((++spins & 0x3FFu) == 0 && (clock64() - t0) > PNR_WATCHDOG_CYCLES) {
-      printf("pnr: mbarrier watchdog: block %d thread %d bar 0x%x parity %u\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if ((++spins & 0x3FFu) == 0 && (clock64() - t0) > PNR_WATCHDOG_CYCLES) __trap();
   }
 }
 
