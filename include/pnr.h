@@ -51,7 +51,16 @@ typedef struct pnr_config {
   int32_t num_instances; /* K instance logits, 0 = no head            a8 */
   int32_t precision;     /* PNR_PREC_*                                   */
   int32_t device;        /* CUDA ordinal                                 */
+  /* Trunk input (8(f) rank 4).  An all-zero tail is the frequency network above.  PNR_XYZ_HASHGRID: the trunk input
+   * is h(x), the hash-grid features of the sample point (pnr_hashgrid_encode with these arguments and the table bound
+   * by pnr_bind_hashgrid_table), E = hash_levels * hash_features <= 64 columns in place of gamma(x) in layer 0 and in
+   * the skip concatenation; xyz_res is ignored.  The view branch keeps gamma(d).  hash_aabb = {lo.xyz, hi.xyz}. */
+  int32_t xyz_encoding;  /* PNR_XYZ_*                                    */
+  int32_t hash_levels, hash_features, hash_log2_size;
+  float hash_base_resolution, hash_per_level_scale;
+  float hash_aabb[6];
 } pnr_config;
+enum { PNR_XYZ_FREQUENCY = 0, PNR_XYZ_HASHGRID = 1 };
 
 int pnr_version(void);
 const char* pnr_last_error(void);
@@ -67,11 +76,20 @@ int pnr_destroy(pnr_ctx* ctx);
 #define PNR_STATUS_RANGE 1u
 int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, void* stream);
 
+/* Hash-grid contexts (cfg.xyz_encoding = PNR_XYZ_HASHGRID): the table [hash_levels, 2^hash_log2_size, hash_features]
+ * fp32, a caller-owned DEVICE pointer.  It is not copied: every fused-MLP launch of the context (pnr_mlp_forward,
+ * pnr_mlp_composite, pnr_mlp_trunk_forward, pnr_mlp_backward_trunk, pnr_render_fused) reads it when it executes, so an
+ * in-place update on the same stream is seen by the next launch.  Those entry points return PNR_ERR_STATE on a
+ * hash-grid context without a table; NULL unbinds.  PNR_ERR_STATE on a frequency context. */
+int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
+
 /* a2: load a Network state_dict.  `tensors_host[i]` are HOST fp32 pointers in this fixed order:
  *   pts_linears.{0..D-1}.weight/.bias (interleaved w,b), alpha_linear.w/.b, feature_linear.w/.b,
  *   views_linears.0.w/.b, rgb_linear.w/.b, [semantic_linears.0.w/.b, semantic_linears.1.w/.b],
  *   [instance_linears.0.w/.b, instance_linears.1.w/.b]
- * `shapes[2*i], shapes[2*i+1]` = (out, in) for weights, (out, 1) for biases.  Weights are split
+ * `shapes[2*i], shapes[2*i+1]` = (out, in) for weights, (out, 1) for biases.  The trunk input width (layer 0's `in`,
+ * the skip layer's first columns) is 3 + 6*xyz_res, or E = hash_levels * hash_features for a hash-grid context (whose
+ * table is not in this list: pnr_bind_hashgrid_table).  Weights are split
  * into 16-bit hi/lo parts of the context's operand format (fp16 or bf16, cfg.precision), laid out as
  * no-swizzle K-major UMMA stage images and uploaded.  In the fp16 modes a weight with |w| > 65504 is
  * rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode. */
@@ -251,8 +269,9 @@ int pnr_composite_backward(const float* raw, const float* z, const float* rays, 
                            int32_t B, const pnr_composite_grads* g, float* d_raw, void* stream);
 
 /* a8 backward, first slice (SURVEY 8(f) rank 2; replaces autograd through Network.forward's trunk - the D
- * `pts_linears` with their ReLUs and the skip concatenation): dL/d(embedded xyz) (the first 3 + 6*xyz_res columns
- * of grad_emb [R*N, ld_emb]; ld_emb = 64 on a 16-byte aligned base lets the kernel use 16-byte stores) from
+ * `pts_linears` with their ReLUs and the skip concatenation): dL/d(trunk input) (the first 3 + 6*xyz_res columns
+ * of grad_emb [R*N, ld_emb], or E = hash_levels * hash_features columns = dL/dh(x) for a hash-grid context; ld_emb =
+ * that width rounded up to 16 on a 16-byte aligned base lets the kernel use 16-byte stores) from
  * grad_h = dL/dh of the trunk output [R*N, W].  One kernel on the same 128-sample tiles as pnr_mlp_forward: the
  * forward trunk is recomputed (ReLU sign patterns stay in shared memory), then the layers run in reverse with the
  * transposed weight stream on the tensor cores, gradients split hi/lo like activations.  Samples are given as pts

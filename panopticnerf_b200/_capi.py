@@ -24,9 +24,15 @@ class PnrError(RuntimeError):
 
 
 class PnrConfig(C.Structure):
+    """pnr_config of include/pnr.h.  Fields left out of a positional call stay zero: the frequency network."""
     _fields_ = [("D", C.c_int32), ("W", C.c_int32), ("xyz_res", C.c_int32), ("view_res", C.c_int32),
                 ("num_classes", C.c_int32), ("num_instances", C.c_int32), ("precision", C.c_int32),
-                ("device", C.c_int32)]
+                ("device", C.c_int32), ("xyz_encoding", C.c_int32), ("hash_levels", C.c_int32),
+                ("hash_features", C.c_int32), ("hash_log2_size", C.c_int32), ("hash_base_resolution", C.c_float),
+                ("hash_per_level_scale", C.c_float), ("hash_aabb", C.c_float * 6)]
+
+
+XYZ_ENCODING = {"frequency": 0, "hashgrid": 1}
 
 
 class PnrCompositeOut(C.Structure):
@@ -77,6 +83,7 @@ SIGNATURES = {
     "pnr_create": (C.c_int, [C.POINTER(PnrConfig), C.POINTER(_vp)]),
     "pnr_destroy": (C.c_int, [_vp]),
     "pnr_status": (C.c_int, [_vp, C.POINTER(C.c_uint32), _i32, _vp]),
+    "pnr_bind_hashgrid_table": (C.c_int, [_vp, _vp]),
     "pnr_load_weights": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32]),
     "pnr_intersect": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "pnr_scene_near_far": (C.c_int, [_vp, _i64, C.POINTER(_f32), _f32, _f32, _vp, _vp, _vp]),

@@ -16,6 +16,11 @@ _DEFAULTS = dict(
     renderer_module="panopticnerf_b200.lib.networks.renderer.panopticnerf_renderer",
     # MLP (SURVEY 8a a8)
     D=8, W=256, xyz_res=10, view_res=4, num_classes=0, num_instances=0,
+    # trunk input: "frequency" = gamma(x) (the network above) | "hashgrid" = h(x), the multi-resolution hash-grid features
+    # of the point (E = hash_levels * hash_features <= 64 columns in place of gamma(x); rule chosen here, the reference's
+    # 360 architecture is not in the mount).  hash_aabb [lo.xyz, hi.xyz] is required with "hashgrid".
+    xyz_encoding="frequency", hash_levels=16, hash_features=2, hash_log2_size=19,
+    hash_base_resolution=16.0, hash_per_level_scale=1.3819, hash_aabb=None,
     # sampling / rendering (a5, a6, a9, a10)
     N_samples=64, N_importance=0, perturb=0.0, white_bkgd=False, raw_noise_std=0.0,
     near=0.05, far=80.0, max_hits=4, bound_by_primitives=False, mask_outside=False,

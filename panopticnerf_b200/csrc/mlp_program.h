@@ -146,7 +146,7 @@ struct EpiDesc {
 struct MlpProgram {
   int32_t n_stages, n_steps, n_consts;
   int32_t sigma_bias_off, rgb_bias_off;   // float offsets into consts
-  int32_t Lx, Ld;
+  int32_t Lx, Ld;                          // octaves of gamma(x) (0 for a hash-grid trunk input) and gamma(d)
   int32_t passes;                          // 1 or 3
   int32_t acc_flip;                        // 1: odd tiles use the accumulator columns XOR 128 (see below)
   int32_t view_step;                       // >= 0: this (last) step's epilogue runs on the producer warps (see below)
@@ -197,6 +197,13 @@ struct MlpParams {
   // stash slot k, as the bit pattern of its 16-bit hi part in the operand format and BEFORE grad_unscale is applied -
   // what the caller needs to pick the power-of-two scale of the weight-gradient GEMM without another pass over the stash
   uint32_t* stash_absmax;
+  // ---- hash-grid trunk input (pnr_config.xyz_encoding = PNR_XYZ_HASHGRID): hash_table != null makes the prologue write
+  // h(x) (hashgrid_math.cuh) instead of gamma(x) into the embedding operand; its E = hash_L * hash_F columns are padded
+  // with zeros to the program's K (a multiple of 16)
+  const float* hash_table;     // [hash_L, 2^hash_T_log2, hash_F] fp32, read as the launch executes
+  int32_t hash_L, hash_F, hash_T_log2;
+  float hash_aabb[6];          // {lo.xyz, hi.xyz}
+  uint32_t hash_res[32];       // per-level resolutions (hash_level_resolutions)
 };
 
 // What a launch carries: arguments + the context's program, as ONE __grid_constant__ kernel parameter.

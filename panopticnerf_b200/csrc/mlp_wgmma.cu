@@ -4,7 +4,8 @@
 // runs on-chip:
 //   * the consumer warpgroup (128 threads) forms pts = o + d*z and the positional encodings gamma(x) (threads 0-63,
 //     one row each) and gamma(d) (threads 64-127), splits them into 16-bit hi/lo parts and writes them into shared
-//     memory in the no-swizzle K-major operand layout;
+//     memory in the no-swizzle K-major operand layout (a hash-grid network: h(x) gathered from its table in place of
+//     gamma(x), hashgrid_math.cuh);
 //   * one weight-stream warp copies the pre-packed weight stages (<= 32 KB: hi image then lo image of an N-row x 64-K
 //     tile) from L2 into a 4-slot shared-memory ring, one K-half of a stage per 16 KB slot, with cp.async.bulk +
 //     mbarrier complete_tx;
@@ -30,6 +31,7 @@
 #include <mutex>
 #include "common.cuh"
 #include "composite_math.cuh"
+#include "hashgrid_math.cuh"
 #include "mlp_program.h"
 #include "sm90.cuh"
 
@@ -75,6 +77,54 @@ __device__ __forceinline__ void encode_row(const float (&p)[3], int L, uint8_t* 
 #pragma unroll
     for (int j = 0; j < 8; ++j) w8[j] = v[g * 8 + j];
     store_core_row<PASSES, FMT>(hi_base, lo_base, g, row, w8);
+  }
+}
+
+// h(x) of one row (hash-grid trunk input): core rows [g0, g1) of the embedding operand, each = 8 features = 8 / F whole
+// levels (hash_level_blend, the arithmetic of pnr_hashgrid_encode), features past L*F = the zero padding; split hi/lo
+// like gamma(x).  The features carry a sign: `vmax` collects the magnitudes of the hi parts (range check).
+template <int PASSES, int FMT, int F>
+__device__ __forceinline__ void hash_rows(const MlpParams& p, const float (&v)[3], int g0, int g1, uint8_t* hi_base,
+                                          uint8_t* lo_base, int row, uint32_t& vmax) {
+  constexpr int kLevelsPerCore = 8 / F;
+  const size_t level_floats = (size_t)F << p.hash_T_log2;
+#pragma unroll 1
+  for (int g = g0; g < g1; ++g) {
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+    // one level at a time (a rolled loop keeps this rarely taken branch small next to the MMA code)
+#pragma unroll 1
+    for (int ll = 0; ll < kLevelsPerCore; ++ll) {
+      const int l = g * kLevelsPerCore + ll;
+      if (l >= p.hash_L) break;
+      float f[F];
+#pragma unroll
+      for (int j = 0; j < F; ++j) f[j] = 0.f;
+      hash_level_blend<F>(p.hash_table + (size_t)l * level_floats, v, p.hash_res[l], (uint32_t)p.hash_T_log2, f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (j / F == ll) acc[j] = f[j % F];
+    }
+    uint32_t h[4], lo[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) split_x2<FMT>(acc[2 * j], acc[2 * j + 1], h[j], lo[j]);
+    const int off = (g * kRows + row) * 16;
+    *reinterpret_cast<uint4*>(hi_base + off) = make_uint4(h[0], h[1], h[2], h[3]);
+    if (PASSES == 3) *reinterpret_cast<uint4*>(lo_base + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    vmax = __vimax3_u16x2(vmax, h[0] & 0x7FFF7FFFu, h[1] & 0x7FFF7FFFu);
+    vmax = __vimax3_u16x2(vmax, h[2] & 0x7FFF7FFFu, h[3] & 0x7FFF7FFFu);
+  }
+}
+
+template <int PASSES, int FMT>
+__device__ __forceinline__ void hash_rows_f(const MlpParams& p, const float (&v)[3], int g0, int g1, uint8_t* hi_base,
+                                            uint8_t* lo_base, int row, uint32_t& vmax) {
+  switch (p.hash_F) {
+    case 1: hash_rows<PASSES, FMT, 1>(p, v, g0, g1, hi_base, lo_base, row, vmax); break;
+    case 2: hash_rows<PASSES, FMT, 2>(p, v, g0, g1, hi_base, lo_base, row, vmax); break;
+    case 4: hash_rows<PASSES, FMT, 4>(p, v, g0, g1, hi_base, lo_base, row, vmax); break;
+    default: hash_rows<PASSES, FMT, 8>(p, v, g0, g1, hi_base, lo_base, row, vmax); break;
   }
 }
 
@@ -559,12 +609,15 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       float w_mine = 0.f;                                            // this row's compositing weight (COMP)
       float sig = 0.f;
 
-      // ---- embeddings of this tile: threads 0-63 gamma(x) of row t, threads 64-127 gamma(d) of row t - 64
+      // ---- embeddings of this tile: threads 0-63 gamma(x) of row t, threads 64-127 gamma(d) of row t - 64.  A hash-grid
+      // trunk input (p.hash_table set) replaces gamma(x) by h(x): both threads of a row form its point, the xyz thread
+      // gathers the first half of the feature core rows, the dir thread (after gamma(d), if any) the second half.
       named_bar_sync(1, kConsumerThreads);    // the previous tile's end-of-tile reads are done
       {
         const int erow = threadIdx.x & (kRows - 1);
         const bool dir_thread = threadIdx.x >= kRows;
-        if (!(BWD && dir_thread)) {
+        const bool hashgrid = p.hash_table != nullptr;
+        if (!(BWD && dir_thread) || hashgrid) {
           int64_t se = s_base + erow;
           if (se >= p.S) se = p.S - 1;  // clamp: tail rows compute on a valid sample, results are discarded
           float x[3], d[3];
@@ -587,10 +640,17 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
 #pragma unroll
             for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(d[c], nrm);
           }
-          if (!dir_thread) {
+          if (dir_thread) {
+            if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow);
+          } else if (!hashgrid) {
             encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow);
-          } else {
-            encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow);
+          }
+          if (hashgrid) {
+            float v[3];
+            hash_normalize(x, p.hash_aabb, v);
+            const int nc = ((p.hash_L * p.hash_F + 15) & ~15) / 8, half = (nc + 1) / 2;   // core rows the MMAs read
+            hash_rows_f<PASSES, FMT>(p, v, dir_thread ? half : 0, dir_thread ? nc : half, smem + kSmemEmb,
+                                     smem + kSmemEmb + kEmbPartBytes, erow, vmax);
           }
         }
         fence_proxy_async_smem();   // generic-proxy stores -> visible to the MMAs' async proxy

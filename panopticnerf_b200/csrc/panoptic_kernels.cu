@@ -8,6 +8,7 @@
 #include <stdint.h>
 #include "../../include/pnr.h"
 #include "common.cuh"
+#include "hashgrid_math.cuh"
 
 namespace pnr {
 namespace {
@@ -85,13 +86,8 @@ struct HashArgs {
   const float* x; int64_t n; const float* table; float* out;
   const float* aabb;   // device {lo.xyz, hi.xyz} or null (x already in [0,1]^3)
   int L, F, T_log2;
-  uint32_t res[32];    // resolution of every level, floor(base * scale^l) evaluated in double on the host
+  uint32_t res[kHashMaxLevels];   // resolution of every level (hash_level_resolutions)
 };
-
-__device__ __forceinline__ uint32_t hash_index(uint32_t x, uint32_t y, uint32_t z, uint32_t res1, bool dense, uint32_t mask) {
-  if (dense) return x + y * res1 + z * res1 * res1;
-  return (x ^ (y * 2654435761u) ^ (z * 805459861u)) & mask;
-}
 
 // One thread = one point x LPT consecutive levels with LPT * F = 8 features: its output is one whole 32-byte sector
 // (a thread per (point, level) writes 8 bytes into every 128-byte row - four partial writes per sector from four
@@ -103,14 +99,10 @@ __global__ void __launch_bounds__(256) hashgrid_kernel(HashArgs a) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int l0 = blockIdx.y * LPT;
   if (i >= a.n) return;
-  const uint32_t T = 1u << a.T_log2, mask = T - 1u;
+  const uint32_t T = 1u << a.T_log2;
   float v[3];
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    float t = a.x[i * 3 + d];
-    if (a.aabb) t = __fdiv_rn(__fsub_rn(t, a.aabb[d]), __fsub_rn(a.aabb[3 + d], a.aabb[d]));
-    v[d] = fminf(fmaxf(t, 0.0f), 1.0f);                  // outside points take the border cell
-  }
+  const float x[3] = {a.x[i * 3], a.x[i * 3 + 1], a.x[i * 3 + 2]};
+  hash_normalize(x, a.aabb, v);
   float acc[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
@@ -118,44 +110,7 @@ __global__ void __launch_bounds__(256) hashgrid_kernel(HashArgs a) {
   for (int ll = 0; ll < LPT; ++ll) {
     const int l = l0 + ll;
     if (l >= a.L) break;
-    const uint32_t res = a.res[l], res1 = res + 1u;
-    const float res_f = (float)res;
-    const bool dense = (uint64_t)res1 * res1 * res1 <= (uint64_t)T;
-    float w[3];
-    uint32_t c[3];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-      const float p = __fmul_rn(v[d], res_f);
-      float fl = floorf(p);
-      if (fl >= res_f) fl = res_f - 1.0f;                // v == 1 belongs to the last cell (weight 1 on its far corner)
-      c[d] = (uint32_t)fl;
-      w[d] = __fsub_rn(p, fl);
-    }
-    const float* tab = a.table + (size_t)l * T * F;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {   // corner order: x fastest; the sum runs in this order (fixed for the oracle)
-      const uint32_t dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
-      const float wx = dx ? w[0] : __fsub_rn(1.0f, w[0]);
-      const float wy = dy ? w[1] : __fsub_rn(1.0f, w[1]);
-      const float wz = dz ? w[2] : __fsub_rn(1.0f, w[2]);
-      const float wk = __fmul_rn(__fmul_rn(wx, wy), wz);
-      const uint32_t idx = hash_index(c[0] + dx, c[1] + dy, c[2] + dz, res1, dense, mask);
-      if (F == 2) {
-        const float2 t = __ldg(reinterpret_cast<const float2*>(tab) + idx);
-        acc[ll * 2] = __fadd_rn(acc[ll * 2], __fmul_rn(wk, t.x));
-        acc[ll * 2 + 1] = __fadd_rn(acc[ll * 2 + 1], __fmul_rn(wk, t.y));
-      } else if (F == 4) {
-        const float4 t = __ldg(reinterpret_cast<const float4*>(tab) + idx);
-        acc[ll * 4] = __fadd_rn(acc[ll * 4], __fmul_rn(wk, t.x));
-        acc[ll * 4 + 1] = __fadd_rn(acc[ll * 4 + 1], __fmul_rn(wk, t.y));
-        acc[ll * 4 + 2] = __fadd_rn(acc[ll * 4 + 2], __fmul_rn(wk, t.z));
-        acc[ll * 4 + 3] = __fadd_rn(acc[ll * 4 + 3], __fmul_rn(wk, t.w));
-      } else {
-#pragma unroll
-        for (int f = 0; f < F; ++f)
-          acc[ll * F + f] = __fadd_rn(acc[ll * F + f], __fmul_rn(wk, __ldg(tab + (size_t)idx * F + f)));
-      }
-    }
+    hash_level_blend<F>(a.table + (size_t)l * T * F, v, a.res[l], (uint32_t)a.T_log2, acc + ll * F);
   }
   const int width = a.L * F;
   float* o = a.out + i * (int64_t)width + l0 * F;
@@ -182,41 +137,25 @@ __global__ void __launch_bounds__(256) hashgrid_backward_kernel(HashArgs a, cons
   if (i >= a.n) return;
   const uint32_t T = 1u << a.T_log2, mask = T - 1u;
   float v[3];
-#pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    float t = a.x[i * 3 + d];
-    if (a.aabb) t = __fdiv_rn(__fsub_rn(t, a.aabb[d]), __fsub_rn(a.aabb[3 + d], a.aabb[d]));
-    v[d] = fminf(fmaxf(t, 0.0f), 1.0f);
-  }
+  const float x[3] = {a.x[i * 3], a.x[i * 3 + 1], a.x[i * 3 + 2]};
+  hash_normalize(x, a.aabb, v);
   const float* go = gout + i * (int64_t)(a.L * F);
 #pragma unroll
   for (int ll = 0; ll < LPT; ++ll) {
     const int l = l0 + ll;
     if (l >= a.L) break;
     const uint32_t res = a.res[l], res1 = res + 1u;
-    const float res_f = (float)res;
     const bool dense = (uint64_t)res1 * res1 * res1 <= (uint64_t)T;
     float w[3], g[F];
     uint32_t c[3];
 #pragma unroll
     for (int f = 0; f < F; ++f) g[f] = go[l * F + f];
-#pragma unroll
-    for (int d = 0; d < 3; ++d) {
-      const float p = __fmul_rn(v[d], res_f);
-      float fl = floorf(p);
-      if (fl >= res_f) fl = res_f - 1.0f;
-      c[d] = (uint32_t)fl;
-      w[d] = __fsub_rn(p, fl);
-    }
+    hash_cell(v, res, c, w);
     float* tab = gtab + (size_t)l * T * F;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const uint32_t dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
-      const float wx = dx ? w[0] : __fsub_rn(1.0f, w[0]);
-      const float wy = dy ? w[1] : __fsub_rn(1.0f, w[1]);
-      const float wz = dz ? w[2] : __fsub_rn(1.0f, w[2]);
-      const float wk = __fmul_rn(__fmul_rn(wx, wy), wz);
-      const uint32_t idx = hash_index(c[0] + dx, c[1] + dy, c[2] + dz, res1, dense, mask);
+      uint32_t idx;
+      const float wk = hash_corner(c, w, k, res1, dense, mask, idx);
       if (F == 2) {
         atomicAdd(reinterpret_cast<float2*>(tab) + idx, make_float2(wk * g[0], wk * g[1]));
       } else if (F == 4) {
@@ -258,7 +197,7 @@ extern "C" int pnr_hashgrid_encode(const float* x, int64_t n, const float* aabb,
   PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "pnr_hashgrid_encode: base_resolution / per_level_scale < 1");
   PNR_CHECK_ARG((double)base_resolution * pow((double)per_level_scale, (double)(L - 1)) < 1048576.0, "pnr_hashgrid_encode: finest resolution >= 2^20");
   HashArgs a{x, n, table, out, aabb, L, F, T_log2, {}};
-  for (int l = 0; l < L; ++l) a.res[l] = (uint32_t)floor((double)base_resolution * pow((double)per_level_scale, (double)l));
+  hash_level_resolutions(L, base_resolution, per_level_scale, a.res);
   const int lpt = 8 / F;   // levels per thread: 8 output features = one 32-byte sector
   const dim3 grid((unsigned)((n + 255) / 256), (unsigned)((L + lpt - 1) / lpt));
   switch (F) {
@@ -281,7 +220,7 @@ extern "C" int pnr_hashgrid_backward(const float* x, int64_t n, const float* aab
   PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "pnr_hashgrid_backward: base_resolution / per_level_scale < 1");
   PNR_CHECK_ARG((double)base_resolution * pow((double)per_level_scale, (double)(L - 1)) < 1048576.0, "pnr_hashgrid_backward: finest resolution >= 2^20");
   HashArgs a{x, n, nullptr, nullptr, aabb, L, F, T_log2, {}};
-  for (int l = 0; l < L; ++l) a.res[l] = (uint32_t)floor((double)base_resolution * pow((double)per_level_scale, (double)l));
+  hash_level_resolutions(L, base_resolution, per_level_scale, a.res);
   const int lpt = 8 / F;
   const dim3 grid((unsigned)((n + 255) / 256), (unsigned)((L + lpt - 1) / lpt));
   switch (F) {

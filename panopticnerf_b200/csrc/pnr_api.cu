@@ -6,6 +6,7 @@
 #include <string>
 #include <vector>
 #include "common.cuh"
+#include "hashgrid_math.cuh"
 #include "mlp_program.h"
 #include "sm90.cuh"
 
@@ -43,6 +44,8 @@ struct pnr_ctx {
   uint8_t* d_wpacked = nullptr;
   float* d_consts = nullptr;
   uint32_t* d_status = nullptr; // sticky range-check word of the fused MLP (bit 0: activation out of operand range)
+  const float* hash_table = nullptr;   // hash-grid contexts: the caller's table (pnr_bind_hashgrid_table), not owned
+  uint32_t hash_res[kHashMaxLevels] = {};
   size_t wpacked_bytes = 0;
   // backward program of the trunk (pnr_mlp_backward_trunk): built from a host copy of the trunk weights on first use
   std::vector<std::vector<float>> host_trunk;   // weight, bias per trunk layer, as given to pnr_load_weights
@@ -396,6 +399,19 @@ static int precision_fmt(int precision) {   // instruction-descriptor operand fo
   return (precision == PNR_PREC_BF16X3 || precision == PNR_PREC_BF16) ? 1 : 0;
 }
 
+static bool is_hashgrid(const pnr_config& c) { return c.xyz_encoding == PNR_XYZ_HASHGRID; }
+
+// Width of the trunk input (layer 0 and the skip layer's first columns): gamma(x) or the hash-grid features h(x)
+static int trunk_input_width(const pnr_config& c) {
+  return is_hashgrid(c) ? c.hash_levels * c.hash_features : 3 + 6 * c.xyz_res;
+}
+
+// K of the embedding operand the MMAs read: gamma(x)'s 63 columns padded to 64 (the whole region), h(x)'s E columns to
+// a multiple of 16 (zero weight columns; the prologue writes zeros there)
+static int trunk_input_kpad(const pnr_config& c) {
+  return is_hashgrid(c) ? (trunk_input_width(c) + 15) / 16 * 16 : 64;
+}
+
 static int check_config(const pnr_config* cfg) {
   PNR_CHECK_ARG(cfg->D >= 3 && cfg->D <= 16, "pnr_create: D=%d outside [3,16]", cfg->D);
   PNR_CHECK_ARG(cfg->W == 64 || cfg->W == 128 || cfg->W == 256, "pnr_create: W=%d not in {64,128,256}", cfg->W);
@@ -404,6 +420,23 @@ static int check_config(const pnr_config* cfg) {
   PNR_CHECK_ARG(cfg->num_classes >= 0 && cfg->num_classes <= 128, "pnr_create: num_classes=%d outside [0,128]", cfg->num_classes);
   PNR_CHECK_ARG(cfg->num_instances >= 0 && cfg->num_instances <= 128, "pnr_create: num_instances=%d outside [0,128]", cfg->num_instances);
   PNR_CHECK_ARG(cfg->precision >= 0 && cfg->precision <= 3, "pnr_create: bad precision %d", cfg->precision);
+  PNR_CHECK_ARG(cfg->xyz_encoding == PNR_XYZ_FREQUENCY || cfg->xyz_encoding == PNR_XYZ_HASHGRID,
+                "pnr_create: bad xyz_encoding %d", cfg->xyz_encoding);
+  if (is_hashgrid(*cfg)) {   // the checks of pnr_hashgrid_encode, and the features must fit the 64-K embedding operand
+    const int L = cfg->hash_levels, F = cfg->hash_features;
+    PNR_CHECK_ARG(L >= 1 && L <= kHashMaxLevels && (F == 1 || F == 2 || F == 4 || F == 8),
+                  "pnr_create: hash_levels=%d hash_features=%d (levels in [1,32], features in {1,2,4,8})", L, F);
+    PNR_CHECK_ARG(L * F <= 64, "pnr_create: hash-grid features E=%d > 64 (hash_levels * hash_features)", L * F);
+    PNR_CHECK_ARG(cfg->hash_log2_size >= 4 && cfg->hash_log2_size <= 28, "pnr_create: hash_log2_size=%d outside [4,28]",
+                  cfg->hash_log2_size);
+    PNR_CHECK_ARG(cfg->hash_base_resolution >= 1.0f && cfg->hash_per_level_scale >= 1.0f,
+                  "pnr_create: hash_base_resolution / hash_per_level_scale < 1");
+    PNR_CHECK_ARG((double)cfg->hash_base_resolution * pow((double)cfg->hash_per_level_scale, (double)(L - 1)) < 1048576.0,
+                  "pnr_create: hash-grid finest resolution >= 2^20");
+    for (int d = 0; d < 3; ++d)
+      PNR_CHECK_ARG(cfg->hash_aabb[3 + d] > cfg->hash_aabb[d] && cfg->hash_aabb[3 + d] - cfg->hash_aabb[d] < 3.0e38f,
+                    "pnr_create: hash_aabb axis %d: hi must exceed lo (a hash-grid network needs its aabb)", d);
+  }
   return PNR_OK;
 }
 
@@ -424,6 +457,7 @@ extern "C" int pnr_create(const pnr_config* cfg, pnr_ctx** out) {
   c->cfg = *cfg;
   c->passes = precision_passes(cfg->precision);
   c->fmt = precision_fmt(cfg->precision);
+  if (is_hashgrid(*cfg)) hash_level_resolutions(cfg->hash_levels, cfg->hash_base_resolution, cfg->hash_per_level_scale, c->hash_res);
   memset(&c->launch, 0, sizeof(c->launch));
   memset(&c->launch_vp, 0, sizeof(c->launch_vp));
   cudaError_t e = cudaMalloc(&c->d_status, sizeof(uint32_t));
@@ -472,7 +506,7 @@ extern "C" int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, vo
 static int build_program(const pnr_config& c, const float* const* t, const int64_t* shapes, int32_t n,
                          Builder& bld) {
   const int D = c.D, W = c.W, W2 = W / 2, C = c.num_classes, K = c.num_instances;
-  const int Ex = 3 + 6 * c.xyz_res, Ed = 3 + 6 * c.view_res, skip = D / 2;
+  const int Ex = trunk_input_width(c), Ekpad = trunk_input_kpad(c), Ed = 3 + 6 * c.view_res, skip = D / 2;
   const int expected = 2 * D + 8 + (C > 0 ? 4 : 0) + (K > 0 ? 4 : 0);
   PNR_CHECK_ARG(n == expected, "pnr_load_weights: got %d tensors, expected %d", n, expected);
   int ti = 0;
@@ -490,7 +524,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     return set_error(PNR_ERR_ARG, "pnr_load_weights: tensor %d: expected weight [%d,%d] + bias [%d,1]", \
                      ti, out, in, out)
 
-  bld.prog.Lx = c.xyz_res;
+  bld.prog.Lx = is_hashgrid(c) ? 0 : c.xyz_res;
   bld.prog.Ld = c.view_res;
   bld.prog.passes = bld.passes;
 
@@ -533,9 +567,9 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     ed.aux_off = (uint16_t)sig_w_off;
     std::vector<Seg> segs;
     if (i == 0) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, 64, 0, 0, false});
+      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, false});
     } else if (i == skip + 1) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, 64, 0, 0, true});
+      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, true});
       segs.push_back(seg_tmem(trunk[i], Ex, W, kColAHi, kColALo));
     } else {
       segs.push_back(seg_tmem(trunk[i], 0, W, kColAHi, kColALo));
@@ -660,7 +694,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
 // 2D-2-j (the order they are produced in: dZ_{D-1} by the last forward layer's epilogue, then D-2 .. 0).
 static int build_backward_program(const pnr_config& c, const float* const* t, const int64_t* shapes, int32_t n,
                                   Builder& bld, bool forward_only = false) {
-  const int D = c.D, W = c.W, Ex = 3 + 6 * c.xyz_res, skip = D / 2;
+  const int D = c.D, W = c.W, Ex = trunk_input_width(c), Ekpad = trunk_input_kpad(c), skip = D / 2;
   PNR_CHECK_ARG(n >= 2 * D, "backward program: got %d tensors, the trunk has %d", n, 2 * D);
   if (bld.passes != 3)
     return set_error(PNR_ERR_UNSUPPORTED, "backward program: precision must be fp16x3 or bf16x3");
@@ -675,7 +709,7 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
     trunk[i] = Mat{t[2 * i], W, in};
     trunk_b[i] = t[2 * i + 1];
   }
-  bld.prog.Lx = c.xyz_res;
+  bld.prog.Lx = is_hashgrid(c) ? 0 : c.xyz_res;
   bld.prog.Ld = c.view_res;
   bld.prog.passes = bld.passes;
   auto seg_tmem = [&](const Mat& m, int col0, int k) {
@@ -692,9 +726,9 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
     ed.bias_off = (uint16_t)bld.add_consts(trunk_b[i], W, W);
     std::vector<Seg> segs;
     if (i == 0) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, 64, 0, 0, false});
+      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, false});
     } else if (i == skip + 1) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, 64, 0, 0, true});
+      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, true});
       segs.push_back(seg_tmem(trunk[i], Ex, W));
     } else {
       segs.push_back(seg_tmem(trunk[i], 0, W));
@@ -713,8 +747,8 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
       eo.n_valid = (uint16_t)Ex;
       eo.n_valid1 = accumulate ? 1 : 0;
       eo.out_off = 0;
-      // one N = 64 half: two N = 32 halves would double the MMA count for the same tensor time per MMA
-      return bld.add_step({seg_tmem(Mat{rows, Ex, W}, 0, W)}, 64, kColAcc, eo, false, nullptr, 64);
+      // one N = Ekpad half: two N = 32 halves would double the MMA count for the same tensor time per MMA
+      return bld.add_step({seg_tmem(Mat{rows, Ex, W}, 0, W)}, Ekpad, kColAcc, eo, false, nullptr, Ekpad);
     };
     auto grad_h = [&](const float* rows) {                       // hidden columns, gated by layer l-1's sign pattern
       EpiDesc em{};
@@ -829,6 +863,27 @@ extern "C" int pnr_program_host(const pnr_config* cfg, const float* const* t, co
 static int mlp_forward_impl(pnr_ctx* ctx, const float* pts, const float* viewdirs, const float* rays,
                             const float* z, int64_t R, int32_t N, float* raw, void* stream, long long* dbg);
 
+extern "C" int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table) {
+  PNR_CHECK_ARG(ctx, "pnr_bind_hashgrid_table: null context");
+  if (!is_hashgrid(ctx->cfg)) return set_error(PNR_ERR_STATE, "pnr_bind_hashgrid_table: not a hash-grid context");
+  ctx->hash_table = table;
+  return PNR_OK;
+}
+
+// The trunk-input fields of a launch: a hash-grid context's table and level constants, or none (gamma(x)).
+static int set_trunk_input(const pnr_ctx* ctx, MlpParams& p, const char* what) {
+  p.hash_table = nullptr;
+  if (!is_hashgrid(ctx->cfg)) return PNR_OK;
+  if (ctx->hash_table == nullptr)
+    return set_error(PNR_ERR_STATE, "%s: hash-grid network without a table (pnr_bind_hashgrid_table)", what);
+  const pnr_config& c = ctx->cfg;
+  p.hash_table = ctx->hash_table;
+  p.hash_L = c.hash_levels; p.hash_F = c.hash_features; p.hash_T_log2 = c.hash_log2_size;
+  memcpy(p.hash_aabb, c.hash_aabb, sizeof(p.hash_aabb));
+  memcpy(p.hash_res, ctx->hash_res, sizeof(p.hash_res));
+  return PNR_OK;
+}
+
 extern "C" int pnr_debug_timeline(pnr_ctx* ctx, int64_t* timeline) {
   PNR_CHECK_ARG(ctx, "pnr_debug_timeline: null context");
   ctx->dbg_timeline = (long long*)timeline;
@@ -864,6 +919,7 @@ static int mlp_forward_impl(pnr_ctx* ctx, const float* pts, const float* viewdir
   p.num_tiles = (int32_t)((S + kTileM - 1) / kTileM);
   p.status = ctx->d_status;
   p.dbg = dbg;
+  if (const int rc = set_trunk_input(ctx, p, "pnr_mlp_forward")) return rc;
   DeviceGuard guard(ctx->cfg.device);   // launch on the context's device whatever the caller's current one is
   return launch_mlp(L, ctx->passes, ctx->fmt, ctx->has_vp ? kMlpForwardVP : kMlpForward, (cudaStream_t)stream);
 }
@@ -894,6 +950,7 @@ extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z
   p.C = C; p.K = K;
   p.weights = out->weights; p.rgb_map = out->rgb_map; p.depth_map = out->depth_map; p.acc_map = out->acc_map;
   p.disp_map = out->disp_map; p.sem_map = C > 0 ? out->semantic_map : nullptr; p.inst_map = K > 0 ? out->instance_map : nullptr;
+  if (const int rc = set_trunk_input(ctx, p, "pnr_mlp_composite")) return rc;
   DeviceGuard guard(ctx->cfg.device);
   if (const int rc = launch_mlp(ctx->launch, ctx->passes, ctx->fmt, kMlpComposite, (cudaStream_t)stream)) return rc;
   const bool fs = C > 0 && out->fixed_semantic_map && sample_box && box_sem;
@@ -1103,13 +1160,15 @@ static int aux_launch(pnr_ctx* ctx, pnr_ctx::Aux& aux, const char* what, const f
     PNR_CUDA(cudaMemsetAsync(stash_absmax, 0, sizeof(uint32_t) * (size_t)(2 * ctx->cfg.D - 1), (cudaStream_t)stream));
   p.grad_scale = grad_scale;
   p.grad_unscale = 1.0f / grad_scale;
+  if (const int rc = set_trunk_input(ctx, p, what)) return rc;
   return launch_mlp(aux.launch, ctx->passes, ctx->fmt, kMlpBackward, (cudaStream_t)stream);
 }
 
 // dL/d(embedded xyz) through the trunk (the tensor-core part of the MLP backward, SURVEY 8f rank 2): the forward
 // trunk is recomputed per tile (sign patterns stay in shared memory), then the layers run in reverse on the same tiles
 // with the transposed weight stream.  grad_h = dL/dh of the trunk output [R*N, W]; grad_emb [R*N, ld_emb], the first
-// 3 + 6*xyz_res columns of a row are the gradient (ld_emb = 64 with a 16-byte aligned base: vector stores).
+// trunk_input_width columns of a row are the gradient (ld_emb = trunk_input_kpad with a 16-byte aligned base: vector
+// stores).  For a hash-grid context that is dL/dh(x), which pnr_hashgrid_backward turns into the table's gradient.
 // stash (nullable) [2D-1, R*N, W] fp32 receives every A operand on the way: H_i (i < D-1) in slot i, the
 // pre-activation gradient dZ_j in slot 2D-2-j - the operands of the weight-gradient GEMMs dW_j = dZ_j^T H_{j-1}.
 // grad_scale: a power of two the incoming gradient is multiplied by on load (every gradient leaving the kernel is
@@ -1120,8 +1179,8 @@ extern "C" int pnr_mlp_backward_trunk(pnr_ctx* ctx, const float* pts, const floa
                                       float* stash, uint32_t* stash_absmax, void* stream) {
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(ctx && grad_h && grad_emb, "pnr_mlp_backward_trunk: null pointer");
-  PNR_CHECK_ARG(ld_emb >= 3 + 6 * ctx->cfg.xyz_res, "pnr_mlp_backward_trunk: ld_emb=%d < %d columns", ld_emb,
-                3 + 6 * ctx->cfg.xyz_res);
+  PNR_CHECK_ARG(ld_emb >= trunk_input_width(ctx->cfg), "pnr_mlp_backward_trunk: ld_emb=%d < %d columns", ld_emb,
+                trunk_input_width(ctx->cfg));
   int gexp = 0;
   PNR_CHECK_ARG(grad_scale > 0.f && grad_scale < 1.0e30f && grad_scale > 1.0e-30f && frexpf(grad_scale, &gexp) == 0.5f,
                 "pnr_mlp_backward_trunk: grad_scale=%g must be a positive power of two", (double)grad_scale);

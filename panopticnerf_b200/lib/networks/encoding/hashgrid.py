@@ -27,13 +27,18 @@ class _HashGridFn(torch.autograd.Function):
     def backward(ctx, g):
         xc, aabb = ctx.saved_tensors
         shape, has_aabb, L, F, T_log2, base, scale = ctx.meta
-        p = _capi.ptr
-        gt = torch.zeros(shape, dtype=torch.float32, device=xc.device)
-        gc = g.to(torch.float32).contiguous()
-        with torch.cuda.device(xc.device):
-            _capi.check(_capi.lib().pnr_hashgrid_backward(p(xc), xc.shape[0], p(aabb) if has_aabb else None, p(gc), L, F, T_log2,
-                                                          base, scale, p(gt), _capi.stream_ptr()), "pnr_hashgrid_backward")
+        gt = _table_grad(shape, xc, aabb if has_aabb else None, g, L, F, T_log2, base, scale)
         return gt, None, None, None, None, None, None, None
+
+
+def _table_grad(shape, xc, aabb, g, L, F, T_log2, base, scale) -> torch.Tensor:
+    p = _capi.ptr
+    gt = torch.zeros(shape, dtype=torch.float32, device=xc.device)
+    gc = g.to(torch.float32).contiguous()
+    with torch.cuda.device(xc.device):
+        _capi.check(_capi.lib().pnr_hashgrid_backward(p(xc), xc.shape[0], p(aabb), p(gc), L, F, T_log2,
+                                                      base, scale, p(gt), _capi.stream_ptr()), "pnr_hashgrid_backward")
+    return gt
 
 
 class HashGrid(nn.Module):
@@ -55,3 +60,10 @@ class HashGrid(nn.Module):
         _capi.ptr(xc, torch.float32, "x")                                          # CPU tensors raise here
         out = _HashGridFn.apply(self.table, xc, self.aabb, self.L, self.F, self.T_log2, self.base, self.scale)
         return out.reshape(*x.shape[:-1], self.out_dim)
+
+    def table_grad(self, x: torch.Tensor, grad_out: torch.Tensor) -> torch.Tensor:
+        """dL/dtable [L, 2^T_log2, F] for dL/d(features) grad_out [n, L*F] at the points x [n, 3] (pnr_hashgrid_backward;
+        fp32 atomics, so the last bits vary between runs)."""
+        xc = x.reshape(-1, 3).to(torch.float32).contiguous()
+        return _table_grad(tuple(self.table.shape), xc, self.aabb, grad_out.reshape(xc.shape[0], self.out_dim), self.L,
+                           self.F, self.T_log2, self.base, self.scale)

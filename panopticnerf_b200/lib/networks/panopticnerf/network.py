@@ -9,6 +9,12 @@ Parameter names follow nerf-pytorch, which the reference is recalled to inherit,
 ``forward(pts, viewdirs)`` runs the fused sm_90a kernel (positional encoding + all layers + heads in one
 launch, activations kept in shared memory) through the libpnr C ABI.  There is no PyTorch forward:
 CPU tensors raise.
+
+``cfg.xyz_encoding = "hashgrid"`` (a rule chosen here: the reference's 360 architecture is not in the mount) replaces
+gamma(x) in layer 0 and in the skip concatenation by h(x), the features of a multi-resolution hash grid
+(``xyz_encoder``, a `HashGrid`: parameter ``xyz_encoder.table`` [L, 2^T, F], buffer ``xyz_encoder.aabb``), E = L*F
+<= 64 columns.  The fused kernel gathers h(x) on chip from the table in place, so an optimiser step on the table is
+seen by the next launch without a repack.
 """
 from __future__ import annotations
 
@@ -20,10 +26,30 @@ import torch
 import torch.nn as nn
 
 from panopticnerf_b200 import _capi
+from panopticnerf_b200.lib.networks.encoding import HashGrid
 
 
 def embed_dim(L: int) -> int:
     return 3 + 6 * L
+
+
+def make_xyz_encoder(cfg) -> Optional[HashGrid]:
+    """The hash grid of a cfg.xyz_encoding = "hashgrid" network (None for "frequency"), its limits checked."""
+    enc = str(getattr(cfg, "xyz_encoding", "frequency"))
+    if enc == "frequency":
+        return None
+    if enc != "hashgrid":
+        raise ValueError(f"cfg.xyz_encoding={enc!r}: 'frequency' or 'hashgrid'")
+    L, F_ = int(getattr(cfg, "hash_levels", 16)), int(getattr(cfg, "hash_features", 2))
+    if F_ not in (1, 2, 4, 8) or not 1 <= L <= 32:
+        raise ValueError(f"hash grid: hash_features={F_} must be in {{1, 2, 4, 8}} and hash_levels={L} in [1, 32]")
+    if L * F_ > 64:
+        raise ValueError(f"hash grid: E = hash_levels * hash_features = {L * F_} > 64 (the fused kernel's embedding operand)")
+    aabb = getattr(cfg, "hash_aabb", None)
+    if aabb is None:
+        raise ValueError("cfg.xyz_encoding='hashgrid' needs cfg.hash_aabb = [lo.xyz, hi.xyz]")
+    return HashGrid(L, F_, int(getattr(cfg, "hash_log2_size", 19)), float(getattr(cfg, "hash_base_resolution", 16.0)),
+                    float(getattr(cfg, "hash_per_level_scale", 1.3819)), aabb=torch.as_tensor(aabb, dtype=torch.float32))
 
 
 class Network(nn.Module):
@@ -35,7 +61,9 @@ class Network(nn.Module):
         self.K = int(getattr(cfg, "num_instances", 0))
         self.precision = str(getattr(cfg, "precision", "fp16x3"))
         self.skip = self.D // 2
-        Ex, Ed, W = embed_dim(self.Lx), embed_dim(self.Ld), self.W
+        encoder = make_xyz_encoder(cfg)
+        Ex, Ed, W = embed_dim(self.Lx) if encoder is None else encoder.out_dim, embed_dim(self.Ld), self.W
+        self.in_dim = Ex                          # trunk input width: 3 + 6*xyz_res, or E = L*F of the hash grid
         self.pts_linears = nn.ModuleList(
             [nn.Linear(Ex, W)] + [nn.Linear(W + Ex if i == self.skip + 1 else W, W) for i in range(1, self.D)])
         self.alpha_linear = nn.Linear(W, 1)
@@ -46,6 +74,8 @@ class Network(nn.Module):
             self.semantic_linears = nn.ModuleList([nn.Linear(W, W // 2), nn.Linear(W // 2, self.C)])
         if self.K > 0:
             self.instance_linears = nn.ModuleList([nn.Linear(W, W // 2), nn.Linear(W // 2, self.K)])
+        if encoder is not None:
+            self.xyz_encoder = encoder
         self._ctx: Optional[int] = None
         self._ctx_key = None
 
@@ -84,10 +114,32 @@ class Network(nn.Module):
             ls += list(self.instance_linears)
         return ls
 
+    @property
+    def hashgrid(self) -> bool:
+        return hasattr(self, "xyz_encoder")
+
     def _weights_key(self, device):
-        return (str(device), self.precision) + tuple((p.data_ptr(), p._version) for p in self.parameters())
+        # the hash-grid table is not packed (the kernel reads it in place): its updates do not repack the linears
+        return (str(device), self.precision) + tuple((p.data_ptr(), p._version) for n, p in self.named_parameters()
+                                                     if not n.startswith("xyz_encoder."))
+
+    def _bind_table(self, device) -> None:
+        """Hand the current table tensor to the context (every pack: a replaced parameter is picked up)."""
+        t = self.xyz_encoder.table
+        if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
+            raise _capi.PnrError(f"Network: xyz_encoder.table must be a contiguous float32 tensor on {device}, got "
+                                 f"{t.dtype} on {t.device}")
+        _capi.check(_capi.lib().pnr_bind_hashgrid_table(self._ctx, t.data_ptr()), "pnr_bind_hashgrid_table")
 
     def pack(self, device=None) -> int:
+        """The libpnr context of this network on `device` (built on first use, refreshed when a linear changed); a
+        hash-grid network's table is (re)bound on every call."""
+        ctx = self._pack(device)
+        if self.hashgrid:
+            self._bind_table(torch.device(self._ctx_key[0]))
+        return ctx
+
+    def _pack(self, device=None) -> int:
         """(Re)build the libpnr context: weights are split into 16-bit hi/lo UMMA stage images (fp16 or bf16 per cfg.precision) once, and
         again only when a parameter changed (SURVEY.md section 5, 'weight packer')."""
         device = torch.device(device if device is not None else next(self.parameters()).device)
@@ -113,6 +165,12 @@ class Network(nn.Module):
         cfg = _capi.PnrConfig(self.D, self.W, self.Lx, self.Ld, self.C, self.K,
                               _capi.PREC[self.precision], device.index if device.index is not None
                               else torch.cuda.current_device())
+        if self.hashgrid:
+            e = self.xyz_encoder
+            cfg.xyz_encoding = _capi.XYZ_ENCODING["hashgrid"]
+            cfg.hash_levels, cfg.hash_features, cfg.hash_log2_size = e.L, e.F, e.T_log2
+            cfg.hash_base_resolution, cfg.hash_per_level_scale = e.base, e.scale
+            cfg.hash_aabb[:] = [float(v) for v in e.aabb.detach().cpu().reshape(6)]
         handle = C.c_void_p()
         _capi.check(L.pnr_create(C.byref(cfg), C.byref(handle)), "pnr_create")
         host, shapes = [], []
@@ -221,7 +279,8 @@ class Network(nn.Module):
     def backward_trunk(self, grad_h: torch.Tensor, pts: Optional[torch.Tensor] = None,
                        rays: Optional[torch.Tensor] = None, z: Optional[torch.Tensor] = None,
                        stash: bool = False, grad_scale: Optional[float] = None, absmax: bool = False):
-        """The tensor-core part of the MLP backward (pnr_mlp_backward_trunk): dL/d(embedded xyz) [S, 3 + 6*xyz_res] from
+        """The tensor-core part of the MLP backward (pnr_mlp_backward_trunk): dL/d(trunk input) [S, in_dim] (gamma(x), or
+        h(x) for a hash-grid network) from
         grad_h = dL/dh of the trunk output [S, W], for the samples given as pts [S,3] or as (rays [R,6], z [R,N]).
         What autograd computes through `pts_linears` (ReLUs, skip concatenation) of the reference Network.
         stash=True also returns the operands of the weight-gradient GEMMs, [2D-1, S, W] fp32: slot i < D-1 = the
@@ -234,7 +293,7 @@ class Network(nn.Module):
         R, N, S_, dev = self._samples(pts, rays, z)
         assert grad_h.shape == (S_, self.W), f"grad_h must be [{S_}, {self.W}]"
         ctx = self.pack(dev if grad_h.is_cuda else None)
-        Ex = 3 + 6 * self.Lx
+        Ex = self.in_dim
         ld = (Ex + 15) // 16 * 16                  # rows padded to whole 16-column groups: 16-byte stores in the kernel
         out = torch.empty(S_, ld, dtype=torch.float32, device=dev)
         st = torch.empty(2 * self.D - 1, S_, self.W, dtype=torch.float32, device=dev) if stash else None

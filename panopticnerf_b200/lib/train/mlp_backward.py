@@ -187,7 +187,8 @@ def network_backward(net, d_raw: torch.Tensor, pts: Optional[torch.Tensor] = Non
                      rays: Optional[torch.Tensor] = None, z: Optional[torch.Tensor] = None,
                      return_input_grad: bool = False) -> Dict[str, torch.Tensor]:
     """{parameter name: gradient} of `net` for dL/draw = d_raw [S, 4+C+K], samples given as (pts, viewdirs) [S,3] each
-    or as (rays [R,6], z [R,N]).  With return_input_grad also 'embedded_xyz': dL/d gamma(x) [S, 3+6*xyz_res]."""
+    or as (rays [R,6], z [R,N]).  With return_input_grad also 'embedded_xyz': dL/d(trunk input) [S, net.in_dim] (gamma(x),
+    or h(x) of a hash-grid network, whose table gradient 'xyz_encoder.table' comes from it through pnr_hashgrid_backward)."""
     if pts is None:
         o, d = rays[:, None, :3], rays[:, None, 3:]
         pts_ = (o + d * z[..., None]).reshape(-1, 3)                 # the kernel forms the same points (mul, then add)
@@ -198,20 +199,25 @@ def network_backward(net, d_raw: torch.Tensor, pts: Optional[torch.Tensor] = Non
     d_raw = d_raw.reshape(S_, -1).to(torch.float32)
     h = net.trunk_forward(pts=pts, rays=rays, z=z).requires_grad_(True)
     ed = P.embed(vd.contiguous(), net.Ld)
-    tail_named = [(n, p) for n, p in net.named_parameters() if not n.startswith("pts_linears.")]
+    tail_named = [(n, p) for n, p in net.named_parameters() if not n.startswith(("pts_linears.", "xyz_encoder."))]
     with torch.enable_grad():
         raw = _tail(net, h, ed)
         g = torch.autograd.grad(raw, [h] + [p for _, p in tail_named], d_raw, allow_unused=True)
     grads = {n: (gi if gi is not None else torch.zeros_like(p)) for (n, p), gi in zip(tail_named, g[1:])}
     d_emb, st, st_max = net.backward_trunk(g[0].contiguous(), pts=pts, rays=rays, z=z, stash=True, absmax=True)
-    ex = P.embed(pts_.contiguous(), net.Lx)
+    if net.hashgrid:             # h(x) of the same points (pnr_hashgrid_encode: the features the fused kernel gathered)
+        with torch.no_grad():
+            ex = net.xyz_encoder(pts_.contiguous())
+        grads["xyz_encoder.table"] = net.xyz_encoder.table_grad(pts_, d_emb)
+    else:
+        ex = P.embed(pts_.contiguous(), net.Lx)
     D = net.D
     pr = net.precision if net.precision in ("fp16x3", "bf16x3") else "fp16x3"
     # fp16 parts: one power-of-two scale per dZ_j, from the maxima the backward kernel collected while writing the stash
     scales = _pow2_from_max(st_max[D - 1:])[::-1] if pr == "fp16x3" else [None] * D
     for j in range(D):
         dZ = st[2 * D - 2 - j]
-        if j == net.skip + 1:        # input [gamma(x), H_{j-1}]: two column blocks of dW, no concatenated copy
+        if j == net.skip + 1:        # input [gamma(x) or h(x), H_{j-1}]: two column blocks of dW, no concatenated copy
             dWx, db = wgrad(dZ, ex, precision=pr, scale=scales[j])
             dW = torch.cat([dWx, wgrad(dZ, st[j - 1], bias=False, precision=pr, scale=scales[j])[0]], -1)
         else:

@@ -65,10 +65,13 @@ def make_batch(cfg, seed: int = 0, row0: int = 0, rows: Optional[int] = None, nu
 
 def init_network_weights(net: torch.nn.Module, seed: int = 0) -> torch.nn.Module:
     """Re-draws every nn.Linear with PyTorch's default init from a fixed seed, then shifts the sigma
-    bias so that accumulated opacity is non-trivial on the synthetic scene."""
+    bias so that accumulated opacity is non-trivial on the synthetic scene.  A hash-grid network's table is drawn
+    U(-1, 1) after the linears (features of O(1)); the linears get the same values as without it."""
     g = torch.Generator().manual_seed(seed)
     with torch.no_grad():
         for name, p in sorted(net.named_parameters()):
+            if name.startswith("xyz_encoder."):
+                continue
             if p.dim() == 2:
                 bound = 1.0 / math.sqrt(p.shape[1])
                 p.copy_((torch.rand(p.shape, generator=g) * 2 - 1) * bound)
@@ -77,4 +80,7 @@ def init_network_weights(net: torch.nn.Module, seed: int = 0) -> torch.nn.Module
                 bound = 1.0 / math.sqrt(w.shape[1])
                 p.copy_((torch.rand(p.shape, generator=g) * 2 - 1) * bound)
         net.alpha_linear.bias.add_(0.1)
+        enc = getattr(net, "xyz_encoder", None)
+        if enc is not None:
+            enc.table.copy_(torch.rand(enc.table.shape, generator=g) * 2 - 1)
     return net
