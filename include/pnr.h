@@ -91,7 +91,7 @@ int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
  * the skip layer's first columns) is 3 + 6*xyz_res, or E = hash_levels * hash_features for a hash-grid context (whose
  * table is not in this list: pnr_bind_hashgrid_table).  Weights are split
  * into 16-bit hi/lo parts of the context's operand format (fp16 or bf16, cfg.precision), laid out as
- * no-swizzle K-major UMMA stage images and uploaded.  In the fp16 modes a weight with |w| > 65504 is
+ * the no-swizzle K-major wgmma stage images of the packed weight stream (csrc/mlp_program.h) and uploaded.  In the fp16 modes a weight with |w| > 65504 is
  * rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode. */
 int pnr_load_weights(pnr_ctx* ctx, const float* const* tensors_host, const int64_t* shapes, int32_t n);
 
@@ -151,15 +151,6 @@ int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void* stream);
  * normalised view direction formed in-kernel (pass pts = NULL).  raw [n or R*N, 4+C+K]. */
 int pnr_mlp_forward(pnr_ctx* ctx, const float* pts, const float* viewdirs, const float* rays,
                     const float* z, int64_t R, int32_t N, float* raw, void* stream);
-
-/* Development aid: as pnr_mlp_forward(rays, z) but block 0 also records a clock64 timeline of its third
- * tile into timeline[8192] (i64, device): [3*stage+{0,1,2}] MMA issuer (arrive / ready / issued),
- * [4096 + 3*(2*step+half)+{0,1,2}] epilogue (wait / accumulator ready / done), [6144 + stage] TMA issue. */
-int pnr_mlp_forward_timeline(pnr_ctx* ctx, const float* rays, const float* z, int64_t R, int32_t N,
-                             float* raw, int64_t* timeline, void* stream);
-/* Development aid: the pnr_mlp_composite and pnr_mlp_backward_trunk launches of `ctx` record the same timeline into timeline[8192] (device i64)
- * until this is called again with NULL (-DPNR_TIMELINE builds only; ignored otherwise). */
-int pnr_debug_timeline(pnr_ctx* ctx, int64_t* timeline);
 
 /* a9: raw2outputs.  raw [R,N,4+C+K], z [R,N], rays [R,6].  Any output pointer may be NULL.
  * sem_softmax: composite softmax(logits) instead of logits.  sample_box/box_sem/box_inst nullable. */

@@ -96,8 +96,6 @@ SIGNATURES = {
     "pnr_mlp_forward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_composite": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i32,
                                     C.POINTER(PnrCompositeOut), _vp]),
-    "pnr_mlp_forward_timeline": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
-    "pnr_debug_timeline": (C.c_int, [_vp, _vp]),
     "pnr_mlp_backward_trunk": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, C.c_float, _vp, _i32, _vp, _vp, _vp]),
     "pnr_mlp_trunk_forward": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "pnr_composite": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _i32,

@@ -23,9 +23,10 @@
 // straddles column 128), so that the first half of a tile's layer 0 does not wait for the previous tile's last
 // epilogue.
 //
-// VIEW ON PRODUCERS (networks without heads, forward).  view_step >= 0: the view step is the tile's last and may run its
-// epilogue apart from the other steps (on sm_90 such a program runs exactly like the plain one); its last stage is flagged F_COMMIT_VIEW and the first stage of the next tile
-// that reuses its accumulator columns waits for it.
+// VIEW ON PRODUCERS (networks without heads, forward; built by pnr_program_host with PNR_PROGRAM_VIEW_PRODUCERS only, a
+// context does not launch it).  view_step >= 0: the view step is the tile's last and may run its epilogue apart from
+// the other steps; its last stage is flagged F_COMMIT_VIEW and the first stage of the next tile that reuses its
+// accumulator columns waits for it.
 //
 // BACKWARD (dL/d(embedded input) through the trunk, on the same tiles).  A backward program is the trunk's forward
 // steps - whose EPI_RELU_TO_A epilogues also save the 16-column sign patterns of their activations - followed by one
@@ -40,6 +41,10 @@
 // streams, devices or graph replays).
 #pragma once
 #include <stdint.h>
+#include <string.h>
+#if defined(__CUDACC__)
+#include <cuda_fp16.h>
+#endif
 
 namespace pnr {
 
@@ -99,6 +104,31 @@ __host__ __device__
 #endif
 constexpr bool epi_writes_a(uint8_t kind) { return kind == EPI_RELU_TO_A || kind == EPI_MASK_TO_A || kind == EPI_LOADG_TO_A; }
 
+#if defined(__CUDACC__)
+__host__ __device__ inline uint16_t bf16_rne(float x) {   // round to nearest even on the bit pattern (= cvt.rn.bf16.f32)
+  uint32_t u;
+  memcpy(&u, &x, 4);
+  return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+
+// Element of the packed weight stream: part 0 (hi) or 1 (lo) of weight w in the operand format (fmt 0 = fp16, 1 = bf16),
+// hi = w rounded to nearest even, lo = (w - hi) rounded to nearest even.  A stage's hi image holds part 0 of its
+// weights, the lo image (x3 modes) part 1.  The host builder and the device-side weight update (pnr_update_weights)
+// both pack with this function, so that a refreshed stream is bit-identical to a freshly built one.
+__host__ __device__ inline uint16_t weight_part16(float w, int part, int fmt) {
+  if (fmt == 1) {
+    const uint16_t hi = bf16_rne(w);
+    if (part == 0) return hi;
+    const uint32_t hb = (uint32_t)hi << 16;
+    float h;
+    memcpy(&h, &hb, 4);
+    return bf16_rne(w - h);
+  }
+  const __half h = __float2half_rn(w);
+  return __half_as_ushort(part == 0 ? h : __float2half_rn(w - __half2float(h)));
+}
+#endif
+
 struct StageDesc {     // one weight stage = one bulk copy + its MMAs
   uint32_t gofs;       // byte offset into the packed weight stream
   uint32_t bytes;
@@ -155,7 +185,7 @@ struct MlpProgram {
   EpiDesc ep[kMaxSteps];
 };
 
-enum { kMlpForward = 0, kMlpComposite = 1, kMlpBackward = 2, kMlpForwardVP = 3 };   // launch_mlp's `mode`
+enum { kMlpForward = 0, kMlpComposite = 1, kMlpBackward = 2 };   // launch_mlp's `mode`
 
 // Launch arguments of the fused kernel (device pointers).
 struct MlpParams {
@@ -171,7 +201,6 @@ struct MlpParams {
   float* raw;
   int32_t num_tiles;
   uint32_t* status;       // sticky device word: bit 0 = a non-finite / out-of-range activation was seen (may be null)
-  long long* dbg;         // optional clock64 timeline of block 0 (development aid), else null
   // ---- compositing epilogue (COMPOSITE kernels only: rays mode, N % 32 == 0; `raw` is not written)
   int64_t rays_per_cta;   // every CTA owns a contiguous range of whole rays (carries stay on chip)
   const int32_t* sample_box;   // [S] primitive id per sample, or null (only read when mask_outside)

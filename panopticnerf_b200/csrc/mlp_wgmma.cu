@@ -904,8 +904,7 @@ static int launch_one(const MlpLaunch& L, int dev, int grid, cudaStream_t stream
 
 // Launches on the CURRENT device (the caller has made the context's device current).  mode 1: the
 // compositing-epilogue variant; the launch's rays_per_cta is set here (whole rays per CTA, so that every CTA's range
-// starts on a 32-sample boundary).  mode 2: L.prog is a backward program (x3 precisions only).  mode 3 (a program whose
-// view step was built for an epilogue on separate warps) runs like mode 0: this kernel runs every epilogue itself.
+// starts on a 32-sample boundary).  mode 2: L.prog is a backward program (x3 precisions only).
 int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream) {
   const bool composite = mode == kMlpComposite;
   int dev = 0;
@@ -926,7 +925,6 @@ int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream)
     return fmt == kFmtF16 ? launch_one<3, kFmtF16, false, true>(L, dev, grid, stream)
                           : launch_one<3, kFmtBF16, false, true>(L, dev, grid, stream);
   }
-  if (mode == kMlpForwardVP && L.prog.view_step < 0) return set_error(PNR_ERR_STATE, "launch_mlp: not a view-on-producers program");
 #define PNR_LAUNCH(P, F) (composite ? launch_one<P, F, true>(L, dev, grid, stream) : launch_one<P, F, false>(L, dev, grid, stream))
   if (fmt == kFmtF16) return passes == 3 ? PNR_LAUNCH(3, kFmtF16) : PNR_LAUNCH(1, kFmtF16);
   return passes == 3 ? PNR_LAUNCH(3, kFmtBF16) : PNR_LAUNCH(1, kFmtBF16);

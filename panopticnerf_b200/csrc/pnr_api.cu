@@ -1,8 +1,6 @@
 // pnr_api.cu — context management, weight packing / MLP program construction and the
 // pnr_mlp_forward entry point of the C ABI (include/pnr.h).
-#include <cstdlib>
 #include <cstring>
-#include <cuda_fp16.h>
 #include <string>
 #include <vector>
 #include "common.cuh"
@@ -31,72 +29,45 @@ int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream)
 
 using namespace pnr;
 
+// The MLP programs of a context, all over the same weights: forward (pnr_mlp_forward, pnr_mlp_composite,
+// pnr_render_fused), backward (pnr_mlp_backward_trunk) and trunk-forward (pnr_mlp_trunk_forward).  pnr_load_weights
+// builds the forward program; the other two are built on first use.
+enum ProgramKind { kProgForward = 0, kProgBackward = 1, kProgTrunkForward = 2, kNumPrograms = 3 };
+
+struct PackedProgram {
+  bool ready = false;             // built and uploaded since the last pnr_load_weights
+  MlpLaunch launch;               // launch.prog = the program; launch.p is filled per call.  The whole struct travels as
+                                  // the kernel's __grid_constant__ parameter: nothing is shared between contexts,
+                                  // streams, devices or CUDA-graph replays.
+  uint8_t* d_wpacked = nullptr;
+  float* d_consts = nullptr;
+  size_t n_w = 0, n_c = 0;        // packed 16-bit elements / constants
+  // device-side weight updates: packed element p = part d_wpart[p] of V[d_widx[p]], constant c = V[d_cidx[c]]
+  // (Builder index mode), built by the first pnr_update_weights that refreshes this program
+  bool plan_ready = false;
+  int32_t* d_widx = nullptr;
+  uint8_t* d_wpart = nullptr;
+  int32_t* d_cidx = nullptr;
+};
+
 struct pnr_ctx {
   pnr_config cfg;
   int passes = 3;
   int fmt = 0;   // 0 = fp16, 1 = bf16 (instruction-descriptor encoding)
   bool loaded = false;
-  MlpLaunch launch;             // launch.prog = this context's program; launch.p is filled per call.  The whole
-                                // struct travels as the kernel's __grid_constant__ parameter: nothing is shared
-                                // between contexts, streams, devices or CUDA-graph replays.
-  MlpLaunch launch_vp;          // the same stages with the view epilogue on the producer warps (networks without heads;
-  bool has_vp = false;          //   pnr_mlp_forward uses it, pnr_mlp_composite keeps the standard program)
-  uint8_t* d_wpacked = nullptr;
-  float* d_consts = nullptr;
+  PackedProgram prog[kNumPrograms];
   uint32_t* d_status = nullptr; // sticky range-check word of the fused MLP (bit 0: activation out of operand range)
   const float* hash_table = nullptr;   // hash-grid contexts: the caller's table (pnr_bind_hashgrid_table), not owned
   uint32_t hash_res[kHashMaxLevels] = {};
-  size_t wpacked_bytes = 0;
-  // backward program of the trunk (pnr_mlp_backward_trunk): built from a host copy of the trunk weights on first use
-  std::vector<std::vector<float>> host_trunk;   // weight, bias per trunk layer, as given to pnr_load_weights
+  // what the backward and trunk-forward programs are built from: weight, bias per trunk layer, as given to pnr_load_weights
+  std::vector<std::vector<float>> host_trunk;
   std::vector<int64_t> host_trunk_shapes;
-  long long* dbg_timeline = nullptr;   // development aid (pnr_debug_timeline)
-  struct Aux {                         // a second program over the same weights, with its own packed stream
-    bool ready = false;
-    MlpLaunch launch;
-    uint8_t* d_wpacked = nullptr;
-    float* d_consts = nullptr;
-    size_t n_w = 0, n_c = 0;           // packed 16-bit elements / constants
-  };
-  Aux bwd;                             // forward trunk + the layers in reverse (pnr_mlp_backward_trunk)
-  Aux trunk_fwd;                       // forward trunk only, output = its activations (pnr_mlp_trunk_forward)
-  // device-side weight updates (pnr_update_weights): V = all input tensors concatenated + the derived (folded) values,
-  // and per program the plan "packed element p = part wpart[p] of V[widx[p]]" (Builder index mode)
-  struct Plan {
-    bool ready = false;
-    int32_t* d_widx = nullptr; uint8_t* d_wpart = nullptr; size_t n_w = 0;
-    int32_t* d_cidx = nullptr; size_t n_c = 0;
-  };
-  Plan plan_main, plan_bwd, plan_tf;
+  // device-side weight updates (pnr_update_weights): V = all input tensors concatenated + the derived (folded) values
   float* d_V = nullptr;
   std::vector<int64_t> v_off, all_shapes;   // position of every input tensor in V; the shapes given to pnr_load_weights
   int64_t v_total = 0, v_derived = 0;
-  bool device_weights = false;              // the weights in V are newer than the host copies (aux programs re-pack from V)
+  bool device_weights = false;              // the weights in V are newer than the host copies (programs built later are packed from V)
 };
-
-// ---------------------------------------------------------------- host-side 16-bit split (RNE, = cvt.rn.*.f32)
-static inline uint16_t f2h(float x) {
-  const __half h = __float2half_rn(x);
-  uint16_t u;
-  memcpy(&u, &h, 2);
-  return u;
-}
-static inline float h2f(uint16_t u) {
-  __half h;
-  memcpy(&h, &u, 2);
-  return __half2float(h);
-}
-static inline uint16_t f2bf(float x) {
-  uint32_t u;
-  memcpy(&u, &x, 4);
-  return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
-}
-static inline float bf2f(uint16_t h) {
-  uint32_t u = (uint32_t)h << 16;
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
-}
 
 namespace {
 
@@ -127,10 +98,9 @@ struct Builder {
   // (the x3 modes, K = 64 per stage: 75.4 k -> 71.5 k cycles per tile); the 1-pass modes keep one block.
   bool split_e1;
   bool acc_flip = true;             // odd tiles use the accumulator columns XOR 128 when the program allows it
-  bool view_one_half = true;        // the view step is issued as one N = W/2 half
   bool view_on_producers = false;   // the (last, one-half) view step's epilogue runs on the producer warps (mlp_program.h)
   bool out_of_fp16_range = false;   // a weight (after the feature_linear fold) exceeds 65504 or is not finite
-  // INDEX MODE (device-side weight updates, weights_update.cu): the builder is run once on tensors whose VALUES are
+  // INDEX MODE (device-side weight updates, pnr_update_weights): the builder is run once on tensors whose VALUES are
   // their own position (+1) in the concatenation V of all input tensors followed by the derived values (the folded
   // view matrix and bias, which build_program then fills with positions instead of arithmetic).  Everything else in a
   // program's packed stream and constant table is a copy of one source value, so this run yields, per packed element,
@@ -144,8 +114,6 @@ struct Builder {
   Builder(int passes_, int fmt_) : passes(passes_), fmt(fmt_) {
     memset(&prog, 0, sizeof(prog));
     split_e1 = passes == 3;
-    if (const char* v = getenv("PNR_ACC_FLIP")) acc_flip = *v != '0';   // tuning aids (A/B on the GPU)
-    if (const char* v = getenv("PNR_VIEW_ONE_HALF")) view_one_half = *v != '0';
   }
 
   int add_consts(const float* src, int n_valid, int n_pad) {
@@ -173,15 +141,7 @@ struct Builder {
           } else if (!(w >= -65504.f && w <= 65504.f)) {
             out_of_fp16_range = true;   // also catches NaN
           }
-          uint16_t v;
-          if (fmt == 1) {
-            const uint16_t h = f2bf(w);
-            v = part == 0 ? h : f2bf(w - bf2f(h));
-          } else {
-            const uint16_t h = f2h(w);
-            v = part == 0 ? h : f2h(w - h2f(h));
-          }
-          wbuf[base + ((size_t)kc * n_pad + nn) * 8 + e] = v;
+          wbuf[base + ((size_t)kc * n_pad + nn) * 8 + e] = weight_part16(w, part, fmt);
         }
   }
 
@@ -377,9 +337,27 @@ struct Builder {
       d.flags_k = (uint32_t)sd.flags | ((uint32_t)sd.ksteps << 16) | ((uint32_t)sd.a_kind << 24);
     }
   }
+
+  // The end of every build: `ok` = every step was added; `what` names the program in the error text.
+  int finish(bool ok, const char* what) {
+    if (!ok) return set_error(PNR_ERR_UNSUPPORTED, "%s: program build failed: %s", what, err.c_str());
+    if ((int)consts.size() > kMaxConsts)
+      return set_error(PNR_ERR_UNSUPPORTED, "%s: %d constants > %d", what, (int)consts.size(), kMaxConsts);
+    if (out_of_fp16_range && fmt == kFmtF16)
+      return set_error(PNR_ERR_UNSUPPORTED, "%s: a weight is outside the fp16 range (|w| > 65504 or not finite): use "
+                       "precision bf16x3", what);
+    prog.n_consts = (int)consts.size();
+    finalize();
+    return PNR_OK;
+  }
 };
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// A segment that reads columns [col0, col0 + k) of m against the activation operand columns a_hi / a_lo
+Seg seg_tmem(const Mat& m, int col0, int k, int a_hi = kColAHi, int a_lo = kColALo) {
+  return Seg{A_TMEM, m, col0, k, round_up(k, 16), a_hi, a_lo, false};
+}
 
 
 }  // namespace
@@ -458,8 +436,6 @@ extern "C" int pnr_create(const pnr_config* cfg, pnr_ctx** out) {
   c->passes = precision_passes(cfg->precision);
   c->fmt = precision_fmt(cfg->precision);
   if (is_hashgrid(*cfg)) hash_level_resolutions(cfg->hash_levels, cfg->hash_base_resolution, cfg->hash_per_level_scale, c->hash_res);
-  memset(&c->launch, 0, sizeof(c->launch));
-  memset(&c->launch_vp, 0, sizeof(c->launch_vp));
   cudaError_t e = cudaMalloc(&c->d_status, sizeof(uint32_t));
   if (e == cudaSuccess) e = cudaMemset(c->d_status, 0, sizeof(uint32_t));
   if (e != cudaSuccess) {
@@ -470,18 +446,21 @@ extern "C" int pnr_create(const pnr_config* cfg, pnr_ctx** out) {
   return PNR_OK;
 }
 
+// Frees the program's device buffers and forgets it (plain cudaFree: it synchronises with the device, so no launch still
+// reads them).
+static void release(PackedProgram& pp) {
+  cudaFree(pp.d_wpacked);
+  cudaFree(pp.d_consts);
+  cudaFree(pp.d_widx);
+  cudaFree(pp.d_wpart);
+  cudaFree(pp.d_cidx);
+  pp = PackedProgram();
+}
+
 extern "C" int pnr_destroy(pnr_ctx* ctx) {
   if (!ctx) return PNR_OK;
   DeviceGuard guard(ctx->cfg.device);
-  cudaFree(ctx->d_wpacked);
-  cudaFree(ctx->d_consts);
-  cudaFree(ctx->bwd.d_wpacked);
-  cudaFree(ctx->bwd.d_consts);
-  cudaFree(ctx->trunk_fwd.d_wpacked);
-  cudaFree(ctx->trunk_fwd.d_consts);
-  for (pnr_ctx::Plan* pl : {&ctx->plan_main, &ctx->plan_bwd, &ctx->plan_tf}) {
-    cudaFree(pl->d_widx); cudaFree(pl->d_wpart); cudaFree(pl->d_cidx);
-  }
+  for (PackedProgram& pp : ctx->prog) release(pp);
   cudaFree(ctx->d_V);
   cudaFree(ctx->d_status);
   delete ctx;
@@ -501,15 +480,76 @@ extern "C" int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, vo
   return PNR_OK;
 }
 
+// The trunk layers of a network: weight [W, in] and bias [W] of layers 0..D-1, the first 2*D tensors of
+// pnr_load_weights' list.  Layer 0 reads the trunk input, the skip layer D/2 + 1 [trunk input ; h].
+struct Trunk {
+  std::vector<Mat> w;
+  std::vector<const float*> b;
+};
+
+static int take_trunk(const pnr_config& c, const float* const* t, const int64_t* shapes, const char* what, Trunk& tr) {
+  const int D = c.D, W = c.W, Ex = trunk_input_width(c), skip = D / 2;
+  tr.w.resize(D);
+  tr.b.resize(D);
+  for (int i = 0; i < D; ++i) {
+    const int in = i == 0 ? Ex : (i == skip + 1 ? W + Ex : W);
+    if (shapes[4 * i] != W || shapes[4 * i + 1] != in || shapes[4 * i + 2] != W || shapes[4 * i + 3] != 1 || !t[2 * i] ||
+        !t[2 * i + 1])
+      return set_error(PNR_ERR_ARG, "%s: tensor %d: expected weight [%d,%d] + bias [%d,1]", what, 2 * i, W, in, W);
+    tr.w[i] = Mat{t[2 * i], W, in};
+    tr.b[i] = t[2 * i + 1];
+  }
+  return PNR_OK;
+}
+
+// Steps 0..D-1 of a program, the trunk's forward layers: ReLU activations into the A operand columns, the last layer's
+// epilogue `last_kind`.  sigma_w_off >= 0: the last layer also accumulates the sigma head, whose weights are at that
+// constant offset.  slots: layer i keeps what its epilogue produces in stash slot i (H_i; dZ_{D-1} for the last layer)
+// and, below the last, its sign pattern in slot i - the backward program's forward half.
+static bool add_trunk_steps(const pnr_config& c, const Trunk& tr, uint8_t last_kind, int sigma_w_off, bool slots,
+                            Builder& bld) {
+  const int D = c.D, W = c.W, Ex = trunk_input_width(c), Ekpad = trunk_input_kpad(c), skip = D / 2;
+  bld.prog.Lx = is_hashgrid(c) ? 0 : c.xyz_res;
+  bld.prog.Ld = c.view_res;
+  bld.prog.passes = bld.passes;
+  for (int i = 0; i < D; ++i) {
+    EpiDesc ed{};
+    ed.kind = i == D - 1 ? last_kind : EPI_RELU_TO_A;
+    if (sigma_w_off >= 0) {
+      ed.sigma = i == D - 1 ? 1 : 0;
+      ed.aux_off = (uint16_t)sigma_w_off;
+    }
+    if (slots) {
+      ed.n_valid = i == D - 1 ? 0 : (uint16_t)(i + 1);   // sign-pattern slot + 1
+      ed.out_off1 = (uint16_t)(i + 1);                   // stash slot + 1: H_i, or dZ_{D-1} for i = D-1
+    }
+    ed.dst_col = kColAHi;
+    ed.dst_lo_col = kColALo;
+    ed.bias_off = (uint16_t)bld.add_consts(tr.b[i], W, W);
+    std::vector<Seg> segs;
+    if (i == 0) {
+      segs.push_back(Seg{A_EMB, tr.w[i], 0, Ex, Ekpad, 0, 0, false});
+    } else if (i == skip + 1) {
+      segs.push_back(Seg{A_EMB, tr.w[i], 0, Ex, Ekpad, 0, 0, true});
+      segs.push_back(seg_tmem(tr.w[i], Ex, W));
+    } else {
+      segs.push_back(seg_tmem(tr.w[i], 0, W));
+    }
+    if (!bld.add_step(segs, W, kColAcc, ed, i == 0)) return false;
+  }
+  return true;
+}
+
 // Host only (no CUDA call): checks the tensor list against cfg, builds the per-tile program, the packed
 // weight stream and the constant table.  Shared by pnr_load_weights and pnr_program_host.
 static int build_program(const pnr_config& c, const float* const* t, const int64_t* shapes, int32_t n,
                          Builder& bld) {
-  const int D = c.D, W = c.W, W2 = W / 2, C = c.num_classes, K = c.num_instances;
-  const int Ex = trunk_input_width(c), Ekpad = trunk_input_kpad(c), Ed = 3 + 6 * c.view_res, skip = D / 2;
+  const int D = c.D, W = c.W, W2 = W / 2, C = c.num_classes, K = c.num_instances, Ed = 3 + 6 * c.view_res;
   const int expected = 2 * D + 8 + (C > 0 ? 4 : 0) + (K > 0 ? 4 : 0);
   PNR_CHECK_ARG(n == expected, "pnr_load_weights: got %d tensors, expected %d", n, expected);
-  int ti = 0;
+  Trunk trunk;
+  if (const int rc = take_trunk(c, t, shapes, "pnr_load_weights", trunk)) return rc;
+  int ti = 2 * D;
   auto take = [&](int out, int in, Mat* m, const float** bias) -> bool {
     if (shapes[2 * ti] != out || shapes[2 * ti + 1] != in) return false;
     if (shapes[2 * ti + 2] != out || shapes[2 * ti + 3] != 1) return false;
@@ -523,17 +563,6 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
   if (!take(out, in, m, b))                                                                            \
     return set_error(PNR_ERR_ARG, "pnr_load_weights: tensor %d: expected weight [%d,%d] + bias [%d,1]", \
                      ti, out, in, out)
-
-  bld.prog.Lx = is_hashgrid(c) ? 0 : c.xyz_res;
-  bld.prog.Ld = c.view_res;
-  bld.prog.passes = bld.passes;
-
-  std::vector<Mat> trunk(D);
-  std::vector<const float*> trunk_b(D);
-  for (int i = 0; i < D; ++i) {
-    const int in = i == 0 ? Ex : (i == skip + 1 ? W + Ex : W);
-    PNR_TAKE(W, in, &trunk[i], &trunk_b[i]);
-  }
   Mat m_sig, m_feat, m_view, m_rgb, m_s1, m_s2, m_i1, m_i2;
   const float *b_sig, *b_feat, *b_view, *b_rgb, *b_s1 = nullptr, *b_s2 = nullptr, *b_i1 = nullptr, *b_i2 = nullptr;
   PNR_TAKE(1, W, &m_sig, &b_sig);
@@ -552,30 +581,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
   const int rgb_w_off = bld.add_consts(rgbw.data(), 3 * W2, 3 * W2);
   bld.prog.rgb_bias_off = bld.add_consts(b_rgb, 3, 4);
 
-  auto seg_tmem = [&](const Mat& m, int col0, int k, int a_hi, int a_lo) {
-    return Seg{A_TMEM, m, col0, k, round_up(k, 16), a_hi, a_lo, false};
-  };
-  bool ok = true;
-  // trunk
-  for (int i = 0; i < D && ok; ++i) {
-    EpiDesc ed{};
-    ed.kind = EPI_RELU_TO_A;
-    ed.sigma = (i == D - 1) ? 1 : 0;
-    ed.dst_col = kColAHi;
-    ed.dst_lo_col = kColALo;
-    ed.bias_off = (uint16_t)bld.add_consts(trunk_b[i], W, W);
-    ed.aux_off = (uint16_t)sig_w_off;
-    std::vector<Seg> segs;
-    if (i == 0) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, false});
-    } else if (i == skip + 1) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, true});
-      segs.push_back(seg_tmem(trunk[i], Ex, W, kColAHi, kColALo));
-    } else {
-      segs.push_back(seg_tmem(trunk[i], 0, W, kColAHi, kColALo));
-    }
-    ok = bld.add_step(segs, W, kColAcc, ed, i == 0);
-  }
+  bool ok = add_trunk_steps(c, trunk, EPI_RELU_TO_A, sig_w_off, false, bld);
   // feature_linear has no activation, so it is folded into the view layer when the weights are loaded
   // (exact algebra, done in double):  W_view [feat ; gamma(d)] + b_view  with  feat = W_feat h + b_feat
   //   = (W_view[:, :W] W_feat) h + W_view[:, W:] gamma(d) + (W_view[:, :W] b_feat + b_view).
@@ -614,7 +620,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     // (an M=128 N=64 K=16 MMA is no faster than 0.84 of an N=128 one: profiles/r01_mma_rate_probe.log) - 7-8 k cycles
     // of tensor pipe at the one place of the tile where nothing else can be issued.  What the halves bought, the view
     // epilogue's first part overlapping the second half's MMAs, is worth less than that.
-    ok = ok && bld.add_step(segs, W2, acc_col, ed, false, nullptr, (bld.view_one_half && W2 <= 128) ? W2 : 0);
+    ok = ok && bld.add_step(segs, W2, acc_col, ed, false, nullptr, W2 <= 128 ? W2 : 0);
   };
   // heads: hidden layer -> logits
   auto add_head = [&](const Mat& m1, const float* b1, const Mat& m2, const float* b2, int nout, int out_off) {
@@ -673,17 +679,8 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     if (ok && K > 0) add_head(m_i1, b_i1, m_i2, b_i2, K, 4 + C);
     add_view(kColAcc);
   }
-  if (!ok) return set_error(PNR_ERR_UNSUPPORTED, "pnr_load_weights: program build failed: %s", bld.err.c_str());
-  if ((int)bld.consts.size() > kMaxConsts)
-    return set_error(PNR_ERR_UNSUPPORTED, "pnr_load_weights: %d constants > %d", (int)bld.consts.size(), kMaxConsts);
-  if (bld.out_of_fp16_range && bld.fmt == kFmtF16)
-    return set_error(PNR_ERR_UNSUPPORTED, "pnr_load_weights: a weight is outside the fp16 range (|w| > 65504 or not "
-                     "finite): use precision bf16x3");
-  bld.prog.n_consts = (int)bld.consts.size();
-  bld.finalize();
-  return PNR_OK;
+  return bld.finish(ok, "pnr_load_weights");
 }
-
 
 // Backward program of the trunk (mlp_program.h, "BACKWARD"): t / shapes = the trunk's weight, bias pairs (the first
 // 2*D tensors of pnr_load_weights' list).  Forward steps 0..D-1 (sign patterns kept, the last one loads the incoming
@@ -700,47 +697,15 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
     return set_error(PNR_ERR_UNSUPPORTED, "backward program: precision must be fp16x3 or bf16x3");
   if (D - 1 > kMaxMaskSlots)
     return set_error(PNR_ERR_UNSUPPORTED, "backward program: D=%d needs %d sign-pattern slots, %d fit", D, D - 1, kMaxMaskSlots);
-  std::vector<Mat> trunk(D);
-  std::vector<const float*> trunk_b(D);
-  for (int i = 0; i < D; ++i) {
-    const int in = i == 0 ? Ex : (i == skip + 1 ? W + Ex : W);
-    if (shapes[4 * i] != W || shapes[4 * i + 1] != in || shapes[4 * i + 2] != W || shapes[4 * i + 3] != 1 || !t[2 * i] || !t[2 * i + 1])
-      return set_error(PNR_ERR_ARG, "backward program: trunk layer %d: expected weight [%d,%d] + bias [%d,1]", i, W, in, W);
-    trunk[i] = Mat{t[2 * i], W, in};
-    trunk_b[i] = t[2 * i + 1];
-  }
-  bld.prog.Lx = is_hashgrid(c) ? 0 : c.xyz_res;
-  bld.prog.Ld = c.view_res;
-  bld.prog.passes = bld.passes;
-  auto seg_tmem = [&](const Mat& m, int col0, int k) {
-    return Seg{A_TMEM, m, col0, k, round_up(k, 16), kColAHi, kColALo, false};
-  };
-  bool ok = true;
-  for (int i = 0; i < D && ok; ++i) {   // forward, as in build_program (no sigma head)
-    EpiDesc ed{};
-    ed.kind = (i == D - 1) ? (forward_only ? EPI_ACT_OUT : EPI_LOADG_TO_A) : EPI_RELU_TO_A;
-    ed.n_valid = (i == D - 1 || forward_only) ? 0 : (uint16_t)(i + 1);      // sign-pattern slot + 1
-    ed.out_off1 = forward_only ? 0 : (uint16_t)(i + 1);                       // stash slot + 1: H_i, or dZ_{D-1} for i = D-1
-    ed.dst_col = kColAHi;
-    ed.dst_lo_col = kColALo;
-    ed.bias_off = (uint16_t)bld.add_consts(trunk_b[i], W, W);
-    std::vector<Seg> segs;
-    if (i == 0) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, false});
-    } else if (i == skip + 1) {
-      segs.push_back(Seg{A_EMB, trunk[i], 0, Ex, Ekpad, 0, 0, true});
-      segs.push_back(seg_tmem(trunk[i], Ex, W));
-    } else {
-      segs.push_back(seg_tmem(trunk[i], 0, W));
-    }
-    ok = bld.add_step(segs, W, kColAcc, ed, i == 0);
-  }
+  Trunk trunk;
+  if (const int rc = take_trunk(c, t, shapes, "backward program", trunk)) return rc;
+  bool ok = add_trunk_steps(c, trunk, forward_only ? EPI_ACT_OUT : EPI_LOADG_TO_A, -1, !forward_only, bld);
   std::vector<float> wt;   // W_l transposed: [in_l, W] row-major (packed inside add_step, so one buffer serves all)
   for (int l = forward_only ? -1 : D - 1; l >= 0 && ok; --l) {
-    const int in = trunk[l].in;
+    const int in = trunk.w[l].in;
     wt.assign((size_t)in * W, 0.f);
     for (int o = 0; o < W; ++o)
-      for (int k = 0; k < in; ++k) wt[(size_t)k * W + o] = trunk[l].w[(size_t)o * in + k];
+      for (int k = 0; k < in; ++k) wt[(size_t)k * W + o] = trunk.w[l].w[(size_t)o * in + k];
     auto grad_out = [&](const float* rows, bool accumulate) {    // embedded-input columns -> output rows
       EpiDesc eo{};
       eo.kind = EPI_GRAD_OUT;
@@ -767,13 +732,28 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
       ok = grad_h(wt.data());
     }
   }
-  if (!ok) return set_error(PNR_ERR_UNSUPPORTED, "backward program: build failed: %s", bld.err.c_str());
-  if ((int)bld.consts.size() > kMaxConsts)
-    return set_error(PNR_ERR_UNSUPPORTED, "backward program: %d constants > %d", (int)bld.consts.size(), kMaxConsts);
-  if (bld.out_of_fp16_range && bld.fmt == kFmtF16)
-    return set_error(PNR_ERR_UNSUPPORTED, "backward program: a weight is outside the fp16 range: use precision bf16x3");
-  bld.prog.n_consts = (int)bld.consts.size();
-  bld.finalize();
+  return bld.finish(ok, "backward program");
+}
+
+// Program `kind` of a network, from the tensors of pnr_load_weights' list (the backward and trunk-forward programs read
+// the trunk's only).
+static int build_program_kind(ProgramKind kind, const pnr_config& c, const float* const* t, const int64_t* shapes,
+                              int32_t n, Builder& bld) {
+  return kind == kProgForward ? build_program(c, t, shapes, n, bld)
+                              : build_backward_program(c, t, shapes, n, bld, kind == kProgTrunkForward);
+}
+
+// Replaces the program's device buffers with the builder's packed stream and constants.
+static int upload(PackedProgram& pp, const Builder& bld) {
+  release(pp);
+  pp.n_w = bld.wbuf.size();
+  pp.n_c = bld.consts.size();
+  PNR_CUDA(cudaMalloc(&pp.d_wpacked, pp.n_w * 2));
+  PNR_CUDA(cudaMalloc(&pp.d_consts, pp.n_c * 4));
+  PNR_CUDA(cudaMemcpy(pp.d_wpacked, bld.wbuf.data(), pp.n_w * 2, cudaMemcpyHostToDevice));
+  PNR_CUDA(cudaMemcpy(pp.d_consts, bld.consts.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
+  pp.launch.prog = bld.prog;
+  pp.ready = true;
   return PNR_OK;
 }
 
@@ -781,34 +761,10 @@ extern "C" int pnr_load_weights(pnr_ctx* ctx, const float* const* t, const int64
   PNR_CHECK_ARG(ctx && t && shapes, "pnr_load_weights: null pointer");
   const pnr_config& c = ctx->cfg;
   Builder bld(ctx->passes, ctx->fmt);
-  const int rc = build_program(c, t, shapes, n, bld);
-  if (rc != PNR_OK) return rc;
-  ctx->has_vp = false;
-  if (c.num_classes == 0 && c.num_instances == 0 && !(getenv("PNR_VIEW_PRODUCERS") && *getenv("PNR_VIEW_PRODUCERS") == '0')) {
-    Builder vp(ctx->passes, ctx->fmt);
-    vp.view_on_producers = true;
-    if (build_program(c, t, shapes, n, vp) == PNR_OK && vp.prog.view_step >= 0 && vp.wbuf == bld.wbuf &&
-        vp.consts == bld.consts) {   // same packed stream and constants: only flags and hand-off counts differ
-      ctx->launch_vp.prog = vp.prog;
-      ctx->has_vp = true;
-    }
-  }
-
+  if (const int rc = build_program(c, t, shapes, n, bld)) return rc;
   DeviceGuard guard(c.device);
-  // (plain cudaFree / cudaMemcpy: they synchronise with the device, so no launch still reads the old buffers)
-  cudaFree(ctx->d_wpacked); cudaFree(ctx->d_consts);
-  ctx->d_wpacked = nullptr; ctx->d_consts = nullptr;
   ctx->loaded = false;
-  ctx->wpacked_bytes = bld.wbuf.size() * 2;
-  PNR_CUDA(cudaMalloc(&ctx->d_wpacked, ctx->wpacked_bytes));
-  PNR_CUDA(cudaMalloc(&ctx->d_consts, bld.consts.size() * 4));
-  ctx->launch.prog = bld.prog;
-  // host copy of the trunk for the backward program (built on the first pnr_mlp_backward_trunk after this load)
-  ctx->bwd.ready = ctx->trunk_fwd.ready = false;
-  for (pnr_ctx::Plan* pl : {&ctx->plan_main, &ctx->plan_bwd, &ctx->plan_tf}) {
-    cudaFree(pl->d_widx); cudaFree(pl->d_wpart); cudaFree(pl->d_cidx);
-    *pl = pnr_ctx::Plan();
-  }
+  for (PackedProgram& pp : ctx->prog) release(pp);   // the backward and trunk-forward programs follow on first use
   cudaFree(ctx->d_V);
   ctx->d_V = nullptr;
   ctx->device_weights = false;
@@ -821,8 +777,7 @@ extern "C" int pnr_load_weights(pnr_ctx* ctx, const float* const* t, const int64
   ctx->host_trunk_shapes.assign(shapes, shapes + 4 * c.D);
   for (int i = 0; i < 2 * c.D; ++i)
     ctx->host_trunk.emplace_back(t[i], t[i] + (size_t)shapes[2 * i] * (size_t)shapes[2 * i + 1]);
-  PNR_CUDA(cudaMemcpy(ctx->d_wpacked, bld.wbuf.data(), ctx->wpacked_bytes, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(ctx->d_consts, bld.consts.data(), bld.consts.size() * 4, cudaMemcpyHostToDevice));
+  if (const int rc = upload(ctx->prog[kProgForward], bld)) return rc;
   ctx->loaded = true;
   return PNR_OK;
 }
@@ -839,9 +794,8 @@ extern "C" int pnr_program_host(const pnr_config* cfg, const float* const* t, co
   if (flags & PNR_PROGRAM_NO_SPLIT) bld.split_e1 = false;
   if (flags & PNR_PROGRAM_SPLIT_E1) bld.split_e1 = true;
   if (flags & PNR_PROGRAM_VIEW_PRODUCERS) bld.view_on_producers = true;
-  const int rc = (flags & PNR_PROGRAM_BACKWARD) ? build_backward_program(*cfg, t, shapes, n, bld)
-                                                : build_program(*cfg, t, shapes, n, bld);
-  if (rc != PNR_OK) return rc;
+  if (const int rc = build_program_kind((flags & PNR_PROGRAM_BACKWARD) ? kProgBackward : kProgForward, *cfg, t, shapes, n, bld))
+    return rc;
   *program_bytes = sizeof(MlpProgram);
   *wpacked_bytes = bld.wbuf.size() * 2;
   *n_consts = bld.consts.size();
@@ -859,9 +813,6 @@ extern "C" int pnr_program_host(const pnr_config* cfg, const float* const* t, co
   }
   return PNR_OK;
 }
-
-static int mlp_forward_impl(pnr_ctx* ctx, const float* pts, const float* viewdirs, const float* rays,
-                            const float* z, int64_t R, int32_t N, float* raw, void* stream, long long* dbg);
 
 extern "C" int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table) {
   PNR_CHECK_ARG(ctx, "pnr_bind_hashgrid_table: null context");
@@ -884,44 +835,40 @@ static int set_trunk_input(const pnr_ctx* ctx, MlpParams& p, const char* what) {
   return PNR_OK;
 }
 
-extern "C" int pnr_debug_timeline(pnr_ctx* ctx, int64_t* timeline) {
-  PNR_CHECK_ARG(ctx, "pnr_debug_timeline: null context");
-  ctx->dbg_timeline = (long long*)timeline;
-  return PNR_OK;
+static int ensure_program(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st);   // below, with the device-side updates
+
+// The checks every fused-MLP launch makes, and the fields every launch of program `kind` sets: its packed stream and
+// constants (built on first use), sample source, sizes, status word and trunk input.  The rest of the launch's
+// MlpParams is zero: each entry point sets its own fields.  Needs the context's device current.
+static int prepare_launch(pnr_ctx* ctx, ProgramKind kind, const char* what, const float* pts, const float* viewdirs,
+                          const float* rays, const float* z, int64_t R, int32_t N, cudaStream_t st, MlpLaunch** out) {
+  if (!ctx->loaded) return set_error(PNR_ERR_STATE, "%s: pnr_load_weights has not been called", what);
+  PNR_CHECK_ARG(R > 0 && N >= 1, "%s: bad sizes R=%lld N=%d", what, (long long)R, N);
+  if (const int rc = ensure_program(ctx, kind, st)) return rc;
+  PackedProgram& pp = ctx->prog[kind];
+  MlpParams& p = pp.launch.p;
+  memset(&p, 0, sizeof(p));
+  p.wpacked = pp.d_wpacked; p.consts = pp.d_consts;
+  p.pts = pts; p.viewdirs = viewdirs; p.rays = rays; p.z = z;
+  p.S = R * (int64_t)N; p.N = N;
+  p.status = ctx->d_status;
+  *out = &pp.launch;
+  return set_trunk_input(ctx, p, what);
 }
 
 extern "C" int pnr_mlp_forward(pnr_ctx* ctx, const float* pts, const float* viewdirs, const float* rays,
                                const float* z, int64_t R, int32_t N, float* raw, void* stream) {
-  return mlp_forward_impl(ctx, pts, viewdirs, rays, z, R, N, raw, stream, nullptr);
-}
-
-extern "C" int pnr_mlp_forward_timeline(pnr_ctx* ctx, const float* rays, const float* z, int64_t R, int32_t N,
-                                        float* raw, int64_t* timeline, void* stream) {
-  return mlp_forward_impl(ctx, nullptr, nullptr, rays, z, R, N, raw, stream, (long long*)timeline);
-}
-
-static int mlp_forward_impl(pnr_ctx* ctx, const float* pts, const float* viewdirs, const float* rays,
-                            const float* z, int64_t R, int32_t N, float* raw, void* stream, long long* dbg) {
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(ctx && raw, "pnr_mlp_forward: null pointer");
-  if (!ctx->loaded) return set_error(PNR_ERR_STATE, "pnr_mlp_forward: pnr_load_weights has not been called");
-  PNR_CHECK_ARG(R >= 0 && N >= 1, "pnr_mlp_forward: bad sizes R=%lld N=%d", (long long)R, N);
   PNR_CHECK_ARG((pts && viewdirs) || (!pts && rays && z), "pnr_mlp_forward: need (pts, viewdirs) or (rays, z)");
-  const int64_t S = R * (int64_t)N;
-  if (S == 0) return PNR_OK;
-  PNR_CHECK_ARG((S + kTileM - 1) / kTileM < (int64_t)1 << 31, "pnr_mlp_forward: too many samples");
-  MlpLaunch& L = ctx->has_vp ? ctx->launch_vp : ctx->launch;
-  MlpParams& p = L.p;
-  memset(&p, 0, sizeof(p));
-  p.wpacked = ctx->d_wpacked; p.consts = ctx->d_consts;
-  p.pts = pts; p.viewdirs = viewdirs; p.rays = rays; p.z = z;
-  p.S = S; p.N = N; p.CH = 4 + ctx->cfg.num_classes + ctx->cfg.num_instances; p.raw = raw;
-  p.num_tiles = (int32_t)((S + kTileM - 1) / kTileM);
-  p.status = ctx->d_status;
-  p.dbg = dbg;
-  if (const int rc = set_trunk_input(ctx, p, "pnr_mlp_forward")) return rc;
   DeviceGuard guard(ctx->cfg.device);   // launch on the context's device whatever the caller's current one is
-  return launch_mlp(L, ctx->passes, ctx->fmt, ctx->has_vp ? kMlpForwardVP : kMlpForward, (cudaStream_t)stream);
+  MlpLaunch* L;
+  if (const int rc = prepare_launch(ctx, kProgForward, "pnr_mlp_forward", pts, viewdirs, rays, z, R, N,
+                                    (cudaStream_t)stream, &L))
+    return rc;
+  L->p.CH = 4 + ctx->cfg.num_classes + ctx->cfg.num_instances;
+  L->p.raw = raw;
+  return launch_mlp(*L, ctx->passes, ctx->fmt, kMlpForward, (cudaStream_t)stream);
 }
 
 extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z, int64_t R, int32_t N,
@@ -930,29 +877,23 @@ extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z
                                  const pnr_composite_out* out, void* stream) {
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(ctx && rays && z && out, "pnr_mlp_composite: null pointer");
-  if (!ctx->loaded) return set_error(PNR_ERR_STATE, "pnr_mlp_composite: pnr_load_weights has not been called");
-  PNR_CHECK_ARG(R > 0 && N >= 1, "pnr_mlp_composite: bad sizes R=%lld N=%d", (long long)R, N);
+  DeviceGuard guard(ctx->cfg.device);
+  MlpLaunch* L;
+  if (const int rc = prepare_launch(ctx, kProgForward, "pnr_mlp_composite", nullptr, nullptr, rays, z, R, N,
+                                    (cudaStream_t)stream, &L))
+    return rc;
   if (N % 32 != 0)
     return set_error(PNR_ERR_UNSUPPORTED, "pnr_mlp_composite: N=%d is not a multiple of 32 (use pnr_mlp_forward + pnr_composite)", N);
   PNR_CHECK_ARG(out->weights, "pnr_mlp_composite: out->weights is required");
   PNR_CHECK_ARG(!mask_outside || sample_box, "pnr_mlp_composite: mask_outside needs sample_box");
   const int C = ctx->cfg.num_classes, K = ctx->cfg.num_instances;
-  const int64_t S = R * (int64_t)N;
-  PNR_CHECK_ARG((S + kTileM - 1) / kTileM < (int64_t)1 << 31, "pnr_mlp_composite: too many samples");
-  MlpParams& p = ctx->launch.p;
-  p.wpacked = ctx->d_wpacked; p.consts = ctx->d_consts;
-  p.pts = nullptr; p.viewdirs = nullptr; p.rays = rays; p.z = z;
-  p.S = S; p.N = N; p.CH = 4 + C + K; p.raw = nullptr;
-  p.num_tiles = (int32_t)((S + kTileM - 1) / kTileM);
-  p.status = ctx->d_status;
-  p.dbg = ctx->dbg_timeline;
+  MlpParams& p = L->p;
+  p.CH = 4 + C + K;
   p.sample_box = sample_box; p.mask_outside = mask_outside; p.white_bkgd = white_bkgd;
   p.C = C; p.K = K;
   p.weights = out->weights; p.rgb_map = out->rgb_map; p.depth_map = out->depth_map; p.acc_map = out->acc_map;
   p.disp_map = out->disp_map; p.sem_map = C > 0 ? out->semantic_map : nullptr; p.inst_map = K > 0 ? out->instance_map : nullptr;
-  if (const int rc = set_trunk_input(ctx, p, "pnr_mlp_composite")) return rc;
-  DeviceGuard guard(ctx->cfg.device);
-  if (const int rc = launch_mlp(ctx->launch, ctx->passes, ctx->fmt, kMlpComposite, (cudaStream_t)stream)) return rc;
+  if (const int rc = launch_mlp(*L, ctx->passes, ctx->fmt, kMlpComposite, (cudaStream_t)stream)) return rc;
   const bool fs = C > 0 && out->fixed_semantic_map && sample_box && box_sem;
   const bool fi = K > 0 && out->fixed_instance_map && sample_box && box_inst;
   if (fs || fi)
@@ -962,8 +903,6 @@ extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z
   return PNR_OK;
 }
 
-
-// Build (once per weight load) the second program `aux` runs and upload its packed weights / constants.
 // ------------------------------------------------------------------------------------------------ device-side updates
 // A training loop changes the weights every step; re-running the host builder (three programs, ~30 ms each) and
 // copying the parameters to the host and back would cost more than the step itself.  The structure of a program does
@@ -973,28 +912,14 @@ extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z
 // fresh pnr_load_weights of the same values (tests/test_gpu_backward.py::test_update_weights_equals_fresh_load).
 namespace {
 
-__device__ __forceinline__ uint16_t dev_f2bf(float x) {   // = the host f2bf (RNE on the bit pattern)
-  const uint32_t u = __float_as_uint(x);
-  return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
-}
-
 __global__ void pack_from_plan_kernel(const float* __restrict__ V, const int32_t* __restrict__ idx,
                                       const uint8_t* __restrict__ part, size_t n, int fmt, uint16_t* __restrict__ out,
                                       uint32_t* status) {
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n) return;
   const float w = idx[p] < 0 ? 0.f : V[idx[p]];
-  uint16_t v;
-  if (fmt == 1) {
-    const uint16_t h = dev_f2bf(w);
-    v = part[p] == 0 ? h : dev_f2bf(w - __uint_as_float((uint32_t)h << 16));
-  } else {
-    if (!(w >= -65504.f && w <= 65504.f) && status != nullptr) atomicOr(status, 2u);   // weight outside the fp16 range
-    const __half h = __float2half_rn(w);
-    const __half r = part[p] == 0 ? h : __float2half_rn(w - __half2float(h));
-    v = __half_as_ushort(r);
-  }
-  out[p] = v;
+  if (fmt == kFmtF16 && !(w >= -65504.f && w <= 65504.f) && status != nullptr) atomicOr(status, 2u);   // weight outside the fp16 range
+  out[p] = weight_part16(w, part[p], fmt);
 }
 
 __global__ void consts_from_plan_kernel(const float* __restrict__ V, const int32_t* __restrict__ idx, size_t n,
@@ -1027,12 +952,12 @@ __global__ void fold_kernel(float* V, int64_t off_view_w, int64_t off_view_b, in
 
 }  // namespace
 
-// which: 0 = the forward program, 1 = backward, 2 = trunk forward.  Index-mode build -> plan on the device.
-static int ensure_plan(pnr_ctx* ctx, pnr_ctx::Plan& plan, int which, size_t expect_w, size_t expect_c) {
-  if (plan.ready) return PNR_OK;
+// The device-side update plan of program `kind`: the program built once more in index mode, whose packed stream and
+// constants name the element of V each entry comes from.
+static int ensure_plan(pnr_ctx* ctx, ProgramKind kind) {
+  PackedProgram& pp = ctx->prog[kind];
+  if (pp.plan_ready) return PNR_OK;
   const int n = (int)ctx->v_off.size();
-  if (ctx->v_total + ctx->v_derived + 1 >= (int64_t)1 << 24)
-    return set_error(PNR_ERR_UNSUPPORTED, "pnr_update_weights: %lld values do not index exactly in fp32", (long long)ctx->v_total);
   std::vector<std::vector<float>> it(n);
   std::vector<const float*> tp(n);
   for (int i = 0; i < n; ++i) {
@@ -1044,32 +969,31 @@ static int ensure_plan(pnr_ctx* ctx, pnr_ctx::Plan& plan, int which, size_t expe
   Builder bld(ctx->passes, ctx->fmt);
   bld.index_mode = true;
   bld.derived_base = ctx->v_total;
-  const int rc = which == 0 ? build_program(ctx->cfg, tp.data(), ctx->all_shapes.data(), n, bld)
-                            : build_backward_program(ctx->cfg, tp.data(), ctx->all_shapes.data(), n, bld, which == 2);
-  if (rc != PNR_OK) return rc;
-  if (bld.wbuf.size() != expect_w || bld.consts.size() != expect_c)
+  if (const int rc = build_program_kind(kind, ctx->cfg, tp.data(), ctx->all_shapes.data(), n, bld)) return rc;
+  if (bld.wbuf.size() != pp.n_w || bld.consts.size() != pp.n_c)
     return set_error(PNR_ERR_STATE, "pnr_update_weights: plan / program size mismatch (%zu/%zu vs %zu/%zu)", bld.wbuf.size(),
-                     bld.consts.size(), expect_w, expect_c);
-  std::vector<int32_t> widx(bld.wsrc.size()), cidx(bld.consts.size());
+                     bld.consts.size(), pp.n_w, pp.n_c);
+  std::vector<int32_t> widx(pp.n_w), cidx(pp.n_c);
   for (size_t i = 0; i < widx.size(); ++i) widx[i] = (int32_t)bld.wsrc[i] - 1;
   for (size_t i = 0; i < cidx.size(); ++i) cidx[i] = (int32_t)bld.consts[i] - 1;
-  plan.n_w = widx.size();
-  plan.n_c = cidx.size();
-  PNR_CUDA(cudaMalloc(&plan.d_widx, plan.n_w * 4));
-  PNR_CUDA(cudaMalloc(&plan.d_wpart, plan.n_w));
-  PNR_CUDA(cudaMalloc(&plan.d_cidx, plan.n_c * 4));
-  PNR_CUDA(cudaMemcpy(plan.d_widx, widx.data(), plan.n_w * 4, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(plan.d_wpart, bld.wpart.data(), plan.n_w, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(plan.d_cidx, cidx.data(), plan.n_c * 4, cudaMemcpyHostToDevice));
-  plan.ready = true;
+  PNR_CUDA(cudaMalloc(&pp.d_widx, pp.n_w * 4));
+  PNR_CUDA(cudaMalloc(&pp.d_wpart, pp.n_w));
+  PNR_CUDA(cudaMalloc(&pp.d_cidx, pp.n_c * 4));
+  PNR_CUDA(cudaMemcpy(pp.d_widx, widx.data(), pp.n_w * 4, cudaMemcpyHostToDevice));
+  PNR_CUDA(cudaMemcpy(pp.d_wpart, bld.wpart.data(), pp.n_w, cudaMemcpyHostToDevice));
+  PNR_CUDA(cudaMemcpy(pp.d_cidx, cidx.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
+  pp.plan_ready = true;
   return PNR_OK;
 }
 
-static int repack_from_V(pnr_ctx* ctx, pnr_ctx::Plan& plan, uint8_t* d_wpacked, float* d_consts, cudaStream_t st) {
-  pack_from_plan_kernel<<<(unsigned)((plan.n_w + 255) / 256), 256, 0, st>>>(ctx->d_V, plan.d_widx, plan.d_wpart, plan.n_w, ctx->fmt,
-                                                                              reinterpret_cast<uint16_t*>(d_wpacked), ctx->d_status);
+// Packs program `kind`'s stream and constants from the weights in V, on `st`.
+static int refresh(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st) {
+  if (const int rc = ensure_plan(ctx, kind)) return rc;
+  const PackedProgram& pp = ctx->prog[kind];
+  pack_from_plan_kernel<<<(unsigned)((pp.n_w + 255) / 256), 256, 0, st>>>(ctx->d_V, pp.d_widx, pp.d_wpart, pp.n_w, ctx->fmt,
+                                                                          reinterpret_cast<uint16_t*>(pp.d_wpacked), ctx->d_status);
   PNR_LAUNCH_CHECK("pack_from_plan_kernel");
-  consts_from_plan_kernel<<<(unsigned)((plan.n_c + 255) / 256), 256, 0, st>>>(ctx->d_V, plan.d_cidx, plan.n_c, d_consts);
+  consts_from_plan_kernel<<<(unsigned)((pp.n_c + 255) / 256), 256, 0, st>>>(ctx->d_V, pp.d_cidx, pp.n_c, pp.d_consts);
   PNR_LAUNCH_CHECK("consts_from_plan_kernel");
   return PNR_OK;
 }
@@ -1079,10 +1003,11 @@ extern "C" int pnr_update_weights(pnr_ctx* ctx, const float* const* device_tenso
   if (!ctx->loaded) return set_error(PNR_ERR_STATE, "pnr_update_weights: pnr_load_weights has not been called (it fixes the shapes)");
   PNR_CHECK_ARG(n == (int)ctx->v_off.size(), "pnr_update_weights: got %d tensors, pnr_load_weights had %d", n, (int)ctx->v_off.size());
   for (int i = 0; i < n; ++i) PNR_CHECK_ARG(device_tensors[i], "pnr_update_weights: tensor %d is null", i);
+  if (ctx->v_total + ctx->v_derived + 1 >= (int64_t)1 << 24)   // the plans index V through fp32 values
+    return set_error(PNR_ERR_UNSUPPORTED, "pnr_update_weights: %lld values do not index exactly in fp32", (long long)ctx->v_total);
   DeviceGuard guard(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
   if (!ctx->d_V) PNR_CUDA(cudaMalloc(&ctx->d_V, (size_t)(ctx->v_total + ctx->v_derived) * 4));
-  if (const int rc = ensure_plan(ctx, ctx->plan_main, 0, ctx->wpacked_bytes / 2, (size_t)ctx->launch.prog.n_consts)) return rc;
   for (int i = 0; i < n; ++i)
     PNR_CUDA(cudaMemcpyAsync(ctx->d_V + ctx->v_off[i], device_tensors[i],
                              (size_t)(ctx->all_shapes[2 * i] * ctx->all_shapes[2 * i + 1]) * 4, cudaMemcpyDeviceToDevice, st));
@@ -1094,74 +1019,24 @@ extern "C" int pnr_update_weights(pnr_ctx* ctx, const float* const* device_tenso
   fold_kernel<<<(W2 * (W + Ed + 1) + 127) / 128, 128, 0, st>>>(ctx->d_V, off_view_w, off_view_b, off_feat_w, off_feat_b, W, W2, Ed,
                                                                off_fold, off_fold_b);
   PNR_LAUNCH_CHECK("fold_kernel");
-  if (const int rc = repack_from_V(ctx, ctx->plan_main, ctx->d_wpacked, ctx->d_consts, st)) return rc;
   ctx->device_weights = true;
-  // the aux programs that exist follow; the others are packed from V when they are first built
-  if (ctx->bwd.ready) {
-    if (const int rc = ensure_plan(ctx, ctx->plan_bwd, 1, ctx->bwd.n_w, ctx->bwd.n_c)) return rc;
-    if (const int rc = repack_from_V(ctx, ctx->plan_bwd, ctx->bwd.d_wpacked, ctx->bwd.d_consts, st)) return rc;
-  }
-  if (ctx->trunk_fwd.ready) {
-    if (const int rc = ensure_plan(ctx, ctx->plan_tf, 2, ctx->trunk_fwd.n_w, ctx->trunk_fwd.n_c)) return rc;
-    if (const int rc = repack_from_V(ctx, ctx->plan_tf, ctx->trunk_fwd.d_wpacked, ctx->trunk_fwd.d_consts, st)) return rc;
-  }
+  // the programs that exist follow; the others are packed from V when they are first built
+  for (int k = 0; k < kNumPrograms; ++k)
+    if (ctx->prog[k].ready)
+      if (const int rc = refresh(ctx, (ProgramKind)k, st)) return rc;
   return PNR_OK;
 }
 
-static int ensure_aux(pnr_ctx* ctx, pnr_ctx::Aux& aux, bool forward_only, cudaStream_t st) {
-  if (aux.ready) return PNR_OK;
+static int ensure_program(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st) {
+  if (ctx->prog[kind].ready) return PNR_OK;   // the forward program always is: pnr_load_weights builds it
   Builder bld(ctx->passes, ctx->fmt);
   std::vector<const float*> tp;
   for (const auto& v : ctx->host_trunk) tp.push_back(v.data());
-  if (const int rc = build_backward_program(ctx->cfg, tp.data(), ctx->host_trunk_shapes.data(), (int32_t)tp.size(), bld,
-                                            forward_only))
+  if (const int rc = build_program_kind(kind, ctx->cfg, tp.data(), ctx->host_trunk_shapes.data(), (int32_t)tp.size(), bld))
     return rc;
-  cudaFree(aux.d_wpacked); cudaFree(aux.d_consts);
-  aux.d_wpacked = nullptr; aux.d_consts = nullptr;
-  PNR_CUDA(cudaMalloc(&aux.d_wpacked, bld.wbuf.size() * 2));
-  PNR_CUDA(cudaMalloc(&aux.d_consts, bld.consts.size() * 4));
-  PNR_CUDA(cudaMemcpy(aux.d_wpacked, bld.wbuf.data(), bld.wbuf.size() * 2, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(aux.d_consts, bld.consts.data(), bld.consts.size() * 4, cudaMemcpyHostToDevice));
-  memset(&aux.launch.p, 0, sizeof(MlpParams));
-  aux.launch.prog = bld.prog;
-  aux.n_w = bld.wbuf.size();
-  aux.n_c = bld.consts.size();
-  aux.ready = true;
-  if (ctx->device_weights) {   // the host copies are older than the weights in V: pack this program from V
-    pnr_ctx::Plan& plan = forward_only ? ctx->plan_tf : ctx->plan_bwd;
-    if (const int rc = ensure_plan(ctx, plan, forward_only ? 2 : 1, aux.n_w, aux.n_c)) return rc;
-    return repack_from_V(ctx, plan, aux.d_wpacked, aux.d_consts, st);
-  }
-  return PNR_OK;
-}
-
-static int aux_launch(pnr_ctx* ctx, pnr_ctx::Aux& aux, const char* what, const float* pts, const float* rays, const float* z,
-                      int64_t R, int32_t N, const float* grad_h, float grad_scale, float* out, int32_t ld_out, float* stash,
-                      uint32_t* stash_absmax, void* stream) {
-  if (!ctx->loaded) return set_error(PNR_ERR_STATE, "%s: pnr_load_weights has not been called", what);
-  PNR_CHECK_ARG(R > 0 && N >= 1, "%s: bad sizes R=%lld N=%d", what, (long long)R, N);
-  PNR_CHECK_ARG(pts || (rays && z), "%s: need pts or (rays, z)", what);
-  const int64_t S = R * (int64_t)N;
-  PNR_CHECK_ARG((S + kTileM - 1) / kTileM < (int64_t)1 << 31, "%s: too many samples", what);
-  PNR_CHECK_ARG(stash == nullptr || (reinterpret_cast<uintptr_t>(stash) & 15) == 0, "%s: stash must be 16-byte aligned", what);
-  DeviceGuard guard(ctx->cfg.device);
-  if (const int rc = ensure_aux(ctx, aux, grad_h == nullptr, (cudaStream_t)stream)) return rc;
-  MlpParams& p = aux.launch.p;
-  p.wpacked = aux.d_wpacked; p.consts = aux.d_consts;
-  p.pts = pts; p.viewdirs = nullptr; p.rays = rays; p.z = z;
-  p.S = S; p.N = N; p.CH = ld_out; p.raw = out;
-  p.num_tiles = (int32_t)((S + kTileM - 1) / kTileM);
-  p.status = ctx->d_status;
-  p.dbg = ctx->dbg_timeline;
-  p.grad_in = grad_h;
-  p.stash = stash;
-  p.stash_absmax = stash_absmax;
-  if (stash_absmax != nullptr)
-    PNR_CUDA(cudaMemsetAsync(stash_absmax, 0, sizeof(uint32_t) * (size_t)(2 * ctx->cfg.D - 1), (cudaStream_t)stream));
-  p.grad_scale = grad_scale;
-  p.grad_unscale = 1.0f / grad_scale;
-  if (const int rc = set_trunk_input(ctx, p, what)) return rc;
-  return launch_mlp(aux.launch, ctx->passes, ctx->fmt, kMlpBackward, (cudaStream_t)stream);
+  if (const int rc = upload(ctx->prog[kind], bld)) return rc;
+  // the host copies are older than the weights in V: pack this program from V
+  return ctx->device_weights ? refresh(ctx, kind, st) : PNR_OK;
 }
 
 // dL/d(embedded xyz) through the trunk (the tensor-core part of the MLP backward, SURVEY 8f rank 2): the forward
@@ -1185,8 +1060,24 @@ extern "C" int pnr_mlp_backward_trunk(pnr_ctx* ctx, const float* pts, const floa
   PNR_CHECK_ARG(grad_scale > 0.f && grad_scale < 1.0e30f && grad_scale > 1.0e-30f && frexpf(grad_scale, &gexp) == 0.5f,
                 "pnr_mlp_backward_trunk: grad_scale=%g must be a positive power of two", (double)grad_scale);
   PNR_CHECK_ARG(stash_absmax == nullptr || stash != nullptr, "pnr_mlp_backward_trunk: stash_absmax without a stash");
-  return aux_launch(ctx, ctx->bwd, "pnr_mlp_backward_trunk", pts, rays, z, R, N, grad_h, grad_scale, grad_emb, ld_emb, stash,
-                    stash_absmax, stream);
+  PNR_CHECK_ARG(pts || (rays && z), "pnr_mlp_backward_trunk: need pts or (rays, z)");
+  PNR_CHECK_ARG(stash == nullptr || (reinterpret_cast<uintptr_t>(stash) & 15) == 0,
+                "pnr_mlp_backward_trunk: stash must be 16-byte aligned");
+  DeviceGuard guard(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  MlpLaunch* L;
+  if (const int rc = prepare_launch(ctx, kProgBackward, "pnr_mlp_backward_trunk", pts, nullptr, rays, z, R, N, st, &L))
+    return rc;
+  MlpParams& p = L->p;
+  p.CH = ld_emb; p.raw = grad_emb;
+  p.grad_in = grad_h;
+  p.stash = stash;
+  p.stash_absmax = stash_absmax;
+  if (stash_absmax != nullptr)
+    PNR_CUDA(cudaMemsetAsync(stash_absmax, 0, sizeof(uint32_t) * (size_t)(2 * ctx->cfg.D - 1), st));
+  p.grad_scale = grad_scale;
+  p.grad_unscale = 1.0f / grad_scale;
+  return launch_mlp(*L, ctx->passes, ctx->fmt, kMlpBackward, st);
 }
 
 // The trunk's output activations h [R*N, W] (what alpha_linear, feature_linear and the heads read): the forward
@@ -1197,7 +1088,15 @@ extern "C" int pnr_mlp_trunk_forward(pnr_ctx* ctx, const float* pts, const float
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(ctx && h_out, "pnr_mlp_trunk_forward: null pointer");
   PNR_CHECK_ARG((reinterpret_cast<uintptr_t>(h_out) & 15) == 0, "pnr_mlp_trunk_forward: h_out must be 16-byte aligned");
-  return aux_launch(ctx, ctx->trunk_fwd, "pnr_mlp_trunk_forward", pts, rays, z, R, N, nullptr, 1.0f, h_out, ctx->cfg.W, nullptr, nullptr, stream);
+  PNR_CHECK_ARG(pts || (rays && z), "pnr_mlp_trunk_forward: need pts or (rays, z)");
+  DeviceGuard guard(ctx->cfg.device);
+  cudaStream_t st = (cudaStream_t)stream;
+  MlpLaunch* L;
+  if (const int rc = prepare_launch(ctx, kProgTrunkForward, "pnr_mlp_trunk_forward", pts, nullptr, rays, z, R, N, st, &L))
+    return rc;
+  L->p.CH = ctx->cfg.W; L->p.raw = h_out;
+  L->p.grad_scale = L->p.grad_unscale = 1.0f;
+  return launch_mlp(*L, ctx->passes, ctx->fmt, kMlpBackward, st);
 }
 
 namespace pnr {

@@ -140,7 +140,7 @@ class Network(nn.Module):
         return ctx
 
     def _pack(self, device=None) -> int:
-        """(Re)build the libpnr context: weights are split into 16-bit hi/lo UMMA stage images (fp16 or bf16 per cfg.precision) once, and
+        """(Re)build the libpnr context: weights are split into 16-bit hi/lo wgmma stage images (fp16 or bf16 per cfg.precision; csrc/mlp_program.h) once, and
         again only when a parameter changed (SURVEY.md section 5, 'weight packer')."""
         device = torch.device(device if device is not None else next(self.parameters()).device)
         if device.type != "cuda":

@@ -6,10 +6,10 @@ The work is split where the network splits:
     the layers in reverse with the transposed weight stream and keeps every operand of the weight-gradient GEMMs
     (activations H_i, pre-activation gradients dZ_j) in one fp32 stash;
   * every weight / bias gradient - the trunk's dW_j = dZ_j^T H_{j-1} on that stash and those of the layers after the
-    trunk - is a split-K GEMM over the samples on the tensor cores (`wgrad` -> pnr_wgrad, csrc/wgrad_tc05.cu);
+    trunk - is a split-K GEMM over the samples on the tensor cores (`wgrad` -> pnr_wgrad, csrc/wgrad_wgmma.cu);
   * the layers after the trunk (alpha / feature / view / rgb / the two heads: small GEMMs with K <= W) are
     differentiated layer by layer by autograd on h, each node's forward and input-gradient GEMM on `linear3x` ->
-    pnr_linear (csrc/linear_tc05.cu).  No library GEMM is left on this path.
+    pnr_linear (csrc/linear_wgmma.cu).  No library GEMM is left on this path.
 Nothing here imports the oracle; tests compare every parameter's gradient with autograd through the oracle network."""
 from __future__ import annotations
 
@@ -102,7 +102,7 @@ def linear3x(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor]
              transposed: bool = False, precision: str = "fp16x3", scale: Optional[torch.Tensor] = None,
              out_cols: int = 0) -> torch.Tensor:
     """act(x @ weight.T + bias) [S, N] for x [S, K], weight [N, K] - or x @ weight for weight [K, N] with
-    transposed=True (the input gradient of a linear layer) - on the tensor cores (pnr_linear, csrc/linear_tc05.cu:
+    transposed=True (the input gradient of a linear layer) - on the tensor cores (pnr_linear, csrc/linear_wgmma.cu:
     16-bit hi / lo operand parts, hi.hi + lo.hi + hi.lo, fp32 accumulation).  K <= 512; more than 256 outputs run as
     one call per 256-column block of the result.
     scale: device scalar power of two applied to x inside the kernel and removed from the result (gradients).
