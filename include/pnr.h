@@ -415,6 +415,39 @@ int pnr_comm_init(pnr_comm** out, const uint8_t* id, int32_t rank, int32_t world
 int pnr_comm_destroy(pnr_comm* comm);
 int pnr_allgather_outputs(pnr_comm* comm, const void* send, void* recv, size_t bytes_per_rank, void* stream);
 
+/* Evaluation of rendered frames against their ground truth (the step after pnr_panoptic_fuse; the reference's
+ * evaluator is not in the mount, so these rules are chosen here - DESIGN.md 3.4, oracle/reference_eval.py).
+ * Ids are panoptic ids id*1000 + n, as pnr_panoptic_fuse writes them and KITTI-360's 2D instance images store them.
+ * An id's class channel: a negative id is void; otherwise the dataset id d = id / 1000 maps to
+ * id_to_channel[d] (DEVICE [n_ids] i32) when the table is given - void when d >= n_ids or the entry is outside
+ * [0, C) - and to d itself when d < C without a table (void otherwise).  C in [1, 64]; n < 2^31.
+ * Every accumulator ACCUMULATES (zero it first); counts are exact integers and every floating-point result is
+ * deterministic (no float atomics), so the same inputs give bit-identical accumulators. */
+/* conf [C, C+1] u64 += pixels by (gt channel, prediction channel) over the pixels whose gt channel is not void;
+ * column C counts predictions that map to no channel.  IoU_c = conf[c,c] / (row_c + col_c - conf[c,c]). */
+int pnr_eval_semantic(const int32_t* pred_pan, const int32_t* gt_pan, int64_t n, int32_t C,
+                      const int32_t* id_to_channel, int32_t n_ids, uint64_t* conf, void* stream);
+/* Panoptic quality of one frame (Kirillov et al. 2019, with the void / crowd handling of the COCO / Cityscapes
+ * panoptic tools): segments are the distinct non-void ids; a gt pixel of channel -1 is void; a gt segment of a thing
+ * class (is_thing [C] u8) with n == 0 is a crowd region.  A prediction and a gt of the same channel match when
+ * IoU > 0.5 (exactly 0.5 does not), union = area_p + area_g - inter - |p ∩ void|.  Per channel c:
+ * tp[c], fp[c], fn[c] u64 += the frame's matches, unmatched predictions (except those with
+ * (|p ∩ void| + |p ∩ crowd of c|) / area_p > 0.5) and unmatched non-crowd gt segments; iou_sum[c] (double) += the
+ * frame's matched IoUs, summed exactly and rounded once (so equal to math.fsum of them).
+ * workspace: pnr_eval_workspace_bytes(n) bytes of device scratch, 16-byte aligned (hash tables of >= 2n slots, so
+ * they cannot fill; a smaller workspace is rejected before any launch). */
+size_t pnr_eval_workspace_bytes(int64_t n);
+int pnr_eval_panoptic(const int32_t* pred_pan, const int32_t* gt_pan, int64_t n, int32_t C,
+                      const int32_t* id_to_channel, int32_t n_ids, const uint8_t* is_thing, void* workspace,
+                      size_t workspace_bytes, uint64_t* tp, uint64_t* fp, uint64_t* fn, double* iou_sum, void* stream);
+/* Image and depth error sums of one frame, in double from the fp32 maps: frame_sums [6] +=
+ * {sum over pixels and channels of (rgb_map - rgb_gt)^2 [n,3], pixels, then over the pixels with depth_gt > 0:
+ * sum |d|, sum d^2, sum |d| / depth_gt, pixels} with d = depth_map - depth_gt.  Either pair may be NULL (its sums are
+ * left alone).  Fixed-shape reductions: block trees over a grid that depends on n only, then one fixed tree.
+ * workspace: any buffer of pnr_eval_workspace_bytes(n) bytes (any n) works. */
+int pnr_eval_image(const float* rgb_map, const float* rgb_gt, const float* depth_map, const float* depth_gt,
+                   int64_t n, double* frame_sums, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Number of kernels this library has launched on this thread since the last reset (bench evidence). */
 int64_t pnr_launch_count(int32_t reset);
 

@@ -124,6 +124,10 @@ SIGNATURES = {
     "pnr_comm_destroy": (C.c_int, [_vp]),
     "pnr_allgather_outputs": (C.c_int, [_vp, _vp, _vp, C.c_size_t, _vp]),
     "pnr_launch_count": (_i64, [_i32]),
+    "pnr_eval_workspace_bytes": (C.c_size_t, [_i64]),
+    "pnr_eval_semantic": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _i32, _vp, _vp]),
+    "pnr_eval_panoptic": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _i32, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp, _vp]),
+    "pnr_eval_image": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp, C.c_size_t, _vp]),
 }
 
 

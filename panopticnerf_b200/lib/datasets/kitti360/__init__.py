@@ -6,7 +6,8 @@ from .calib import (load_cam0_to_world, load_cam_to_pose, load_fisheye_yaml, loa
                     perspective_batch, fisheye_batch)
 from .bboxes import Box3D, boxes_to_primitives, parse_bboxes_xml, primitive_batch
 from .intersection_cache import load_intersections, save_intersections
+from .groundtruth import load_panoptic_gt, load_semantic_gt
 
 __all__ = ["load_cam0_to_world", "load_cam_to_pose", "load_fisheye_yaml", "load_perspective", "load_poses",
            "perspective_batch", "fisheye_batch", "Box3D", "boxes_to_primitives", "parse_bboxes_xml",
-           "primitive_batch", "load_intersections", "save_intersections"]
+           "primitive_batch", "load_intersections", "save_intersections", "load_panoptic_gt", "load_semantic_gt"]
