@@ -56,7 +56,10 @@ constexpr int kConsumerThreads = 128;     // one warpgroup: MMAs, positional enc
 constexpr int kMlpThreads = kConsumerThreads + 32;   // + the weight-stream warp
 constexpr int kMaxStages = 256;
 constexpr int kMaxSteps = 24;
-constexpr int kMaxConsts = 4096;          // floats: biases + sigma / rgb weights
+// floats: biases + sigma / rgb weights.  They live in global memory (MlpParams::consts); the bound is what the uint16_t
+// offsets of EpiDesc can address: a table of at most 65536 floats starts every block at an offset <= 65535.
+constexpr int kMaxConsts = 65536;
+static_assert(kMaxConsts - 1 <= 0xFFFF, "EpiDesc::bias_off / aux_off are uint16_t");
 
 // Operand column map.  The program addresses its A operands as "packed columns" of 32 bits (two 16-bit values of
 // consecutive K) - 512 of them per row, the first 256 being accumulator space.
