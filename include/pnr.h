@@ -186,6 +186,7 @@ int pnr_label_tiles(const float* rgb_map, const float* depth_map, const float* s
  *                logits (sem_is_prob = 0), -log(max(p_label, eps)) when it holds rendered probabilities - times
  *                label_weight[r] (optional confidence)
  *   fixed        -log(max(fixed_semantic_map[label], eps)) * label_weight
+ *                (the gradient of max(p, eps) passes at p == eps, as torch.clamp_min's does)
  * per_ray [R,4] receives the four unweighted values; the caller sums them.  Every gradient is already multiplied by
  * the term's weight w_* and normaliser inv_n_* (1 / number of elements or valid rays, which the caller knows), i.e.
  * it is dL/dmap of L = w_rgb*mean_rgb + w_depth*mean_depth + w_sem*mean_sem + w_fix*mean_fix, ready for

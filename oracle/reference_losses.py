@@ -14,8 +14,9 @@ import torch.nn.functional as F
 def losses(rgb_map, rgb_map0, depth_map, semantic_map, fixed_semantic_map, rgb_gt, depth_gt, label, label_weight=None,
            weights=(1.0, 0.1, 1.0, 1.0), sem_is_prob: bool = False, eps: float = 1e-8):
     """Returns (total, terms[4]) with terms = (rgb, depth, sem, fix) means."""
-    zero = torch.zeros((), dtype=torch.float32)
-    R = next(t for t in (rgb_map, depth_map, semantic_map, fixed_semantic_map) if t is not None).shape[0]
+    ref = next(t for t in (rgb_map, depth_map, semantic_map, fixed_semantic_map) if t is not None)
+    R, dt = ref.shape[0], ref.dtype
+    zero = torch.zeros((), dtype=dt)
     l_rgb = zero
     if rgb_map is not None:
         l_rgb = l_rgb + ((rgb_map - rgb_gt) ** 2).sum() / (3 * R)
@@ -31,7 +32,7 @@ def losses(rgb_map, rgb_map0, depth_map, semantic_map, fixed_semantic_map, rgb_g
         has = (label >= 0) & (label < Cn)
         n = max(int(has.sum()), 1)
         lab = label.clamp(0, Cn - 1).long()
-        conf = label_weight if label_weight is not None else torch.ones(R)
+        conf = label_weight if label_weight is not None else torch.ones(R, dtype=dt)
         if semantic_map is not None:
             if sem_is_prob:
                 p = semantic_map.gather(1, lab[:, None])[:, 0]
@@ -42,4 +43,4 @@ def losses(rgb_map, rgb_map0, depth_map, semantic_map, fixed_semantic_map, rgb_g
             p = fixed_semantic_map.gather(1, lab[:, None])[:, 0]
             l_fix = (-torch.log(torch.clamp_min(p, eps)) * conf * has).sum() / n
     terms = torch.stack([l_rgb, l_depth, l_sem, l_fix])
-    return (terms * torch.tensor(weights, dtype=torch.float32)).sum(), terms
+    return (terms * torch.tensor(weights, dtype=dt)).sum(), terms

@@ -303,8 +303,8 @@ def raw2outputs_backward(raw, z_vals, rays_d, grads: Dict[str, torch.Tensor], wh
     tests/test_cpu_backward.py pins it against autograd through `raw2outputs`."""
     C, K = num_classes, num_instances
     R, N = z_vals.shape
-    zero = torch.zeros(())
-    g = lambda k, shape: grads[k] if k in grads and grads[k] is not None else torch.zeros(shape)
+    zero = torch.zeros((), dtype=raw.dtype)
+    g = lambda k, shape: grads[k] if k in grads and grads[k] is not None else torch.zeros(shape, dtype=raw.dtype)
     dists = torch.cat([z_vals[:, 1:] - z_vals[:, :-1], torch.full_like(z_vals[:, :1], 1e10)], -1)
     dists = dists * torch.norm(rays_d[:, None, :], dim=-1)
     live = raw[..., 3] > 0
@@ -332,22 +332,31 @@ def raw2outputs_backward(raw, z_vals, rays_d, grads: Dict[str, torch.Tensor], wh
         d_raw[..., 4 + C:4 + C + K] = w[..., None] * gi[:, None]
     for key, table, n in (("fixed_semantic_map", box_sem, C), ("fixed_instance_map", box_inst, K)):
         if sample_box is not None and table is not None and n > 0 and grads.get(key) is not None:
-            ids = torch.where(sample_box >= 0, table.to(torch.int64)[sample_box.clamp(min=0).to(torch.int64)],
-                              torch.full_like(sample_box, -1, dtype=torch.int64))
+            ids = _box_ids(sample_box, table)
             ok = (ids >= 0) & (ids < n)
             G = G + torch.where(ok, torch.gather(grads[key], 1, ids.clamp(0, n - 1)), torch.zeros_like(G))
     Gw = G * w
-    S = torch.flip(torch.cumsum(torch.flip(Gw, [-1]), -1), [-1]) - Gw        # strictly later samples
+    # strictly later samples, summed without subtracting Gw_i (which cancels behind a surface, where S / t is large)
+    S = torch.cat([torch.flip(torch.cumsum(torch.flip(Gw[:, 1:], [-1]), -1), [-1]), torch.zeros_like(Gw[:, :1])], -1)
     d_raw[..., 3] = (G * T - S / t) * torch.where(live, dists * e, torch.zeros_like(e))
     return d_raw
 
 
+def _box_ids(sample_box, table):
+    """table[sample_box_i] per sample, -1 where the sample is in no box: sample_box < 0 or >= len(table)."""
+    B = table.shape[0]
+    inside = (sample_box >= 0) & (sample_box < B)
+    idx = sample_box.clamp(0, max(B - 1, 0)).to(torch.int64)
+    looked = table.to(torch.int64)[idx] if B > 0 else torch.zeros_like(idx)
+    return torch.where(inside, looked, torch.full_like(idx, -1))
+
+
 def _composite_onehot(weights, sample_box, table, n):
-    """sum_i w_i * onehot(table[sample_box_i]) ; samples with box -1 or an id outside [0,n) add nothing."""
-    ids = torch.where(sample_box >= 0, table.to(torch.int64)[sample_box.clamp(min=0).to(torch.int64)],
-                      torch.full_like(sample_box, -1, dtype=torch.int64))
+    """sum_i w_i * onehot(table[sample_box_i]) ; samples in no box (sample_box < 0 or >= len(table)) or with an id
+    outside [0,n) add nothing."""
+    ids = _box_ids(sample_box, table)
     valid = (ids >= 0) & (ids < n)
-    out = torch.zeros(weights.shape[0], n + 1)
+    out = torch.zeros(weights.shape[0], n + 1, dtype=weights.dtype)
     out.scatter_add_(1, torch.where(valid, ids, torch.full_like(ids, n)), weights)
     return out[:, :n].contiguous()
 

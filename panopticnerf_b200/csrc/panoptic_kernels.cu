@@ -195,7 +195,8 @@ extern "C" int pnr_hashgrid_encode(const float* x, int64_t n, const float* aabb,
   PNR_CHECK_ARG(L >= 1 && L <= 32 && (F == 1 || F == 2 || F == 4 || F == 8), "pnr_hashgrid_encode: L=%d F=%d (L in [1,32], F in {1,2,4,8})", L, F);
   PNR_CHECK_ARG(T_log2 >= 4 && T_log2 <= 28, "pnr_hashgrid_encode: T_log2=%d outside [4,28]", T_log2);
   PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "pnr_hashgrid_encode: base_resolution / per_level_scale < 1");
-  PNR_CHECK_ARG((double)base_resolution * pow((double)per_level_scale, (double)(L - 1)) < 1048576.0, "pnr_hashgrid_encode: finest resolution >= 2^20");
+  const double finest = (double)base_resolution * pow((double)per_level_scale, (double)(L - 1));
+  PNR_CHECK_ARG(finest < 1048576.0, "pnr_hashgrid_encode: finest resolution %.0f >= 2^20", finest);
   HashArgs a{x, n, table, out, aabb, L, F, T_log2, {}};
   hash_level_resolutions(L, base_resolution, per_level_scale, a.res);
   const int lpt = 8 / F;   // levels per thread: 8 output features = one 32-byte sector
@@ -218,7 +219,8 @@ extern "C" int pnr_hashgrid_backward(const float* x, int64_t n, const float* aab
   PNR_CHECK_ARG(L >= 1 && L <= 32 && (F == 1 || F == 2 || F == 4 || F == 8), "pnr_hashgrid_backward: L=%d F=%d (L in [1,32], F in {1,2,4,8})", L, F);
   PNR_CHECK_ARG(T_log2 >= 4 && T_log2 <= 28, "pnr_hashgrid_backward: T_log2=%d outside [4,28]", T_log2);
   PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "pnr_hashgrid_backward: base_resolution / per_level_scale < 1");
-  PNR_CHECK_ARG((double)base_resolution * pow((double)per_level_scale, (double)(L - 1)) < 1048576.0, "pnr_hashgrid_backward: finest resolution >= 2^20");
+  const double finest = (double)base_resolution * pow((double)per_level_scale, (double)(L - 1));
+  PNR_CHECK_ARG(finest < 1048576.0, "pnr_hashgrid_backward: finest resolution %.0f >= 2^20", finest);
   HashArgs a{x, n, nullptr, nullptr, aabb, L, F, T_log2, {}};
   hash_level_resolutions(L, base_resolution, per_level_scale, a.res);
   const int lpt = 8 / F;
@@ -293,13 +295,14 @@ __global__ void __launch_bounds__(256) losses_kernel(LossArgs L) {
   // 2D pseudo-label cross-entropy on the rendered semantics
   if (a.semantic_map != nullptr && a.C > 0) {
     const float* s = a.semantic_map + r * a.C;
-    if (a.sem_is_prob) {     // the map is a rendered probability: -log(max(p_label, eps))
+    // the map is a rendered probability: -log(max(p_label, eps)); the gradient passes at p == eps, as torch.clamp_min's
+    if (a.sem_is_prob) {
       const float p = has ? s[label] : 1.0f;
       const float pc = fmaxf(p, a.eps);
       l_sem = has ? -logf(pc) * conf : 0.f;
       if (a.d_semantic_map)
         for (int c = lane; c < a.C; c += 32)
-          a.d_semantic_map[r * a.C + c] = (has && c == label && p > a.eps) ? -conf * a.w_sem * a.inv_n_sem / pc : 0.f;
+          a.d_semantic_map[r * a.C + c] = (has && c == label && p >= a.eps) ? -conf * a.w_sem * a.inv_n_sem / pc : 0.f;
     } else {                 // the map is rendered logits: softmax cross-entropy
       float m = -INFINITY;
       for (int c = lane; c < a.C; c += 32) m = fmaxf(m, s[c]);
@@ -307,11 +310,13 @@ __global__ void __launch_bounds__(256) losses_kernel(LossArgs L) {
       float z = 0.f;
       for (int c = lane; c < a.C; c += 32) z += expf(s[c] - m);
       z = warp_add(z);
-      const float lse = m + logf(z);
-      l_sem = has ? (lse - s[label]) * conf : 0.f;
+      // lse - s[label] and softmax = exp(s - lse) are not formed through lse = m + log(z): with logits of ~1e4, lse
+      // rounds at ~1e-3 and that error would go straight into the loss and every probability.  m - s[c] is exact
+      // or rounded relative to itself, so both stay within a few ulps of their own value.
+      l_sem = has ? ((m - s[label]) + logf(z)) * conf : 0.f;
       if (a.d_semantic_map)
         for (int c = lane; c < a.C; c += 32)
-          a.d_semantic_map[r * a.C + c] = has ? (expf(s[c] - lse) - (c == label ? 1.f : 0.f)) * conf * a.w_sem * a.inv_n_sem : 0.f;
+          a.d_semantic_map[r * a.C + c] = has ? (expf(s[c] - m) / z - (c == label ? 1.f : 0.f)) * conf * a.w_sem * a.inv_n_sem : 0.f;
     }
   }
   // fixed (bounding-primitive) semantics: a rendered probability by construction
@@ -321,7 +326,7 @@ __global__ void __launch_bounds__(256) losses_kernel(LossArgs L) {
     l_fix = has ? -logf(pc) * conf : 0.f;
     if (a.d_fixed_semantic_map)
       for (int c = lane; c < a.C; c += 32)
-        a.d_fixed_semantic_map[r * a.C + c] = (has && c == label && p > a.eps) ? -conf * a.w_fix * a.inv_n_sem / pc : 0.f;
+        a.d_fixed_semantic_map[r * a.C + c] = (has && c == label && p >= a.eps) ? -conf * a.w_fix * a.inv_n_sem / pc : 0.f;
   }
   if (a.per_ray != nullptr && lane == 0)
     *reinterpret_cast<float4*>(a.per_ray + r * 4) = make_float4(l_rgb, l_depth, l_sem, l_fix);

@@ -318,7 +318,7 @@ extern "C" int pnr_intersect(const float* rays, int64_t R, const float* box_cent
                              uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
                              void* stream) {
   if (R == 0) return PNR_OK;  // empty input: nothing to do (pointers of empty tensors may be null)
-  PNR_CHECK_ARG(R >= 0 && B >= 0, "pnr_intersect: negative size");
+  PNR_CHECK_ARG(R >= 0 && B >= 0, "pnr_intersect: R=%lld or B=%d < 0", (long long)R, B);
   PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_intersect: M=%d outside [1,%d]", M, PNR_MAX_HITS);
   PNR_CHECK_ARG(rays && hit_mask && box_id && t_in && t_out, "pnr_intersect: null pointer");
   PNR_CHECK_ARG(B == 0 || (box_center && box_half && box_rot), "pnr_intersect: null box table");
@@ -351,7 +351,7 @@ extern "C" int pnr_bound_by_primitives(const uint8_t* hit_mask, const int32_t* b
                                        float* near, float* far, void* stream) {
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(hit_mask && box_id && t_in && t_out && near && far, "pnr_bound_by_primitives: null");
-  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_bound_by_primitives: bad M");
+  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_bound_by_primitives: M=%d outside [1,%d]", M, PNR_MAX_HITS);
   if (R == 0) return PNR_OK;
   bound_kernel<<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(hit_mask, box_id, t_in, t_out, R,
                                                                       M, near, far);
@@ -367,8 +367,9 @@ extern "C" int pnr_sample_stratified(const float* near, const float* far, const 
   PNR_CHECK_ARG(near && far && t_vals && z, "pnr_sample_stratified: null pointer");
   PNR_CHECK_ARG(N >= 1, "pnr_sample_stratified: N < 1");
   PNR_CHECK_ARG(!(perturb > 0.f) || u, "pnr_sample_stratified: perturb > 0 needs u");
-  PNR_CHECK_ARG(box_id == nullptr || (t_in && t_out && M >= 1 && M <= PNR_MAX_HITS),
-                "pnr_sample_stratified: bad interval table");
+  PNR_CHECK_ARG(box_id == nullptr || (t_in && t_out), "pnr_sample_stratified: box_id without t_in / t_out");
+  PNR_CHECK_ARG(box_id == nullptr || (M >= 1 && M <= PNR_MAX_HITS), "pnr_sample_stratified: M=%d outside [1,%d]", M,
+                PNR_MAX_HITS);
   if (R == 0) return PNR_OK;
   if (z == near) return set_error(PNR_ERR_ARG, "pnr_sample_stratified: in-place not allowed");
   stratified_kernel<<<blocks_for(R, 8), 256, 0, (cudaStream_t)stream>>>(
@@ -384,7 +385,8 @@ extern "C" int pnr_sample_intervals(const float* near, const float* far, const f
   PNR_CHECK_ARG(near && far && t_vals && z, "pnr_sample_intervals: null pointer");
   PNR_CHECK_ARG(N >= 1 && N <= kIvMaxN, "pnr_sample_intervals: N=%d outside [1,%d]", N, kIvMaxN);
   PNR_CHECK_ARG(!(perturb > 0.f) || u, "pnr_sample_intervals: perturb > 0 needs u");
-  PNR_CHECK_ARG(box_id && t_in && t_out && M >= 1 && M <= PNR_MAX_HITS, "pnr_sample_intervals: bad interval table");
+  PNR_CHECK_ARG(box_id && t_in && t_out, "pnr_sample_intervals: null interval table");
+  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_sample_intervals: M=%d outside [1,%d]", M, PNR_MAX_HITS);
   interval_kernel<<<blocks_for(R, kIvWarps), kIvWarps * 32, 0, (cudaStream_t)stream>>>(
       near, far, t_vals, u, R, N, perturb, box_id, t_in, t_out, M, z, sample_box);
   PNR_LAUNCH_CHECK("interval_kernel");
@@ -396,7 +398,8 @@ extern "C" int pnr_tag_samples(const float* z, int64_t R, int32_t N, const int32
                                void* stream) {
   if (R == 0) return PNR_OK;
   PNR_CHECK_ARG(z && box_id && t_in && t_out && sample_box, "pnr_tag_samples: null pointer");
-  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_tag_samples: bad M");
+  PNR_CHECK_ARG(R > 0 && N >= 1, "pnr_tag_samples: R=%lld or N=%d < 1", (long long)R, N);
+  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_tag_samples: M=%d outside [1,%d]", M, PNR_MAX_HITS);
   if (R == 0) return PNR_OK;
   tag_kernel<<<blocks_for(R * N, 256), 256, 0, (cudaStream_t)stream>>>(z, R, N, box_id, t_in, t_out, M,
                                                                         sample_box);
@@ -416,7 +419,8 @@ int pnr::sample_pdf_strided(const float* z, const float* weights, int64_t R, int
   PNR_CHECK_ARG(z && weights && u, "pnr_sample_pdf: null pointer (u is required; for the deterministic\n"
                 "                 sampler pass torch.linspace(0,1,Ni) broadcast over rays)");
   PNR_CHECK_ARG(N >= 3 && N <= kPdfMaxN, "pnr_sample_pdf: N=%d outside [3,%d]", N, kPdfMaxN);
-  PNR_CHECK_ARG(Ni >= 1 && N + Ni <= kPdfMaxAll, "pnr_sample_pdf: N+Ni=%d > %d", N + Ni, kPdfMaxAll);
+  PNR_CHECK_ARG(Ni >= 1, "pnr_sample_pdf: Ni=%d < 1", Ni);
+  PNR_CHECK_ARG(N + Ni <= kPdfMaxAll, "pnr_sample_pdf: N+Ni=%d > %d", N + Ni, kPdfMaxAll);
   if (R == 0) return PNR_OK;
   sample_pdf_kernel<<<blocks_for(R, kPdfWarps), kPdfWarps * 32, 0, (cudaStream_t)stream>>>(
       z, weights, R, N, Ni, u, u_stride, z_fine, idx, z_all);

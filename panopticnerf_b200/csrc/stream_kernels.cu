@@ -368,7 +368,11 @@ __global__ void __launch_bounds__(kCompWarps * 32) composite_backward_kernel(Com
       const float o = __shfl_down_sync(0xffffffffu, incl, d);
       if (lane + d < 32) incl += o;
     }
-    const float S = tail + (incl - v);   // strictly later samples
+    // strictly later samples: the next lane's inclusive sum, not incl - v, which cancels when sample i holds most of
+    // the weight (a surface) and would leave S, then S / t with t ~ 1e-10, wrong by ulps of G_i w_i
+    float later = __shfl_down_sync(0xffffffffu, incl, 1);
+    if (lane == 31) later = 0.f;
+    const float S = tail + later;
     tail += __shfl_sync(0xffffffffu, incl, 0);
     if (i < N) {
       const float t = tv[j];
@@ -502,6 +506,7 @@ extern "C" int pnr_composite_backward(const float* raw, const float* z, const fl
                                       const int32_t* box_inst, int32_t B, const pnr_composite_grads* g,
                                       float* d_raw, void* stream) {
   if (R == 0) return PNR_OK;
+  PNR_CHECK_ARG(R > 0, "pnr_composite_backward: R=%lld < 0", (long long)R);
   PNR_CHECK_ARG(raw && z && rays && g && d_raw, "pnr_composite_backward: null pointer");
   PNR_CHECK_ARG(N >= 1 && N <= 32 * kCompMaxPerLane, "pnr_composite_backward: N=%d outside [1,%d]", N,
                 32 * kCompMaxPerLane);
@@ -567,6 +572,7 @@ extern "C" int pnr_composite(const float* raw, const float* z, const float* rays
                              const int32_t* box_inst, int32_t B, const pnr_composite_out* out,
                              void* stream) {
   if (R == 0) return PNR_OK;
+  PNR_CHECK_ARG(R > 0, "pnr_composite: R=%lld < 0", (long long)R);
   PNR_CHECK_ARG(raw && z && rays && out, "pnr_composite: null pointer");
   PNR_CHECK_ARG(N >= 1 && N <= 32 * kCompMaxPerLane, "pnr_composite: N=%d outside [1,%d]", N,
                 32 * kCompMaxPerLane);
