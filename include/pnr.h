@@ -297,6 +297,8 @@ int pnr_mlp_trunk_forward(pnr_ctx* ctx, const float* pts, const float* rays, con
  * by, exact, so that the fp16 parts of ~1e-6 gradients stay normal; |X| and |dZ * scale| must stay below 65504).
  * accumulate != 0 adds to dW / db instead of overwriting them.
  * workspace: pnr_wgrad_workspace_bytes(No, Ni) bytes of device scratch (16-byte aligned) on the current device.
+ * S = 0 needs no workspace (NULL is accepted): dW and db (when given) are set to 0, or left as they are under
+ * accumulate.  A NaN or Inf in dZ[s, o] reaches only row o of dW and db[o]; one in X[s, i] only column i of dW.
  * Replaces the trunk's dW_j = dZ_j^T [H_{j-1}] on pnr_mlp_backward_trunk's stash and the weight gradients of the
  * layers after the trunk; the reference gets them from torch.autograd through nn.Linear. */
 size_t pnr_wgrad_workspace_bytes(int32_t No, int32_t Ni);
@@ -309,7 +311,8 @@ int pnr_wgrad(const float* dz, int64_t ld_dz, int32_t No, const float* x, int64_
  * tensor cores with the 3-product 16-bit operand split of the fused MLP kernel (precision = PNR_PREC_FP16X3 or
  * PNR_PREC_BF16X3), fp32 accumulation in registers.  W is [N, K] (row stride ld_w), or with transposed != 0 a
  * [K, N] matrix read transposed: dL/dx = g W of a layer y = x W^T is pnr_linear(g, W, transposed = 1).  bias [N] or
- * NULL; relu != 0 applies max(., 0).  in_scale: DEVICE scalar or NULL - a power of two the rows of x are multiplied
+ * NULL; relu != 0 applies max(., 0) and keeps NaN as NaN (as torch.relu does).  S = 0 writes nothing.
+ * in_scale: DEVICE scalar or NULL - a power of two the rows of x are multiplied
  * by on load, the result divided by it (exact): gradients of a mean-reduced loss are ~1e-6 and their fp16 parts would
  * go subnormal unscaled.  workspace: pnr_linear_workspace_bytes(N, K) bytes, 16-byte aligned (the packed weights).
  * The render path does not use this (there these layers are steps of the fused kernel); the reference runs

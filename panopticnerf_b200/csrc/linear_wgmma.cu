@@ -196,7 +196,7 @@ __global__ void __launch_bounds__(kLnThreads, 1) linear_kernel(const LinearParam
                 for (int e = 0; e < 2; ++e) {
                   if (col + e < p.N) {
                     const float tv = d[4 * j + 2 * hr + e] * inv + (p.bias != nullptr ? __ldg(p.bias + col + e) : 0.f);
-                    p.y[s * p.ld_y + col + e] = p.relu ? fmaxf(tv, 0.f) : tv;
+                    p.y[s * p.ld_y + col + e] = p.relu && !(tv != tv) ? fmaxf(tv, 0.f) : tv;   // NaN stays NaN (as torch.relu)
                   }
                 }
               }
@@ -252,7 +252,10 @@ extern "C" int pnr_linear(const float* x, int64_t ld_x, int32_t K, const float* 
                           float* y, int64_t ld_y, void* workspace, size_t workspace_bytes, void* stream) {
   PNR_CHECK_ARG(x != nullptr && W != nullptr && y != nullptr, "pnr_linear: x, W and y are required");
   PNR_CHECK_ARG(N >= 1 && N <= 256 && K >= 1 && K <= 512, "pnr_linear: N = %d must be in [1, 256], K = %d in [1, 512]", N, K);
-  PNR_CHECK_ARG(ld_x >= K && ld_y >= N && ld_w >= (transposed ? N : K), "pnr_linear: leading dimensions smaller than the widths");
+  PNR_CHECK_ARG(ld_x >= K, "pnr_linear: leading dimensions: ld_x = %lld < K = %d", (long long)ld_x, K);
+  PNR_CHECK_ARG(ld_y >= N, "pnr_linear: leading dimensions: ld_y = %lld < N = %d", (long long)ld_y, N);
+  PNR_CHECK_ARG(ld_w >= (transposed ? N : K), "pnr_linear: leading dimensions: ld_w = %lld < %s = %d", (long long)ld_w,
+                transposed ? "N" : "K", transposed ? N : K);
   PNR_CHECK_ARG(S >= 0, "pnr_linear: S = %lld", (long long)S);
   PNR_CHECK_ARG(precision == PNR_PREC_BF16X3 || precision == PNR_PREC_FP16X3, "pnr_linear: x3 precisions only (got %d)", precision);
   const size_t need = pnr_linear_workspace_bytes(N, K);

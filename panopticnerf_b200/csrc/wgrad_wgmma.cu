@@ -6,8 +6,8 @@
 // the inputs / output gradients of the layers after the trunk; No, Ni <= 256.  The reduction runs over the SAMPLES,
 // so this is a split-K GEMM with a tiny output.  A CTA owns 128 output rows (blockIdx.y: which 128) and every
 // gridDim.x-th slab of 64 samples; its two warpgroups accumulate 64 rows x NP columns each in registers (two wgmma
-// halves of <= 128 columns) over all of its slabs and write the partial product out once; a second kernel adds the
-// partials in CTA order (deterministic: no atomics).  Per slab:
+// halves of <= 128 columns) over runs of kWgFlush slabs and add each run to the CTA's partial product in global
+// memory; a second kernel adds the partials in CTA order (deterministic).  Per slab:
 //   * the 256 consumer threads read the slab: a work item is 4 consecutive features of 8 consecutive samples (8
 //     16-byte loads), split into 16-bit hi / lo parts and written as four 16-byte rows of the no-swizzle K-major
 //     images (K = samples): a thread's 8 samples of one feature ARE one core-matrix row, so the transposition
@@ -36,6 +36,13 @@ constexpr int kWgBLbo = kWgRows * 16;               // B images: [8 K-cores][256
 constexpr int kWgBPart = (kWgSlab / 8) * kWgBLbo;   // 32 KB
 constexpr int kWgStage = 2 * kWgAPart + 2 * kWgBPart;   // A hi, A lo, B hi, B lo: 96 KB
 constexpr int kWgRing = 2;
+// Slabs per run of the register accumulators.  The tensor cores' fp32 accumulation truncates: on all-positive operands
+// (activations are >= 0, gradient columns have a mean) a run of n accumulating wgmmas loses ~0.75 n 2^-24 of the sum
+// (measured on an H100), so one run over a CTA's whole share of the samples lost 5e-5 of the sum at S = 393 216
+// (256 x 256) and 8e-4 at S = 2^23.  Every kWgFlush slabs the run is added to the CTA's partial product in global
+// memory (round to nearest) and restarted, which bounds the drift at ~8e-6 of the sum whatever S is.  Each flush
+// costs a pipeline drain and a read-modify-write of the partial: pnr_wgrad takes ~20 % longer at 393 216 x 256 x 256.
+constexpr int kWgFlush = 16;
 constexpr int kWgSmemDb = kWgRing * kWgStage;       // [8 sample groups][128] partial bias sums
 constexpr int kWgSmemTotal = kWgSmemDb + 8 * 128 * 4;
 
@@ -65,6 +72,28 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
   float db[4] = {0.f, 0.f, 0.f, 0.f};                         // item 0 of every thread is an A item: its bias sums
   float acc0[64], acc1[64];
   const uint32_t b_lbo = kWgBLbo;
+  // accumulators -> this CTA's partial product (fragment rows 16 w + lane/4 (+8), columns 8 j + 2 (lane % 4)): stored by
+  // the first flush, added to by the later ones (fp32, round to nearest; each element has one reader and writer, this
+  // thread: no atomics, deterministic)
+  const int o0 = ob * 128 + wg * 64 + ((t >> 5) * 16) + (lane >> 2);
+  auto out = [&](const float (&d)[64], int cbase, int nh, bool add) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      if (8 * j < nh) {
+        const int col = cbase + 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          float2* dst = reinterpret_cast<float2*>(p.part + ((int64_t)blockIdx.x * (p.mh * 128) + o0 + 8 * hr) * p.NP + col);
+          float2 v = make_float2(d[4 * j + 2 * hr], d[4 * j + 2 * hr + 1]);
+          if (add) {
+            const float2 o = *dst;
+            v = make_float2(o.x + v.x, o.y + v.y);
+          }
+          *dst = v;
+        }
+      }
+    }
+  };
 #pragma unroll 1
   for (int i = 0; i < n_mine; ++i) {
     const int slot = i & 1;
@@ -125,7 +154,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
     const uint64_t b_hi = make_smem_desc_noswz(sb, b_lbo, 128), b_lo = make_smem_desc_noswz(sb + kWgBPart, b_lbo, 128);
     const uint64_t h1 = (128u * 16u) >> 4;   // row 128 of the B images
     const int n0 = p.NP < 128 ? p.NP : 128;
-    const uint32_t acc = i == 0 ? 0u : 1u;
+    const uint32_t acc = i % kWgFlush == 0 ? 0u : 1u;   // a run restarts after each flush
     wgmma_fence();
 #define PNR_WG_N(NN, D, BH, BL) \
   case NN / 8: mma_run<NN, 3, FMT>(D, a_hi, a_lo, BH, BL, kWgSlab / 16, (2u * kWgALbo) >> 4, (2u * kWgBLbo) >> 4, acc); break;
@@ -141,8 +170,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
     wgmma_commit();
     wgmma_wait<1>();   // slab i - 1's MMAs have retired: its slot may be rewritten by slab i + 1
     __syncthreads();   // (by either warpgroup)
+    if ((i + 1) % kWgFlush == 0 || i + 1 == n_mine) {
+      wgmma_wait<0>();
+      out(acc0, 0, n0, i >= kWgFlush);
+      if (p.NP > 128) out(acc1, 128, p.NP - 128, i >= kWgFlush);
+    }
   }
-  wgmma_wait<0>();
   // ---- bias partial sums: 8 sample groups per feature, added in a fixed order
   if (threadIdx.x < 256) {
     const int quad = threadIdx.x & 31, sg = threadIdx.x >> 5;
@@ -157,23 +190,6 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
     for (int g = 0; g < 8; ++g) sum += dbs[g * 128 + f];
     p.dbp[(int64_t)blockIdx.x * kWgRows + ob * 128 + f] = sum;
   }
-  // ---- accumulators -> this CTA's partial product (fragment rows 16 w + lane/4 (+8), columns 8 j + 2 (lane % 4))
-  const int o0 = ob * 128 + wg * 64 + ((t >> 5) * 16) + (lane >> 2);
-  auto out = [&](const float (&d)[64], int cbase, int nh) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      if (8 * j < nh) {
-        const int col = cbase + 8 * j + 2 * (lane & 3);
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          float* dst = p.part + ((int64_t)blockIdx.x * (p.mh * 128) + o0 + 8 * hr) * p.NP + col;
-          *reinterpret_cast<float2*>(dst) = make_float2(d[4 * j + 2 * hr], d[4 * j + 2 * hr + 1]);
-        }
-      }
-    }
-  };
-  out(acc0, 0, p.NP < 128 ? p.NP : 128);
-  if (p.NP > 128) out(acc1, 128, p.NP - 128);
 }
 
 // dW[o, i] (+)= sum over the CTAs' partial products, in CTA order; db likewise.
@@ -199,7 +215,7 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, const float*
       *d = accumulate ? *d + s : s;
     }
   }
-  if (db != nullptr && dbp != nullptr && idx < No) {
+  if (db != nullptr && idx < No) {   // (G == 0: S = 0, no partials and possibly no workspace; the sum is 0)
     float s = 0.f;
     for (int c = 0; c < G; ++c) s += dbp[(int64_t)c * kWgRows + idx];
     db[idx] = accumulate ? db[idx] + s : s;
@@ -247,7 +263,9 @@ extern "C" int pnr_wgrad(const float* dz, int64_t ld_dz, int32_t No, const float
   PNR_CHECK_ARG(precision == PNR_PREC_BF16X3 || precision == PNR_PREC_FP16X3, "pnr_wgrad: x3 precisions only (got %d)", precision);
   PNR_CHECK_ARG(dz != nullptr && x != nullptr && dW != nullptr, "pnr_wgrad: dz, x and dW are required");
   PNR_CHECK_ARG(No >= 1 && No <= 256 && Ni >= 1 && Ni <= 256, "pnr_wgrad: No = %d, Ni = %d must be in [1, 256] (split wider layers by columns)", No, Ni);
-  PNR_CHECK_ARG(ld_dz >= No && ld_x >= Ni && ld_w >= Ni, "pnr_wgrad: leading dimensions smaller than the widths");
+  PNR_CHECK_ARG(ld_dz >= No, "pnr_wgrad: leading dimensions: ld_dz = %lld < No = %d", (long long)ld_dz, No);
+  PNR_CHECK_ARG(ld_x >= Ni, "pnr_wgrad: leading dimensions: ld_x = %lld < Ni = %d", (long long)ld_x, Ni);
+  PNR_CHECK_ARG(ld_w >= Ni, "pnr_wgrad: leading dimensions: ld_w = %lld < Ni = %d", (long long)ld_w, Ni);
   PNR_CHECK_ARG(S >= 0, "pnr_wgrad: S = %lld", (long long)S);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int dev = 0;
