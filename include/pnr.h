@@ -89,10 +89,12 @@ int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
  *   [instance_linears.0.w/.b, instance_linears.1.w/.b]
  * `shapes[2*i], shapes[2*i+1]` = (out, in) for weights, (out, 1) for biases.  The trunk input width (layer 0's `in`,
  * the skip layer's first columns) is 3 + 6*xyz_res, or E = hash_levels * hash_features for a hash-grid context (whose
- * table is not in this list: pnr_bind_hashgrid_table).  Weights are split
- * into 16-bit hi/lo parts of the context's operand format (fp16 or bf16, cfg.precision), laid out as
- * the no-swizzle K-major wgmma stage images of the packed weight stream (csrc/mlp_program.h) and uploaded.  In the fp16 modes a weight with |w| > 65504 is
- * rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode. */
+ * table is not in this list: pnr_bind_hashgrid_table).  The forward program's packing plan (built from cfg and the
+ * shapes) is applied to the weights on the host: they are split into 16-bit hi/lo parts of the context's operand
+ * format (fp16 or bf16, cfg.precision), laid out as the no-swizzle K-major wgmma stage images of the packed weight
+ * stream (csrc/mlp_program.h) and uploaded, together with the weights themselves, from which the programs built later
+ * and pnr_update_weights pack on the device.  In the fp16 modes a packed weight with |w| > 65504 (after the
+ * feature_linear fold) or not finite is rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode. */
 int pnr_load_weights(pnr_ctx* ctx, const float* const* tensors_host, const int64_t* shapes, int32_t n);
 
 /* a5: ray / oriented-box slab test.  rays [R,6] (o||d); box_center, box_half [B,3]; box_rot [B,3,3]
@@ -330,16 +332,18 @@ int pnr_sample_pdf(const float* z, const float* weights, int64_t R, int32_t N, i
                    const float* u, float* z_fine, int64_t* idx, float* z_all, void* stream);
 
 /* Refresh the weights of a loaded context from DEVICE tensors (same list, order and shapes as pnr_load_weights; fp32,
- * contiguous), stream-ordered on `stream`: what a training loop calls after every optimiser step.  The structure of
- * the per-tile programs does not depend on the values, so nothing is rebuilt or copied through the host: the packed
- * 16-bit streams and constant tables of the forward program (and of the trunk-forward / backward programs once they
- * exist) are rewritten by kernels, including the feature_linear fold.  Bit-identical to a fresh pnr_load_weights of the
- * same values.  A weight outside the fp16 range sets bit 1 of the status word (pnr_status) in the fp16 modes. */
+ * contiguous), stream-ordered on `stream`: what a training loop calls after every optimiser step.  The per-tile
+ * programs and their packing plans do not depend on the values, so nothing is rebuilt or copied through the host: the
+ * tensors are copied into the context's weight vector, the feature_linear fold is recomputed there, and kernels apply
+ * the plans of the forward program (and of the trunk-forward / backward programs once they exist) to it; a plan goes
+ * to the device on its program's first update.  Bit-identical to a fresh pnr_load_weights of the same values.  A
+ * packed weight outside the fp16 range sets bit 1 of the status word (pnr_status) in the fp16 modes. */
 int pnr_update_weights(pnr_ctx* ctx, const float* const* device_tensors, int32_t n, void* stream);
 
 /* Host-only twin of pnr_load_weights (no CUDA call, no context): builds the per-tile program of the fused MLP
- * kernel, the packed 16-bit weight stream and the constant table for `cfg` and returns them in caller buffers
- * (each may be NULL to query sizes only).  `program` receives the MlpProgram struct of csrc/mlp_program.h.
+ * kernel and its packing plan for `cfg`, applies the plan to the tensors as pnr_load_weights does (same checks), and
+ * returns the program, the packed 16-bit weight stream and the constant table in caller buffers (each may be NULL to
+ * query sizes only).  `program` receives the MlpProgram struct of csrc/mlp_program.h.
  * For the CPU test tier: tests/test_cpu_program.py replays the program on the host and compares it with
  * the oracle's Network.forward. */
 #define PNR_PROGRAM_SPLIT_E1 4  /* flags: E1 signalled in two blocks */

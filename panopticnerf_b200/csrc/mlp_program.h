@@ -116,8 +116,8 @@ __host__ __device__ inline uint16_t bf16_rne(float x) {   // round to nearest ev
 
 // Element of the packed weight stream: part 0 (hi) or 1 (lo) of weight w in the operand format (fmt 0 = fp16, 1 = bf16),
 // hi = w rounded to nearest even, lo = (w - hi) rounded to nearest even.  A stage's hi image holds part 0 of its
-// weights, the lo image (x3 modes) part 1.  The host builder and the device-side weight update (pnr_update_weights)
-// both pack with this function, so that a refreshed stream is bit-identical to a freshly built one.
+// weights, the lo image (x3 modes) part 1.  Packing plans are applied with this function on the host and on the device
+// (pnr_update_weights, programs built after the load), so a stream packed on either is bit-identical to the other.
 __host__ __device__ inline uint16_t weight_part16(float w, int part, int fmt) {
   if (fmt == 1) {
     const uint16_t hi = bf16_rne(w);

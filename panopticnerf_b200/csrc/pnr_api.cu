@@ -34,17 +34,23 @@ using namespace pnr;
 // builds the forward program; the other two are built on first use.
 enum ProgramKind { kProgForward = 0, kProgBackward = 1, kProgTrunkForward = 2, kNumPrograms = 3 };
 
+// A program's packing plan, which depends on the configuration and the shapes only.  V is the weight vector: the
+// tensors of pnr_load_weights' list concatenated in order, then the derived block (Fold).  Packed element p is part
+// wpart[p] (weight_part16) of V[wpos[p]], constant c is V[cpos[c]]; position -1 is zero padding.
+struct Plan {
+  std::vector<int32_t> wpos, cpos;
+  std::vector<uint8_t> wpart;
+};
+
 struct PackedProgram {
-  bool ready = false;             // built and uploaded since the last pnr_load_weights
+  bool ready = false;             // built and packed since the last pnr_load_weights
   MlpLaunch launch;               // launch.prog = the program; launch.p is filled per call.  The whole struct travels as
                                   // the kernel's __grid_constant__ parameter: nothing is shared between contexts,
                                   // streams, devices or CUDA-graph replays.
   uint8_t* d_wpacked = nullptr;
   float* d_consts = nullptr;
   size_t n_w = 0, n_c = 0;        // packed 16-bit elements / constants
-  // device-side weight updates: packed element p = part d_wpart[p] of V[d_widx[p]], constant c = V[d_cidx[c]]
-  // (Builder index mode), built by the first pnr_update_weights that refreshes this program
-  bool plan_ready = false;
+  Plan plan;                      // on the host until the program is first packed on the device (refresh)
   int32_t* d_widx = nullptr;
   uint8_t* d_wpart = nullptr;
   int32_t* d_cidx = nullptr;
@@ -59,14 +65,8 @@ struct pnr_ctx {
   uint32_t* d_status = nullptr; // sticky range-check word of the fused MLP (bit 0: activation out of operand range)
   const float* hash_table = nullptr;   // hash-grid contexts: the caller's table (pnr_bind_hashgrid_table), not owned
   uint32_t hash_res[kHashMaxLevels] = {};
-  // what the backward and trunk-forward programs are built from: weight, bias per trunk layer, as given to pnr_load_weights
-  std::vector<std::vector<float>> host_trunk;
-  std::vector<int64_t> host_trunk_shapes;
-  // device-side weight updates (pnr_update_weights): V = all input tensors concatenated + the derived (folded) values
-  float* d_V = nullptr;
-  std::vector<int64_t> v_off, all_shapes;   // position of every input tensor in V; the shapes given to pnr_load_weights
-  int64_t v_total = 0, v_derived = 0;
-  bool device_weights = false;              // the weights in V are newer than the host copies (programs built later are packed from V)
+  float* d_V = nullptr;   // V of the load or of the last pnr_update_weights: what programs are packed from on the device
+  std::vector<int64_t> v_off, shapes;   // V's layout (Builder::v_off); the shapes given to pnr_load_weights
 };
 
 namespace {
@@ -78,7 +78,14 @@ constexpr uint32_t make_idesc_f32acc(int M, int N, int fmt) {
   return (1u << 4) | (uint32_t(fmt) << 7) | (uint32_t(fmt) << 10) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
 }
 
-struct Mat { const float* w; int out, in; };  // row-major [out, in]
+// A row-major [out, in] matrix by the positions of its elements in V: element (r, c) is V[first + r * in + c] for a
+// tensor of the list, V[pos[r * in + c]] for a matrix the build derives (a transposed or stacked copy of positions).
+struct Mat {
+  int32_t first;
+  int out, in;
+  const int32_t* pos = nullptr;
+  int32_t at(int r, int c) const { return pos ? pos[(size_t)r * in + c] : first + r * in + c; }
+};
 
 struct Seg {
   uint8_t kind;        // A_TMEM / A_EMB / A_DIR
@@ -89,26 +96,21 @@ struct Seg {
   bool release;        // A_EMB/A_DIR: last reader in the tile
 };
 
+// Builds a program and its plan from the configuration and the tensors' shapes: it never reads a weight value, and
+// looks at the tensor pointers only to check that they are given.
 struct Builder {
   MlpProgram prog;
-  std::vector<uint16_t> wbuf;   // packed weight stream (bf16 elements)
-  std::vector<float> consts;
+  Plan plan;
   int passes, fmt;
   // E1 in two blocks signalled separately (mlp_program.h).  Pays off when a half spans several weight stages
   // (the x3 modes, K = 64 per stage: 75.4 k -> 71.5 k cycles per tile); the 1-pass modes keep one block.
   bool split_e1;
   bool acc_flip = true;             // odd tiles use the accumulator columns XOR 128 when the program allows it
   bool view_on_producers = false;   // the (last, one-half) view step's epilogue runs on the producer warps (mlp_program.h)
-  bool out_of_fp16_range = false;   // a weight (after the feature_linear fold) exceeds 65504 or is not finite
-  // INDEX MODE (device-side weight updates, pnr_update_weights): the builder is run once on tensors whose VALUES are
-  // their own position (+1) in the concatenation V of all input tensors followed by the derived values (the folded
-  // view matrix and bias, which build_program then fills with positions instead of arithmetic).  Everything else in a
-  // program's packed stream and constant table is a copy of one source value, so this run yields, per packed element,
-  // where it comes from (wsrc, 0 = padding) and which 16-bit part it is (wpart) - the plan a kernel replays on device.
-  bool index_mode = false;
-  int64_t derived_base = 0;         // position of the first derived value in V
-  std::vector<float> wsrc;
-  std::vector<uint8_t> wpart;
+  // V's layout, laid down as the build takes the tensors of the list, in list order: tensor i at v_off[i], and
+  // v_off.back() the end of the last one taken - where the derived block starts once every tensor is taken
+  std::vector<int64_t> v_off{0};
+  const char* what = "";            // names the program in error texts (finish, pack_host)
   std::string err;
 
   Builder(int passes_, int fmt_) : passes(passes_), fmt(fmt_) {
@@ -116,32 +118,31 @@ struct Builder {
     split_e1 = passes == 3;
   }
 
-  int add_consts(const float* src, int n_valid, int n_pad) {
-    const int off = (int)consts.size();
-    for (int i = 0; i < n_pad; ++i) consts.push_back(i < n_valid ? src[i] : 0.f);
+  // Position in V of tensor i, the next one of the list, whose shape has been checked
+  int32_t take_tensor(const int64_t* shapes, int i) {
+    v_off.push_back(v_off.back() + shapes[2 * i] * shapes[2 * i + 1]);
+    return (int32_t)v_off[i];
+  }
+
+  int add_consts(int32_t first, int n_valid, int n_pad) {   // V[first .. first + n_valid), zero padded to n_pad
+    const int off = (int)plan.cpos.size();
+    for (int i = 0; i < n_pad; ++i) plan.cpos.push_back(i < n_valid ? first + i : -1);
     return off;
   }
 
   // Stage image of rows [row0, row0 + n_rows) x K [k0, k0 + 8*kcores): no-swizzle K-major core matrices,
   // byte offset of element (n, k) = ((k/8) * n_rows + n) * 16 + (k%8) * 2  (LBO = n_rows*16, SBO = 128).
   void pack_stage(const Mat& m, int row0, int n_rows, int col0, int kvalid, int k0, int kcores, int part) {
-    const size_t base = wbuf.size();
+    const size_t base = plan.wpos.size();
     const int n_pad = n_rows;
-    wbuf.resize(base + (size_t)n_pad * kcores * 8);
-    if (index_mode) { wsrc.resize(wbuf.size(), 0.f); wpart.resize(wbuf.size(), 0); }
+    plan.wpos.resize(base + (size_t)n_pad * kcores * 8);
+    plan.wpart.resize(plan.wpos.size(), (uint8_t)part);
     for (int kc = 0; kc < kcores; ++kc)
       for (int nn = 0; nn < n_pad; ++nn)
         for (int e = 0; e < 8; ++e) {
           const int n = row0 + nn;
           const int k = k0 + kc * 8 + e;
-          const float w = (n < m.out && k < kvalid) ? m.w[(size_t)n * m.in + col0 + k] : 0.f;
-          if (index_mode) {
-            wsrc[base + ((size_t)kc * n_pad + nn) * 8 + e] = w;
-            wpart[base + ((size_t)kc * n_pad + nn) * 8 + e] = (uint8_t)part;
-          } else if (!(w >= -65504.f && w <= 65504.f)) {
-            out_of_fp16_range = true;   // also catches NaN
-          }
-          wbuf[base + ((size_t)kc * n_pad + nn) * 8 + e] = weight_part16(w, part, fmt);
+          plan.wpos[base + ((size_t)kc * n_pad + nn) * 8 + e] = (n < m.out && k < kvalid) ? m.at(n, col0 + k) : -1;
         }
   }
 
@@ -178,7 +179,7 @@ struct Builder {
             const int parts = passes == 3 ? 2 : 1;
             StageDesc& sd = prog.st[prog.n_stages++];
             memset(&sd, 0, sizeof(sd));
-            sd.gofs = (uint32_t)(wbuf.size() * 2);
+            sd.gofs = (uint32_t)(plan.wpos.size() * 2);
             sd.bytes = (uint32_t)((r1 - r0) * kcores * 16 * parts);
             sd.n = (uint16_t)(r1 - r0);
             sd.acc_col = (uint16_t)(acc_col + r0);
@@ -338,19 +339,83 @@ struct Builder {
     }
   }
 
-  // The end of every build: `ok` = every step was added; `what` names the program in the error text.
-  int finish(bool ok, const char* what) {
+  // The end of every build: `ok` = every step was added; `name` names the program in the error texts.
+  int finish(bool ok, const char* name) {
+    what = name;
     if (!ok) return set_error(PNR_ERR_UNSUPPORTED, "%s: program build failed: %s", what, err.c_str());
-    if ((int)consts.size() > kMaxConsts)
-      return set_error(PNR_ERR_UNSUPPORTED, "%s: %d constants > %d", what, (int)consts.size(), kMaxConsts);
-    if (out_of_fp16_range && fmt == kFmtF16)
-      return set_error(PNR_ERR_UNSUPPORTED, "%s: a weight is outside the fp16 range (|w| > 65504 or not finite): use "
-                       "precision bf16x3", what);
-    prog.n_consts = (int)consts.size();
+    if ((int)plan.cpos.size() > kMaxConsts)
+      return set_error(PNR_ERR_UNSUPPORTED, "%s: %d constants > %d", what, (int)plan.cpos.size(), kMaxConsts);
+    prog.n_consts = (int)plan.cpos.size();
     finalize();
     return PNR_OK;
   }
 };
+
+// The feature_linear fold, V's derived block: the folded view matrix [W/2, W+Ed], then the folded bias [W/2].
+// feature_linear has no activation, so it is folded into the view layer (exact algebra, done in double):
+//   W_view [feat ; gamma(d)] + b_view  with  feat = W_feat h + b_feat
+//   = (W_view[:, :W] W_feat) h + W_view[:, W:] gamma(d) + (W_view[:, :W] b_feat + b_view).
+// One 256x256 GEMM per sample (11 % of the MLP) and its epilogue disappear; the view step reads the trunk output h
+// directly.  Positions in V of the tensors it reads and of the block it writes:
+struct Fold {
+  int64_t view_w, view_b, feat_w, feat_b, out;
+  int W, Ed;
+};
+
+// Element (n, k) of [W/2, W + Ed + 1]: k < W the folded matrix, k < W + Ed a gamma(d) column of W_view, k = W + Ed the
+// folded bias.  Double sums, j ascending: host (host_v) and device (fold_kernel) fold bit-identically with it.
+__host__ __device__ inline void fold_element(float* V, const Fold& f, int n, int k) {
+  const float* vrow = V + f.view_w + (int64_t)n * (f.W + f.Ed);
+  if (k < f.W) {
+    double acc = 0.0;
+    for (int j = 0; j < f.W; ++j) acc += (double)vrow[j] * (double)V[f.feat_w + (int64_t)j * f.W + k];
+    V[f.out + (int64_t)n * (f.W + f.Ed) + k] = (float)acc;
+  } else if (k < f.W + f.Ed) {
+    V[f.out + (int64_t)n * (f.W + f.Ed) + k] = vrow[k];
+  } else {
+    double acc = (double)V[f.view_b + n];
+    for (int j = 0; j < f.W; ++j) acc += (double)vrow[j] * (double)V[f.feat_b + j];
+    V[f.out + (int64_t)(f.W / 2) * (f.W + f.Ed) + n] = (float)acc;
+  }
+}
+
+// The fold of tensors laid out by `v_off` (all taken; list order: trunk (w, b) x D, alpha, feature, view, rgb, heads)
+Fold fold_of(const pnr_config& c, const std::vector<int64_t>& v_off) {
+  const int D = c.D;
+  return Fold{v_off[2 * D + 4], v_off[2 * D + 5], v_off[2 * D + 2], v_off[2 * D + 3], v_off.back(), c.W, 3 + 6 * c.view_res};
+}
+
+// V on the host, from the tensors a build took: them, concatenated, then - for a forward program - the derived block.
+std::vector<float> host_v(const pnr_config& c, const float* const* t, const std::vector<int64_t>& v_off, bool derived) {
+  const int W2 = c.W / 2, Ed = 3 + 6 * c.view_res;
+  std::vector<float> V((size_t)v_off.back() + (derived ? (size_t)W2 * (c.W + Ed + 1) : 0));
+  for (size_t i = 0; i + 1 < v_off.size(); ++i) memcpy(V.data() + v_off[i], t[i], (v_off[i + 1] - v_off[i]) * 4);
+  if (derived) {
+    const Fold f = fold_of(c, v_off);
+    for (int n = 0; n < W2; ++n)
+      for (int k = 0; k <= c.W + Ed; ++k) fold_element(V.data(), f, n, k);
+  }
+  return V;
+}
+
+// A plan applied to V on the host (the device twin: pack_from_plan_kernel, consts_from_plan_kernel).  In the fp16
+// modes a packed weight outside the fp16 range - after the fold - is refused.
+int pack_host(const Builder& bld, const std::vector<float>& V, std::vector<uint16_t>& w, std::vector<float>& consts) {
+  const Plan& pl = bld.plan;
+  w.resize(pl.wpos.size());
+  bool out_of_fp16_range = false;
+  for (size_t p = 0; p < w.size(); ++p) {
+    const float v = pl.wpos[p] < 0 ? 0.f : V[pl.wpos[p]];
+    out_of_fp16_range |= !(v >= -65504.f && v <= 65504.f);   // also catches NaN
+    w[p] = weight_part16(v, pl.wpart[p], bld.fmt);
+  }
+  if (out_of_fp16_range && bld.fmt == kFmtF16)
+    return set_error(PNR_ERR_UNSUPPORTED, "%s: a weight is outside the fp16 range (|w| > 65504 or not finite): use "
+                     "precision bf16x3", bld.what);
+  consts.resize(pl.cpos.size());
+  for (size_t c = 0; c < consts.size(); ++c) consts[c] = pl.cpos[c] < 0 ? 0.f : V[pl.cpos[c]];
+  return PNR_OK;
+}
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
@@ -484,10 +549,11 @@ extern "C" int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, vo
 // pnr_load_weights' list.  Layer 0 reads the trunk input, the skip layer D/2 + 1 [trunk input ; h].
 struct Trunk {
   std::vector<Mat> w;
-  std::vector<const float*> b;
+  std::vector<int32_t> b;   // first position in V
 };
 
-static int take_trunk(const pnr_config& c, const float* const* t, const int64_t* shapes, const char* what, Trunk& tr) {
+static int take_trunk(const pnr_config& c, const float* const* t, const int64_t* shapes, const char* what, Builder& bld,
+                      Trunk& tr) {
   const int D = c.D, W = c.W, Ex = trunk_input_width(c), skip = D / 2;
   tr.w.resize(D);
   tr.b.resize(D);
@@ -496,8 +562,8 @@ static int take_trunk(const pnr_config& c, const float* const* t, const int64_t*
     if (shapes[4 * i] != W || shapes[4 * i + 1] != in || shapes[4 * i + 2] != W || shapes[4 * i + 3] != 1 || !t[2 * i] ||
         !t[2 * i + 1])
       return set_error(PNR_ERR_ARG, "%s: tensor %d: expected weight [%d,%d] + bias [%d,1]", what, 2 * i, W, in, W);
-    tr.w[i] = Mat{t[2 * i], W, in};
-    tr.b[i] = t[2 * i + 1];
+    tr.w[i] = Mat{bld.take_tensor(shapes, 2 * i), W, in};
+    tr.b[i] = bld.take_tensor(shapes, 2 * i + 1);
   }
   return PNR_OK;
 }
@@ -540,22 +606,22 @@ static bool add_trunk_steps(const pnr_config& c, const Trunk& tr, uint8_t last_k
   return true;
 }
 
-// Host only (no CUDA call): checks the tensor list against cfg, builds the per-tile program, the packed
-// weight stream and the constant table.  Shared by pnr_load_weights and pnr_program_host.
+// Host only (no CUDA call): checks the tensor list against cfg, builds the per-tile program and its plan.  Shared by
+// pnr_load_weights and pnr_program_host.
 static int build_program(const pnr_config& c, const float* const* t, const int64_t* shapes, int32_t n,
                          Builder& bld) {
   const int D = c.D, W = c.W, W2 = W / 2, C = c.num_classes, K = c.num_instances, Ed = 3 + 6 * c.view_res;
   const int expected = 2 * D + 8 + (C > 0 ? 4 : 0) + (K > 0 ? 4 : 0);
   PNR_CHECK_ARG(n == expected, "pnr_load_weights: got %d tensors, expected %d", n, expected);
   Trunk trunk;
-  if (const int rc = take_trunk(c, t, shapes, "pnr_load_weights", trunk)) return rc;
+  if (const int rc = take_trunk(c, t, shapes, "pnr_load_weights", bld, trunk)) return rc;
   int ti = 2 * D;
-  auto take = [&](int out, int in, Mat* m, const float** bias) -> bool {
+  auto take = [&](int out, int in, Mat* m, int32_t* bias) -> bool {
     if (shapes[2 * ti] != out || shapes[2 * ti + 1] != in) return false;
     if (shapes[2 * ti + 2] != out || shapes[2 * ti + 3] != 1) return false;
     if (!t[ti] || !t[ti + 1]) return false;
-    *m = Mat{t[ti], out, in};
-    *bias = t[ti + 1];
+    *m = Mat{bld.take_tensor(shapes, ti), out, in};
+    *bias = bld.take_tensor(shapes, ti + 1);
     ti += 2;
     return true;
   };
@@ -564,7 +630,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     return set_error(PNR_ERR_ARG, "pnr_load_weights: tensor %d: expected weight [%d,%d] + bias [%d,1]", \
                      ti, out, in, out)
   Mat m_sig, m_feat, m_view, m_rgb, m_s1, m_s2, m_i1, m_i2;
-  const float *b_sig, *b_feat, *b_view, *b_rgb, *b_s1 = nullptr, *b_s2 = nullptr, *b_i1 = nullptr, *b_i2 = nullptr;
+  int32_t b_sig, b_feat, b_view, b_rgb, b_s1 = -1, b_s2 = -1, b_i1 = -1, b_i2 = -1;
   PNR_TAKE(1, W, &m_sig, &b_sig);
   PNR_TAKE(W, W, &m_feat, &b_feat);
   PNR_TAKE(W2, W + Ed, &m_view, &b_view);
@@ -573,42 +639,19 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
   if (K > 0) { PNR_TAKE(W2, W, &m_i1, &b_i1); PNR_TAKE(K, W2, &m_i2, &b_i2); }
 #undef PNR_TAKE
 
-  const int sig_w_off = bld.add_consts(m_sig.w, W, W);
+  const int sig_w_off = bld.add_consts(m_sig.first, W, W);
   bld.prog.sigma_bias_off = bld.add_consts(b_sig, 1, 4);
-  std::vector<float> rgbw(3 * W2);
-  for (int ch = 0; ch < 3; ++ch)
-    for (int k = 0; k < W2; ++k) rgbw[ch * W2 + k] = m_rgb.w[ch * W2 + k];
-  const int rgb_w_off = bld.add_consts(rgbw.data(), 3 * W2, 3 * W2);
+  const int rgb_w_off = bld.add_consts(m_rgb.first, 3 * W2, 3 * W2);
   bld.prog.rgb_bias_off = bld.add_consts(b_rgb, 3, 4);
 
   bool ok = add_trunk_steps(c, trunk, EPI_RELU_TO_A, sig_w_off, false, bld);
-  // feature_linear has no activation, so it is folded into the view layer when the weights are loaded
-  // (exact algebra, done in double):  W_view [feat ; gamma(d)] + b_view  with  feat = W_feat h + b_feat
-  //   = (W_view[:, :W] W_feat) h + W_view[:, W:] gamma(d) + (W_view[:, :W] b_feat + b_view).
-  // One 256x256 GEMM per sample (11 % of the MLP) and its epilogue disappear; the view step reads the trunk
-  // output h directly.
-  std::vector<float> fold((size_t)W2 * (W + Ed)), fold_b(W2);
-  if (bld.index_mode) {   // derived values: positions in V's derived area (filled on device by fold_kernel)
-    for (size_t i = 0; i < fold.size(); ++i) fold[i] = (float)(bld.derived_base + (int64_t)i + 1);
-    for (int n_ = 0; n_ < W2; ++n_) fold_b[n_] = (float)(bld.derived_base + (int64_t)fold.size() + n_ + 1);
-  }
-  for (int n_ = 0; n_ < W2 && !bld.index_mode; ++n_) {
-    const float* vrow = m_view.w + (size_t)n_ * (W + Ed);
-    for (int k = 0; k < W; ++k) {
-      double acc = 0.0;
-      for (int j = 0; j < W; ++j) acc += (double)vrow[j] * (double)m_feat.w[(size_t)j * W + k];
-      fold[(size_t)n_ * (W + Ed) + k] = (float)acc;
-    }
-    for (int e = 0; e < Ed; ++e) fold[(size_t)n_ * (W + Ed) + W + e] = vrow[W + e];
-    double accb = (double)b_view[n_];
-    for (int j = 0; j < W; ++j) accb += (double)vrow[j] * (double)b_feat[j];
-    fold_b[n_] = (float)accb;
-  }
-  const Mat m_fold{fold.data(), W2, W + Ed};
+  // the view step reads the fold (Fold): V's derived block, after the last tensor
+  const int32_t fold_first = (int32_t)bld.v_off.back();
+  const Mat m_fold{fold_first, W2, W + Ed};
   auto add_view = [&](int acc_col) {  // view branch [h, gamma(d)] -> relu -> rgb (CUDA cores) ; writes rgb + sigma
     EpiDesc ed{};
     ed.kind = EPI_VIEW_RGB;
-    ed.bias_off = (uint16_t)bld.add_consts(fold_b.data(), W2, W2);
+    ed.bias_off = (uint16_t)bld.add_consts(fold_first + W2 * (W + Ed), W2, W2);
     ed.aux_off = (uint16_t)rgb_w_off;
     std::vector<Seg> segs;
     segs.push_back(seg_tmem(m_fold, 0, W, kColAHi, kColALo));
@@ -623,7 +666,7 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     ok = ok && bld.add_step(segs, W2, acc_col, ed, false, nullptr, W2 <= 128 ? W2 : 0);
   };
   // heads: hidden layer -> logits
-  auto add_head = [&](const Mat& m1, const float* b1, const Mat& m2, const float* b2, int nout, int out_off) {
+  auto add_head = [&](const Mat& m1, int32_t b1, const Mat& m2, int32_t b2, int nout, int out_off) {
     EpiDesc e1{};
     e1.kind = EPI_RELU_TO_A;
     e1.dst_col = kColHeadHi;        // head hidden activations (K <= 128) live in the upper half of the
@@ -638,7 +681,6 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     e2.bias_off = (uint16_t)bld.add_consts(b2, nout, npad);
     ok = ok && bld.add_step({seg_tmem(m2, 0, W2, kColHeadHi, kColHeadLo)}, npad, kColAcc, e2, false);
   };
-  std::vector<float> hid_w, hid_b;   // must outlive add_step (Mat holds a pointer)
   if (C > 0 && K > 0 && 2 * W2 == W && W >= 128) {
     // Both heads: the view step runs first (it is the last reader of the trunk output), then ONE W-wide hidden
     // step computes both heads' hidden layers ([W_s1 ; W_i1], ReLU) in place of the trunk activations - a full-size
@@ -650,18 +692,16 @@ static int build_program(const pnr_config& c, const float* const* t, const int64
     // (The view step accumulating in the UPPER accumulator half, so that the hidden step's first half can start right
     // behind the view MMAs, was measured on the cfg3 frame: 411.8 vs 408.9 ms - no gain, not kept.)
     add_view(kColAcc);
-    hid_w.resize((size_t)W * W);
-    hid_b.resize(W);
-    memcpy(hid_w.data(), m_s1.w, sizeof(float) * (size_t)W2 * W);
-    memcpy(hid_w.data() + (size_t)W2 * W, m_i1.w, sizeof(float) * (size_t)W2 * W);
-    memcpy(hid_b.data(), b_s1, sizeof(float) * W2);
-    memcpy(hid_b.data() + W2, b_i1, sizeof(float) * W2);
-    const Mat m_hid{hid_w.data(), W, W};
+    std::vector<int32_t> hid_w((size_t)W * W);   // [W_s1 ; W_i1]
+    for (int r = 0; r < W; ++r)
+      for (int k = 0; k < W; ++k) hid_w[(size_t)r * W + k] = r < W2 ? m_s1.at(r, k) : m_i1.at(r - W2, k);
+    const Mat m_hid{0, W, W, hid_w.data()};
     EpiDesc eh{};
     eh.kind = EPI_RELU_TO_A;
     eh.dst_col = kColAHi;
     eh.dst_lo_col = kColALo;
-    eh.bias_off = (uint16_t)bld.add_consts(hid_b.data(), W, W);
+    eh.bias_off = (uint16_t)bld.add_consts(b_s1, W2, W2);
+    bld.add_consts(b_i1, W2, W2);                         // contiguous: [b_s1 ; b_i1]
     ok = ok && bld.add_step({seg_tmem(m_hid, 0, W, kColAHi, kColALo)}, W, kColAcc, eh, false);
     const int n_s = round_up(C, 16), n_i = round_up(K, 16);
     EpiDesc el{};
@@ -698,31 +738,31 @@ static int build_backward_program(const pnr_config& c, const float* const* t, co
   if (D - 1 > kMaxMaskSlots)
     return set_error(PNR_ERR_UNSUPPORTED, "backward program: D=%d needs %d sign-pattern slots, %d fit", D, D - 1, kMaxMaskSlots);
   Trunk trunk;
-  if (const int rc = take_trunk(c, t, shapes, "backward program", trunk)) return rc;
+  if (const int rc = take_trunk(c, t, shapes, "backward program", bld, trunk)) return rc;
   bool ok = add_trunk_steps(c, trunk, forward_only ? EPI_ACT_OUT : EPI_LOADG_TO_A, -1, !forward_only, bld);
-  std::vector<float> wt;   // W_l transposed: [in_l, W] row-major (packed inside add_step, so one buffer serves all)
+  std::vector<int32_t> wt;   // W_l transposed: [in_l, W] row-major (packed inside add_step, so one buffer serves all)
   for (int l = forward_only ? -1 : D - 1; l >= 0 && ok; --l) {
     const int in = trunk.w[l].in;
-    wt.assign((size_t)in * W, 0.f);
+    wt.assign((size_t)in * W, 0);
     for (int o = 0; o < W; ++o)
-      for (int k = 0; k < in; ++k) wt[(size_t)k * W + o] = trunk.w[l].w[(size_t)o * in + k];
-    auto grad_out = [&](const float* rows, bool accumulate) {    // embedded-input columns -> output rows
+      for (int k = 0; k < in; ++k) wt[(size_t)k * W + o] = trunk.w[l].at(o, k);
+    auto grad_out = [&](const int32_t* rows, bool accumulate) {  // embedded-input columns -> output rows
       EpiDesc eo{};
       eo.kind = EPI_GRAD_OUT;
       eo.n_valid = (uint16_t)Ex;
       eo.n_valid1 = accumulate ? 1 : 0;
       eo.out_off = 0;
       // one N = Ekpad half: two N = 32 halves would double the MMA count for the same tensor time per MMA
-      return bld.add_step({seg_tmem(Mat{rows, Ex, W}, 0, W)}, Ekpad, kColAcc, eo, false, nullptr, Ekpad);
+      return bld.add_step({seg_tmem(Mat{0, Ex, W, rows}, 0, W)}, Ekpad, kColAcc, eo, false, nullptr, Ekpad);
     };
-    auto grad_h = [&](const float* rows) {                       // hidden columns, gated by layer l-1's sign pattern
+    auto grad_h = [&](const int32_t* rows) {                     // hidden columns, gated by layer l-1's sign pattern
       EpiDesc em{};
       em.kind = EPI_MASK_TO_A;
       em.n_valid = (uint16_t)l;                                  // slot (l - 1) + 1
       em.out_off1 = (uint16_t)(2 * D - 2 - (l - 1) + 1);          // stash slot + 1 of dZ_{l-1}
       em.dst_col = kColAHi;
       em.dst_lo_col = kColALo;
-      return bld.add_step({seg_tmem(Mat{rows, W, W}, 0, W)}, W, kColAcc, em, false);
+      return bld.add_step({seg_tmem(Mat{0, W, W, rows}, 0, W)}, W, kColAcc, em, false);
     };
     if (l == 0) {
       ok = grad_out(wt.data(), true);
@@ -743,17 +783,15 @@ static int build_program_kind(ProgramKind kind, const pnr_config& c, const float
                               : build_backward_program(c, t, shapes, n, bld, kind == kProgTrunkForward);
 }
 
-// Replaces the program's device buffers with the builder's packed stream and constants.
-static int upload(PackedProgram& pp, const Builder& bld) {
+// Gives the program the builder's program and plan, and device buffers for the stream and constants the caller packs.
+static int place(PackedProgram& pp, Builder& bld) {
   release(pp);
-  pp.n_w = bld.wbuf.size();
-  pp.n_c = bld.consts.size();
+  pp.n_w = bld.plan.wpos.size();
+  pp.n_c = bld.plan.cpos.size();
   PNR_CUDA(cudaMalloc(&pp.d_wpacked, pp.n_w * 2));
   PNR_CUDA(cudaMalloc(&pp.d_consts, pp.n_c * 4));
-  PNR_CUDA(cudaMemcpy(pp.d_wpacked, bld.wbuf.data(), pp.n_w * 2, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(pp.d_consts, bld.consts.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
   pp.launch.prog = bld.prog;
-  pp.ready = true;
+  pp.plan = std::move(bld.plan);
   return PNR_OK;
 }
 
@@ -762,22 +800,24 @@ extern "C" int pnr_load_weights(pnr_ctx* ctx, const float* const* t, const int64
   const pnr_config& c = ctx->cfg;
   Builder bld(ctx->passes, ctx->fmt);
   if (const int rc = build_program(c, t, shapes, n, bld)) return rc;
+  const std::vector<float> V = host_v(c, t, bld.v_off, true);
+  std::vector<uint16_t> w;
+  std::vector<float> consts;
+  if (const int rc = pack_host(bld, V, w, consts)) return rc;
   DeviceGuard guard(c.device);
   ctx->loaded = false;
   for (PackedProgram& pp : ctx->prog) release(pp);   // the backward and trunk-forward programs follow on first use
   cudaFree(ctx->d_V);
   ctx->d_V = nullptr;
-  ctx->device_weights = false;
-  ctx->all_shapes.assign(shapes, shapes + 2 * n);
-  ctx->v_off.assign(n, 0);
-  ctx->v_total = 0;
-  for (int i = 0; i < n; ++i) { ctx->v_off[i] = ctx->v_total; ctx->v_total += shapes[2 * i] * shapes[2 * i + 1]; }
-  ctx->v_derived = (int64_t)(c.W / 2) * (c.W + 3 + 6 * c.view_res) + c.W / 2;   // folded view matrix + bias
-  ctx->host_trunk.clear();
-  ctx->host_trunk_shapes.assign(shapes, shapes + 4 * c.D);
-  for (int i = 0; i < 2 * c.D; ++i)
-    ctx->host_trunk.emplace_back(t[i], t[i] + (size_t)shapes[2 * i] * (size_t)shapes[2 * i + 1]);
-  if (const int rc = upload(ctx->prog[kProgForward], bld)) return rc;
+  ctx->v_off = bld.v_off;
+  ctx->shapes.assign(shapes, shapes + 2 * n);
+  PackedProgram& pp = ctx->prog[kProgForward];
+  if (const int rc = place(pp, bld)) return rc;
+  PNR_CUDA(cudaMalloc(&ctx->d_V, V.size() * 4));
+  PNR_CUDA(cudaMemcpy(ctx->d_V, V.data(), V.size() * 4, cudaMemcpyHostToDevice));
+  PNR_CUDA(cudaMemcpy(pp.d_wpacked, w.data(), pp.n_w * 2, cudaMemcpyHostToDevice));
+  PNR_CUDA(cudaMemcpy(pp.d_consts, consts.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
+  pp.ready = true;
   ctx->loaded = true;
   return PNR_OK;
 }
@@ -794,22 +834,25 @@ extern "C" int pnr_program_host(const pnr_config* cfg, const float* const* t, co
   if (flags & PNR_PROGRAM_NO_SPLIT) bld.split_e1 = false;
   if (flags & PNR_PROGRAM_SPLIT_E1) bld.split_e1 = true;
   if (flags & PNR_PROGRAM_VIEW_PRODUCERS) bld.view_on_producers = true;
-  if (const int rc = build_program_kind((flags & PNR_PROGRAM_BACKWARD) ? kProgBackward : kProgForward, *cfg, t, shapes, n, bld))
-    return rc;
+  const ProgramKind kind = (flags & PNR_PROGRAM_BACKWARD) ? kProgBackward : kProgForward;
+  if (const int rc = build_program_kind(kind, *cfg, t, shapes, n, bld)) return rc;
+  std::vector<uint16_t> w;
+  std::vector<float> cst;
+  if (const int rc = pack_host(bld, host_v(*cfg, t, bld.v_off, kind == kProgForward), w, cst)) return rc;
   *program_bytes = sizeof(MlpProgram);
-  *wpacked_bytes = bld.wbuf.size() * 2;
-  *n_consts = bld.consts.size();
+  *wpacked_bytes = w.size() * 2;
+  *n_consts = cst.size();
   if (program) {
     PNR_CHECK_ARG(program_cap >= sizeof(MlpProgram), "pnr_program_host: program buffer too small");
     memcpy(program, &bld.prog, sizeof(MlpProgram));
   }
   if (wpacked) {
     PNR_CHECK_ARG(wpacked_cap >= *wpacked_bytes, "pnr_program_host: weight buffer too small");
-    memcpy(wpacked, bld.wbuf.data(), *wpacked_bytes);
+    memcpy(wpacked, w.data(), *wpacked_bytes);
   }
   if (consts) {
     PNR_CHECK_ARG(consts_cap >= *n_consts, "pnr_program_host: constant buffer too small");
-    memcpy(consts, bld.consts.data(), *n_consts * 4);
+    memcpy(consts, cst.data(), *n_consts * 4);
   }
   return PNR_OK;
 }
@@ -903,13 +946,11 @@ extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z
   return PNR_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ device-side updates
+// ------------------------------------------------------------------------------------------------- device-side packing
 // A training loop changes the weights every step; re-running the host builder (three programs, ~30 ms each) and
-// copying the parameters to the host and back would cost more than the step itself.  The structure of a program does
-// not depend on the values, so the builder is run ONCE in index mode and the packed streams / constant tables are
-// refreshed on the device from the caller's DEVICE tensors: V <- tensors, fold_kernel (the feature_linear fold, same
-// double-precision sums in the same order as the host), pack / constants kernels per program.  Bit-identical to a
-// fresh pnr_load_weights of the same values (tests/test_gpu_backward.py::test_update_weights_equals_fresh_load).
+// copying the parameters to the host and back would cost more than the step itself.  So each plan is built once, and
+// pnr_update_weights refreshes V from the caller's DEVICE tensors, folds (fold_kernel) and repacks every program with
+// the pack / constants kernels: bit-identical to a fresh pnr_load_weights of the same values.
 namespace {
 
 __global__ void pack_from_plan_kernel(const float* __restrict__ V, const int32_t* __restrict__ idx,
@@ -928,68 +969,27 @@ __global__ void consts_from_plan_kernel(const float* __restrict__ V, const int32
   if (p < n) out[p] = idx[p] < 0 ? 0.f : V[idx[p]];
 }
 
-// W' = W_view[:, :W] W_feat,  b' = W_view[:, :W] b_feat + b_view (double sums, j ascending, as on the host); the
-// gamma(d) columns of W_view are copied.  One thread per element of [W2, W + Ed] (+ one column for the bias).
-__global__ void fold_kernel(float* V, int64_t off_view_w, int64_t off_view_b, int64_t off_feat_w, int64_t off_feat_b,
-                            int W, int W2, int Ed, int64_t off_fold, int64_t off_fold_b) {
+// One thread per element of [W2, W + Ed + 1] (fold_element)
+__global__ void fold_kernel(float* V, Fold f) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int cols = W + Ed + 1;
-  if (i >= W2 * cols) return;
-  const int n = i / cols, k = i % cols;
-  const float* vrow = V + off_view_w + (int64_t)n * (W + Ed);
-  if (k < W) {
-    double acc = 0.0;
-    for (int j = 0; j < W; ++j) acc += (double)vrow[j] * (double)V[off_feat_w + (int64_t)j * W + k];
-    V[off_fold + (int64_t)n * (W + Ed) + k] = (float)acc;
-  } else if (k < W + Ed) {
-    V[off_fold + (int64_t)n * (W + Ed) + k] = vrow[k];
-  } else {
-    double acc = (double)V[off_view_b + n];
-    for (int j = 0; j < W; ++j) acc += (double)vrow[j] * (double)V[off_feat_b + j];
-    V[off_fold_b + n] = (float)acc;
-  }
+  const int cols = f.W + f.Ed + 1;
+  if (i < f.W / 2 * cols) fold_element(V, f, i / cols, i % cols);
 }
 
 }  // namespace
 
-// The device-side update plan of program `kind`: the program built once more in index mode, whose packed stream and
-// constants name the element of V each entry comes from.
-static int ensure_plan(pnr_ctx* ctx, ProgramKind kind) {
-  PackedProgram& pp = ctx->prog[kind];
-  if (pp.plan_ready) return PNR_OK;
-  const int n = (int)ctx->v_off.size();
-  std::vector<std::vector<float>> it(n);
-  std::vector<const float*> tp(n);
-  for (int i = 0; i < n; ++i) {
-    const int64_t cnt = ctx->all_shapes[2 * i] * ctx->all_shapes[2 * i + 1];
-    it[i].resize((size_t)cnt);
-    for (int64_t j = 0; j < cnt; ++j) it[i][(size_t)j] = (float)(ctx->v_off[i] + j + 1);
-    tp[i] = it[i].data();
-  }
-  Builder bld(ctx->passes, ctx->fmt);
-  bld.index_mode = true;
-  bld.derived_base = ctx->v_total;
-  if (const int rc = build_program_kind(kind, ctx->cfg, tp.data(), ctx->all_shapes.data(), n, bld)) return rc;
-  if (bld.wbuf.size() != pp.n_w || bld.consts.size() != pp.n_c)
-    return set_error(PNR_ERR_STATE, "pnr_update_weights: plan / program size mismatch (%zu/%zu vs %zu/%zu)", bld.wbuf.size(),
-                     bld.consts.size(), pp.n_w, pp.n_c);
-  std::vector<int32_t> widx(pp.n_w), cidx(pp.n_c);
-  for (size_t i = 0; i < widx.size(); ++i) widx[i] = (int32_t)bld.wsrc[i] - 1;
-  for (size_t i = 0; i < cidx.size(); ++i) cidx[i] = (int32_t)bld.consts[i] - 1;
-  PNR_CUDA(cudaMalloc(&pp.d_widx, pp.n_w * 4));
-  PNR_CUDA(cudaMalloc(&pp.d_wpart, pp.n_w));
-  PNR_CUDA(cudaMalloc(&pp.d_cidx, pp.n_c * 4));
-  PNR_CUDA(cudaMemcpy(pp.d_widx, widx.data(), pp.n_w * 4, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(pp.d_wpart, bld.wpart.data(), pp.n_w, cudaMemcpyHostToDevice));
-  PNR_CUDA(cudaMemcpy(pp.d_cidx, cidx.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
-  pp.plan_ready = true;
-  return PNR_OK;
-}
-
-// Packs program `kind`'s stream and constants from the weights in V, on `st`.
+// Packs program `kind`'s stream and constants from V, on `st`; its plan moves to the device the first time.
 static int refresh(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st) {
-  if (const int rc = ensure_plan(ctx, kind)) return rc;
-  const PackedProgram& pp = ctx->prog[kind];
+  PackedProgram& pp = ctx->prog[kind];
+  if (!pp.plan.wpos.empty()) {
+    PNR_CUDA(cudaMalloc(&pp.d_widx, pp.n_w * 4));
+    PNR_CUDA(cudaMalloc(&pp.d_wpart, pp.n_w));
+    PNR_CUDA(cudaMalloc(&pp.d_cidx, pp.n_c * 4));
+    PNR_CUDA(cudaMemcpy(pp.d_widx, pp.plan.wpos.data(), pp.n_w * 4, cudaMemcpyHostToDevice));
+    PNR_CUDA(cudaMemcpy(pp.d_wpart, pp.plan.wpart.data(), pp.n_w, cudaMemcpyHostToDevice));
+    PNR_CUDA(cudaMemcpy(pp.d_cidx, pp.plan.cpos.data(), pp.n_c * 4, cudaMemcpyHostToDevice));
+    pp.plan = Plan();
+  }
   pack_from_plan_kernel<<<(unsigned)((pp.n_w + 255) / 256), 256, 0, st>>>(ctx->d_V, pp.d_widx, pp.d_wpart, pp.n_w, ctx->fmt,
                                                                           reinterpret_cast<uint16_t*>(pp.d_wpacked), ctx->d_status);
   PNR_LAUNCH_CHECK("pack_from_plan_kernel");
@@ -1001,25 +1001,17 @@ static int refresh(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st) {
 extern "C" int pnr_update_weights(pnr_ctx* ctx, const float* const* device_tensors, int32_t n, void* stream) {
   PNR_CHECK_ARG(ctx && device_tensors, "pnr_update_weights: null pointer");
   if (!ctx->loaded) return set_error(PNR_ERR_STATE, "pnr_update_weights: pnr_load_weights has not been called (it fixes the shapes)");
-  PNR_CHECK_ARG(n == (int)ctx->v_off.size(), "pnr_update_weights: got %d tensors, pnr_load_weights had %d", n, (int)ctx->v_off.size());
+  const int n_loaded = (int)ctx->v_off.size() - 1;
+  PNR_CHECK_ARG(n == n_loaded, "pnr_update_weights: got %d tensors, pnr_load_weights had %d", n, n_loaded);
   for (int i = 0; i < n; ++i) PNR_CHECK_ARG(device_tensors[i], "pnr_update_weights: tensor %d is null", i);
-  if (ctx->v_total + ctx->v_derived + 1 >= (int64_t)1 << 24)   // the plans index V through fp32 values
-    return set_error(PNR_ERR_UNSUPPORTED, "pnr_update_weights: %lld values do not index exactly in fp32", (long long)ctx->v_total);
   DeviceGuard guard(ctx->cfg.device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!ctx->d_V) PNR_CUDA(cudaMalloc(&ctx->d_V, (size_t)(ctx->v_total + ctx->v_derived) * 4));
   for (int i = 0; i < n; ++i)
-    PNR_CUDA(cudaMemcpyAsync(ctx->d_V + ctx->v_off[i], device_tensors[i],
-                             (size_t)(ctx->all_shapes[2 * i] * ctx->all_shapes[2 * i + 1]) * 4, cudaMemcpyDeviceToDevice, st));
-  const int D = ctx->cfg.D, W = ctx->cfg.W, W2 = W / 2, Ed = 3 + 6 * ctx->cfg.view_res;
-  // tensor order (pnr_load_weights): trunk (w, b) x D, alpha, feature, view, rgb, heads
-  const int64_t off_feat_w = ctx->v_off[2 * D + 2], off_feat_b = ctx->v_off[2 * D + 3];
-  const int64_t off_view_w = ctx->v_off[2 * D + 4], off_view_b = ctx->v_off[2 * D + 5];
-  const int64_t off_fold = ctx->v_total, off_fold_b = ctx->v_total + (int64_t)W2 * (W + Ed);
-  fold_kernel<<<(W2 * (W + Ed + 1) + 127) / 128, 128, 0, st>>>(ctx->d_V, off_view_w, off_view_b, off_feat_w, off_feat_b, W, W2, Ed,
-                                                               off_fold, off_fold_b);
+    PNR_CUDA(cudaMemcpyAsync(ctx->d_V + ctx->v_off[i], device_tensors[i], (size_t)(ctx->v_off[i + 1] - ctx->v_off[i]) * 4,
+                             cudaMemcpyDeviceToDevice, st));
+  const Fold f = fold_of(ctx->cfg, ctx->v_off);
+  fold_kernel<<<(f.W / 2 * (f.W + f.Ed + 1) + 127) / 128, 128, 0, st>>>(ctx->d_V, f);
   PNR_LAUNCH_CHECK("fold_kernel");
-  ctx->device_weights = true;
   // the programs that exist follow; the others are packed from V when they are first built
   for (int k = 0; k < kNumPrograms; ++k)
     if (ctx->prog[k].ready)
@@ -1027,16 +1019,18 @@ extern "C" int pnr_update_weights(pnr_ctx* ctx, const float* const* device_tenso
   return PNR_OK;
 }
 
+// Program `kind` of a loaded context, built on first use and packed on the device from V.
 static int ensure_program(pnr_ctx* ctx, ProgramKind kind, cudaStream_t st) {
-  if (ctx->prog[kind].ready) return PNR_OK;   // the forward program always is: pnr_load_weights builds it
+  PackedProgram& pp = ctx->prog[kind];
+  if (pp.ready) return PNR_OK;   // the forward program always is: pnr_load_weights builds it
+  std::vector<const float*> tp(ctx->v_off.size() - 1);   // the loaded tensors, where they sit in V
+  for (size_t i = 0; i < tp.size(); ++i) tp[i] = ctx->d_V + ctx->v_off[i];
   Builder bld(ctx->passes, ctx->fmt);
-  std::vector<const float*> tp;
-  for (const auto& v : ctx->host_trunk) tp.push_back(v.data());
-  if (const int rc = build_program_kind(kind, ctx->cfg, tp.data(), ctx->host_trunk_shapes.data(), (int32_t)tp.size(), bld))
-    return rc;
-  if (const int rc = upload(ctx->prog[kind], bld)) return rc;
-  // the host copies are older than the weights in V: pack this program from V
-  return ctx->device_weights ? refresh(ctx, kind, st) : PNR_OK;
+  if (const int rc = build_program_kind(kind, ctx->cfg, tp.data(), ctx->shapes.data(), (int32_t)tp.size(), bld)) return rc;
+  if (const int rc = place(pp, bld)) return rc;
+  if (const int rc = refresh(ctx, kind, st)) return rc;
+  pp.ready = true;
+  return PNR_OK;
 }
 
 // dL/d(embedded xyz) through the trunk (the tensor-core part of the MLP backward, SURVEY 8f rank 2): the forward
