@@ -399,13 +399,16 @@ typedef struct pnr_render_args {
   void* workspace;              /* device scratch, caller-owned                                                   */
   size_t workspace_bytes;
 } pnr_render_args;
-/* ctx_fine: the network of the fine pass (NULL = ctx). */
+/* ctx_fine: the network of the fine pass (NULL = ctx), with the same num_classes and num_instances as ctx
+ * (PNR_ERR_ARG otherwise: the maps are [R,C] / [R,K] of ctx). */
 int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* args, void* stream);
 
 /* Bytes of device scratch pnr_render_fused wants for R rays: enough for one chunk of min(R, rays_per_chunk) rays
  * with every optional output absent, where rays_per_chunk puts `raw` near 1.5 GB and never below ~64 tiles of the
- * fused MLP per SM (smaller chunks cost more in kernel ramp-up than they save).  Any workspace that holds at
- * least one ray works (more chunks). */
+ * fused MLP per SM (smaller chunks cost more in kernel ramp-up than they save), and at least enough for
+ * min(R, ~64 samples per SM) rays of a sem_softmax call, whose passes keep `raw`.  So every call of R rays with
+ * M <= 8 renders in it.  Any workspace that holds at least one ray of the call works (more chunks); a smaller one is
+ * refused before any launch (PNR_ERR_ARG, "cannot hold one ray"). */
 size_t pnr_workspace_bytes(const pnr_ctx* ctx, int64_t R, int32_t N, int32_t Ni);
 
 /* 8(e) multi-GPU entry: one NCCL communicator per rank (NCCL is bound at run time: pnr_comm_available() == 0

@@ -115,13 +115,22 @@ int64_t default_chunk_rays(int Nt, int CH) {
 
 size_t workspace_bytes_for(int64_t R, int N, int Ni, int CH) {
   if (R <= 0) return 0;
-  Layout L = make_layout(N, Ni > 0 ? Ni : 0, CH, PNR_MAX_HITS, true, nullptr);
+  Ni = Ni > 0 ? Ni : 0;
+  Layout L = make_layout(N, Ni, CH, PNR_MAX_HITS, true, nullptr);
   // sized for the worst case (a caller may ask for softmax compositing, which needs raw) when raw is small, for the
   // one-kernel path otherwise: with both heads raw is 456 B per sample against ~20 B of everything else
   if (L.raw == 0 && CH <= 8) L.raw = (size_t)L.Nt * CH * 4;
   int64_t Rc = L.raw ? default_chunk_rays(L.Nt, CH) : R;
   if (Rc > R) Rc = R;
-  return chunk_bytes(L, Rc);
+  // A softmax call runs both passes on the two-kernel path, whose raw the one-kernel layout above leaves out: hold
+  // min(R, ~64 samples per SM) rays of that layout too (cfg3: at most ~3.8 MB more, nothing more for a full frame).
+  pnr_render_args softmax{};
+  softmax.sem_softmax = 1;
+  const Layout S = make_layout(N, Ni, CH, PNR_MAX_HITS, true, &softmax);
+  int64_t Rs = ((int64_t)num_sms() * 64 + S.Nt - 1) / S.Nt;
+  if (Rs > R) Rs = R;
+  const size_t b = chunk_bytes(L, Rc), bs = chunk_bytes(S, Rs);
+  return b > bs ? b : bs;
 }
 
 }  // namespace pnr
@@ -139,10 +148,13 @@ extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_rende
   if (a->R == 0) return PNR_OK;
   if (!ctx_fine) ctx_fine = ctx;
   const int N = a->N, Ni = a->Ni, M = a->M;
-  int C = 0, K = 0;
+  int C = 0, K = 0, Cf = 0, Kf = 0;
   ctx_classes(ctx, &C, &K);
+  ctx_classes(ctx_fine, &Cf, &Kf);
   const int CH = ctx_channels(ctx);
-  PNR_CHECK_ARG(ctx_channels(ctx_fine) == CH, "pnr_render_fused: coarse and fine networks differ in output channels");
+  // the maps are [R, C] / [R, K] of the coarse network, and both passes write them
+  PNR_CHECK_ARG(Cf == C && Kf == K, "pnr_render_fused: the fine network's heads (C=%d, K=%d) differ from the coarse "
+                "network's (C=%d, K=%d)", Cf, Kf, C, K);
   PNR_CHECK_ARG(a->R > 0 && a->rays, "pnr_render_fused: no rays");
   PNR_CHECK_ARG(N >= 1 && Ni >= 0 && N + Ni <= 256, "pnr_render_fused: N=%d, Ni=%d (N + Ni must be in [1,256])", N, Ni);
   PNR_CHECK_ARG(a->t_vals, "pnr_render_fused: t_vals is required (the caller's linspace(0,1,N))");

@@ -467,9 +467,20 @@ class Renderer:
         want = int(getattr(self.cfg, "workspace_mb", 0)) << 20
         chunk = int(getattr(self.cfg, "gpu_chunk", 0) or 0)
         if want <= 0 and chunk > 0:     # rays per chunk given instead of bytes
-            one = int(_capi.lib().pnr_workspace_bytes(ctx, 1, N, Ni))
-            want = int(_capi.lib().pnr_workspace_bytes(ctx, min(chunk, 1 << 16), N, Ni))
-            want += max(0, chunk - (1 << 16)) * one
+            ws = lambda r: int(_capi.lib().pnr_workspace_bytes(ctx, r, N, Ni))
+            want = ws(min(chunk, 1 << 16))
+            if chunk > 1 << 16:
+                # chunk rays of its layout.  pnr_workspace_bytes(R) is exactly R x the bytes per ray of that layout at R
+                # a multiple of 256 between the few softmax rays it always holds (< 2^14 rays) and its own chunk size,
+                # where it stops growing: find such an R (proportional to R + 256 as well); if there is none, fall back
+                # to the bytes of one ray.  Plus the alignment of up to 12 sub-buffers.
+                per_ray = ws(1)
+                for r in (1 << 14, 1 << 15, 1 << 16, 1 << 17):
+                    a, b = ws(r), ws(r + 256)
+                    if a * (r + 256) == b * r:
+                        per_ray = a // r
+                        break
+                want = max(want, chunk * per_ray + 12 * 256)
         if want <= 0:
             want = int(_capi.lib().pnr_workspace_bytes(ctx, R, N, Ni))
         ws = self._ws.get(str(device))
