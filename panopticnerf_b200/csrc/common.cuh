@@ -1,8 +1,11 @@
-// common.cuh — error plumbing and launch accounting shared by the libpnr translation units.
+// common.cuh — error plumbing, launch accounting and per-device launch facts shared by the libpnr translation units.
 #pragma once
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <mutex>
+#include <set>
+#include <utility>
 #include <cuda_runtime.h>
 #include "../../include/pnr.h"
 
@@ -54,6 +57,28 @@ inline int num_sms() {   // of the current device
   int dev = 0;
   cudaGetDevice(&dev);
   return num_sms(dev);
+}
+
+// The current device into *out; refused (`what` names the entry point) when its ordinal is past the per-device tables.
+inline int current_device(const char* what, int* out) {
+  int dev = 0;
+  PNR_CUDA(cudaGetDevice(&dev));
+  PNR_CHECK_ARG(dev >= 0 && dev < kMaxDevices, "%s: device ordinal %d >= %d", what, dev, kMaxDevices);
+  *out = dev;
+  return PNR_OK;
+}
+
+// Lets `kernel` use `bytes` (> 48 KB) of dynamic shared memory on device `dev`.  The opt-in is a per-device function
+// attribute: it is set once per (kernel, device).
+inline int opt_in_smem(const void* kernel, int bytes, int dev) {
+  static std::mutex mu;
+  static std::set<std::pair<const void*, int>> done;
+  std::lock_guard<std::mutex> lock(mu);
+  if (done.count({kernel, dev}) == 0) {
+    PNR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done.insert({kernel, dev});
+  }
+  return PNR_OK;
 }
 
 // Makes `dev` current for a scope and restores the caller's device afterwards (the library never leaves the

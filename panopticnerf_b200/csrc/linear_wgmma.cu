@@ -17,7 +17,6 @@
 //     registers; after the tile's last chunk: * 1/scale, + bias, optional ReLU, stores to the samples' rows of y.
 // HBM-bound by construction for the shapes of this network (4 (K + N) bytes per sample against 6 K N tensor flops).
 #include <cstddef>
-#include <mutex>
 #include "common.cuh"
 #include "sm90.cuh"
 
@@ -67,26 +66,6 @@ __global__ void linear_pack_kernel(const float* __restrict__ W, int64_t ld_w, in
   uint8_t* img = out + (size_t)c * (2 * 8 * NP * 16) + (size_t)(kc * NP + row) * 16;
   *reinterpret_cast<uint4*>(img) = make_uint4(h[0], h[1], h[2], h[3]);
   *reinterpret_cast<uint4*>(img + 8 * NP * 16) = make_uint4(l[0], l[1], l[2], l[3]);
-}
-
-// N = 16 .. 256 as two wgmma halves of <= 128 columns (the second half starts at weight row 128)
-template <int FMT>
-__device__ __forceinline__ void ln_mma(float (&d0)[64], float (&d1)[64], int NP, uint64_t a_hi, uint64_t a_lo, uint64_t b_hi,
-                                       uint64_t b_lo, int ksteps, uint32_t b_inc16, uint32_t acc) {
-  const int n0 = NP < 128 ? NP : 128;
-  const uint64_t h1 = (128u * 16u) >> 4;   // row 128 of the weight images, 16-byte units
-  wgmma_fence();
-#define PNR_LN_N(NN, D, BH, BL) \
-  case NN / 8: mma_run<NN, 3, FMT>(D, a_hi, a_lo, BH, BL, ksteps, (2u * kLnALbo) >> 4, b_inc16, acc); break;
-#define PNR_LN_ALL(D, BH, BL)                                                                                     \
-  PNR_LN_N(16, D, BH, BL) PNR_LN_N(32, D, BH, BL) PNR_LN_N(48, D, BH, BL) PNR_LN_N(64, D, BH, BL)                    \
-  PNR_LN_N(80, D, BH, BL) PNR_LN_N(96, D, BH, BL) PNR_LN_N(112, D, BH, BL) PNR_LN_N(128, D, BH, BL)
-  switch (n0 >> 3) { PNR_LN_ALL(d0, b_hi, b_lo) default: __trap(); }   // (NP: N rounded up to 16, N <= 256 by the argument checks)
-  if (NP > 128) {
-    switch ((NP - 128) >> 3) { PNR_LN_ALL(d1, b_hi + h1, b_lo + h1) default: __trap(); }   // (NP: N rounded up to 16, N <= 256 by the argument checks)
-  }
-#undef PNR_LN_ALL
-#undef PNR_LN_N
 }
 
 template <int FMT>
@@ -172,9 +151,10 @@ __global__ void __launch_bounds__(kLnThreads, 1) linear_kernel(const LinearParam
         const uint32_t sb = smem_u32(smem + kLnSmemB + slot * kLnBStageMax);
         const int kleft = p.K - c * kLnChunk;
         const int ksteps = kleft >= kLnChunk ? kLnChunk / 16 : (kleft + 15) / 16;
-        ln_mma<FMT>(acc0, acc1, p.NP, make_smem_desc_noswz(sa, kLnALbo, 128), make_smem_desc_noswz(sa + kLnAPart, kLnALbo, 128),
-                    make_smem_desc_noswz(sb, b_lbo, 128), make_smem_desc_noswz(sb + b_part, b_lbo, 128), ksteps,
-                    (2u * b_lbo) >> 4, c == 0 ? 0u : 1u);
+        mma_run_halves<FMT>(acc0, acc1, p.NP, make_smem_desc_noswz(sa, kLnALbo, 128),
+                            make_smem_desc_noswz(sa + kLnAPart, kLnALbo, 128), make_smem_desc_noswz(sb, b_lbo, 128),
+                            make_smem_desc_noswz(sb + b_part, b_lbo, 128), ksteps, (2u * kLnALbo) >> 4, (2u * b_lbo) >> 4,
+                            c == 0 ? 0u : 1u);
         wgmma_commit();
         wgmma_wait<1>();   // the previous chunk's MMAs have retired: its weight slot is free (its A slot is rewritten next)
         if (g > 0 && lane == 0) mbar_arrive(bar_b_empty + 8 * ((g - 1) & 1u));
@@ -211,19 +191,10 @@ __global__ void __launch_bounds__(kLnThreads, 1) linear_kernel(const LinearParam
   }
 }
 
-static bool g_ln_attr[kMaxDevices][2] = {};
-static std::mutex g_ln_mutex;
-
 template <int FMT>
 static int linear_launch(const LinearParams& p, const float* W, int64_t ld_w, int trans, uint8_t* wpk, int dev, cudaStream_t st) {
-  {
-    std::lock_guard<std::mutex> lock(g_ln_mutex);
-    bool& done = g_ln_attr[dev][FMT == kFmtBF16];
-    if (!done) {
-      PNR_CUDA(cudaFuncSetAttribute(linear_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLnSmemTotal));
-      done = true;
-    }
-  }
+  const int rc = opt_in_smem((const void*)linear_kernel<FMT>, kLnSmemTotal, dev);
+  if (rc != PNR_OK) return rc;
   const int n_pack = p.n_chunks * 8 * p.NP;
   linear_pack_kernel<FMT><<<(n_pack + 127) / 128, 128, 0, st>>>(W, ld_w, p.N, p.K, p.NP, p.n_chunks, trans, wpk);
   PNR_LAUNCH_CHECK("linear_pack_kernel");
@@ -264,8 +235,8 @@ extern "C" int pnr_linear(const float* x, int64_t ld_x, int32_t K, const float* 
   if (S == 0) return PNR_OK;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int dev = 0;
-  PNR_CUDA(cudaGetDevice(&dev));
-  PNR_CHECK_ARG(dev >= 0 && dev < kMaxDevices, "pnr_linear: device ordinal %d >= %d", dev, kMaxDevices);
+  const int rc = current_device("pnr_linear", &dev);
+  if (rc != PNR_OK) return rc;
   LinearParams p;
   p.x = x; p.ld_x = ld_x; p.K = K;
   p.wpk = static_cast<const uint8_t*>(workspace);

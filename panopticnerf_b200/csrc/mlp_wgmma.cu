@@ -28,7 +28,6 @@
 // An activation outside the operand format's range (|x| > 65504 in the fp16 modes, non-finite in any) sets
 // bit 0 of the context's sticky status word: overflow is reported (pnr_status), never silent.
 #include <cstddef>
-#include <mutex>
 #include "common.cuh"
 #include "composite_math.cuh"
 #include "hashgrid_math.cuh"
@@ -877,26 +876,11 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
   }
 }
 
-// Per-device launch state: the > 48 KB dynamic shared-memory opt-in is a per-device function attribute, and so
-// is the SM count the persistent grid is sized by.
-struct DeviceState {
-  bool attr_done[2][2][3] = {};   // [x3][bf16][plain / compositing epilogue / backward program]
-};
-static DeviceState g_dev[kMaxDevices];
-static std::mutex g_dev_mutex;
-
 template <int PASSES, int FMT, bool COMP, bool BWD = false>
 static int launch_one(const MlpLaunch& L, int dev, int grid, cudaStream_t stream) {
   constexpr int kSmem = COMP ? kSmemTotalComp : kSmemTotal;
-  {
-    std::lock_guard<std::mutex> lock(g_dev_mutex);
-    bool& done = g_dev[dev].attr_done[PASSES == 3][FMT == kFmtBF16][BWD ? 2 : (COMP ? 1 : 0)];
-    if (!done) {
-      PNR_CUDA(cudaFuncSetAttribute(mlp_fused_kernel<PASSES, FMT, COMP, BWD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    kSmem));
-      done = true;
-    }
-  }
+  const int rc = opt_in_smem((const void*)mlp_fused_kernel<PASSES, FMT, COMP, BWD>, kSmem, dev);
+  if (rc != PNR_OK) return rc;
   mlp_fused_kernel<PASSES, FMT, COMP, BWD><<<grid, kMlpThreads, kSmem, stream>>>(L);
   PNR_LAUNCH_CHECK("mlp_fused_kernel");
   return PNR_OK;
@@ -908,8 +892,8 @@ static int launch_one(const MlpLaunch& L, int dev, int grid, cudaStream_t stream
 int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream) {
   const bool composite = mode == kMlpComposite;
   int dev = 0;
-  PNR_CUDA(cudaGetDevice(&dev));
-  PNR_CHECK_ARG(dev >= 0 && dev < kMaxDevices, "launch_mlp: device ordinal %d >= %d", dev, kMaxDevices);
+  const int rc = current_device("launch_mlp", &dev);
+  if (rc != PNR_OK) return rc;
   const int sms = num_sms(dev);
   const int64_t tiles = (L.p.S + kRows - 1) / kRows;
   PNR_CHECK_ARG(tiles < ((int64_t)1 << 31), "launch_mlp: too many samples");

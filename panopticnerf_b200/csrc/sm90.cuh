@@ -142,6 +142,28 @@ __device__ __forceinline__ void mma_run(float* d, uint64_t a_hi, uint64_t a_lo, 
   }
 }
 
+// mma_run (x3) over NP = 16 .. 256 columns (N rounded up to 16) as two wgmma halves of <= 128 columns: the first into
+// d0, the rest - from row 128 of the B images on - into d1.  Fences; the caller commits and waits.
+template <int FMT>
+__device__ __forceinline__ void mma_run_halves(float (&d0)[64], float (&d1)[64], int NP, uint64_t a_hi, uint64_t a_lo,
+                                               uint64_t b_hi, uint64_t b_lo, int ksteps, uint32_t a_inc16,
+                                               uint32_t b_inc16, uint32_t acc) {
+  const int n0 = NP < 128 ? NP : 128;
+  const uint64_t h1 = (128u * 16u) >> 4;   // row 128 of the B images, 16-byte units
+  wgmma_fence();
+#define PNR_HALF_N(NN, D, BH, BL) \
+  case NN / 8: mma_run<NN, 3, FMT>(D, a_hi, a_lo, BH, BL, ksteps, a_inc16, b_inc16, acc); break;
+#define PNR_HALF_ALL(D, BH, BL)                                                                                   \
+  PNR_HALF_N(16, D, BH, BL) PNR_HALF_N(32, D, BH, BL) PNR_HALF_N(48, D, BH, BL) PNR_HALF_N(64, D, BH, BL)            \
+  PNR_HALF_N(80, D, BH, BL) PNR_HALF_N(96, D, BH, BL) PNR_HALF_N(112, D, BH, BL) PNR_HALF_N(128, D, BH, BL)
+  switch (n0 >> 3) { PNR_HALF_ALL(d0, b_hi, b_lo) default: __trap(); }   // not a multiple of 16
+  if (NP > 128) {
+    switch ((NP - 128) >> 3) { PNR_HALF_ALL(d1, b_hi + h1, b_lo + h1) default: __trap(); }
+  }
+#undef PNR_HALF_ALL
+#undef PNR_HALF_N
+}
+
 // ---------------------------------------------------------------- 16-bit hi/lo split
 // x = hi + lo + residual, both parts rounded to nearest even in the operand format:
 //   bf16 (8-bit significand):  residual <= 2^-18 |x|, fp32 exponent range (never overflows)

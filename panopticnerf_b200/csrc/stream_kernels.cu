@@ -5,7 +5,6 @@
 //   composite : one warp per ray; lanes stride the sample axis; transmittance is an exclusive
 //               product scan done with warp shuffles; per-class logits are accumulated with lanes
 //               striding the (contiguous) channel axis so every raw row is read once, coalesced.
-#include <mutex>
 #include "common.cuh"
 #include "composite_math.cuh"
 #include "ray_math.h"
@@ -546,20 +545,12 @@ extern "C" int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void
   if (n == 0) return PNR_OK;
   PNR_CHECK_ARG(x && out, "pnr_encode: null pointer");
   PNR_CHECK_ARG(L >= 0 && L <= 16, "pnr_encode: L=%d outside [0,16]", L);
-  if (n == 0) return PNR_OK;
   const size_t smem = (size_t)kEncTile * (3 + 6 * L) * sizeof(float);
-  {   // the > 48 KB dynamic shared-memory opt-in is a per-device function attribute
-    static bool attr_set[kMaxDevices] = {false};
-    static std::mutex mu;
-    int dev = 0;
-    PNR_CUDA(cudaGetDevice(&dev));
-    PNR_CHECK_ARG(dev >= 0 && dev < kMaxDevices, "pnr_encode: device ordinal %d >= %d", dev, kMaxDevices);
-    std::lock_guard<std::mutex> lock(mu);
-    if (!attr_set[dev]) {
-      PNR_CUDA(cudaFuncSetAttribute(encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-      attr_set[dev] = true;
-    }
-  }
+  int dev = 0;
+  int rc = current_device("pnr_encode", &dev);
+  if (rc != PNR_OK) return rc;
+  rc = opt_in_smem((const void*)encode_kernel, 64 * 1024, dev);
+  if (rc != PNR_OK) return rc;
   encode_kernel<<<(unsigned)((n + kEncTile - 1) / kEncTile), kEncTile, smem, (cudaStream_t)stream>>>(
       x, n, L, out);
   PNR_LAUNCH_CHECK("encode_kernel");
@@ -578,7 +569,6 @@ extern "C" int pnr_composite(const float* raw, const float* z, const float* rays
                 32 * kCompMaxPerLane);
   PNR_CHECK_ARG(C >= 0 && C <= 32 * kCompMaxChan && K >= 0 && K <= 32 * kCompMaxChan,
                 "pnr_composite: C=%d or K=%d outside [0,%d]", C, K, 32 * kCompMaxChan);
-  if (R == 0) return PNR_OK;
   CompositeArgs a;
   a.raw = raw; a.z = z; a.rays = rays; a.R = R; a.N = N; a.C = C; a.K = K; a.CH = 4 + C + K;
   a.white_bkgd = white_bkgd; a.sem_softmax = sem_softmax; a.mask_outside = mask_outside;

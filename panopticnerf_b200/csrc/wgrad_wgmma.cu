@@ -20,7 +20,6 @@
 // The kernel is HBM-bound: 4 (No + Ni) bytes per sample against 6 No Ni tensor flops; X is read once per block of
 // 128 output rows.
 #include <cstddef>
-#include <mutex>
 #include "common.cuh"
 #include "sm90.cuh"
 
@@ -152,21 +151,9 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_kernel(const WgradParams 
     const uint32_t sa = smem_u32(stage) + (uint32_t)(wg * 64 * 16), sb = smem_u32(stage) + 2u * kWgAPart;
     const uint64_t a_hi = make_smem_desc_noswz(sa, kWgALbo, 128), a_lo = make_smem_desc_noswz(sa + kWgAPart, kWgALbo, 128);
     const uint64_t b_hi = make_smem_desc_noswz(sb, b_lbo, 128), b_lo = make_smem_desc_noswz(sb + kWgBPart, b_lbo, 128);
-    const uint64_t h1 = (128u * 16u) >> 4;   // row 128 of the B images
     const int n0 = p.NP < 128 ? p.NP : 128;
     const uint32_t acc = i % kWgFlush == 0 ? 0u : 1u;   // a run restarts after each flush
-    wgmma_fence();
-#define PNR_WG_N(NN, D, BH, BL) \
-  case NN / 8: mma_run<NN, 3, FMT>(D, a_hi, a_lo, BH, BL, kWgSlab / 16, (2u * kWgALbo) >> 4, (2u * kWgBLbo) >> 4, acc); break;
-#define PNR_WG_ALL(D, BH, BL)                                                                                     \
-  PNR_WG_N(16, D, BH, BL) PNR_WG_N(32, D, BH, BL) PNR_WG_N(48, D, BH, BL) PNR_WG_N(64, D, BH, BL)                    \
-  PNR_WG_N(80, D, BH, BL) PNR_WG_N(96, D, BH, BL) PNR_WG_N(112, D, BH, BL) PNR_WG_N(128, D, BH, BL)
-    switch (n0 >> 3) { PNR_WG_ALL(acc0, b_hi, b_lo) default: __trap(); }   // (NP: N rounded up to 16, N <= 256 by the argument checks)
-    if (p.NP > 128) {
-      switch ((p.NP - 128) >> 3) { PNR_WG_ALL(acc1, b_hi + h1, b_lo + h1) default: __trap(); }   // (NP: N rounded up to 16, N <= 256 by the argument checks)
-    }
-#undef PNR_WG_ALL
-#undef PNR_WG_N
+    mma_run_halves<FMT>(acc0, acc1, p.NP, a_hi, a_lo, b_hi, b_lo, kWgSlab / 16, (2u * kWgALbo) >> 4, (2u * kWgBLbo) >> 4, acc);
     wgmma_commit();
     wgmma_wait<1>();   // slab i - 1's MMAs have retired: its slot may be rewritten by slab i + 1
     __syncthreads();   // (by either warpgroup)
@@ -222,9 +209,6 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, const float*
   }
 }
 
-static bool g_wg_attr[kMaxDevices][2] = {};
-static std::mutex g_wg_mutex;
-
 // CTAs along the samples: one per SM over all output blocks, at most one per slab (<= num_sms: the workspace size)
 static int wgrad_grid(int64_t S, int mh, int dev) {
   const int64_t n_slabs = (S + kWgSlab - 1) / kWgSlab;
@@ -244,14 +228,8 @@ extern "C" size_t pnr_wgrad_workspace_bytes(int32_t No, int32_t Ni) {
 
 template <int FMT>
 static int wgrad_launch(const WgradParams& p, int grid, int dev, cudaStream_t st) {
-  {
-    std::lock_guard<std::mutex> lock(g_wg_mutex);
-    bool& done = g_wg_attr[dev][FMT == kFmtBF16];
-    if (!done) {
-      PNR_CUDA(cudaFuncSetAttribute(wgrad_kernel<FMT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemTotal));
-      done = true;
-    }
-  }
+  const int rc = opt_in_smem((const void*)wgrad_kernel<FMT>, kWgSmemTotal, dev);
+  if (rc != PNR_OK) return rc;
   wgrad_kernel<FMT><<<dim3(grid, p.mh), kWgThreads, kWgSmemTotal, st>>>(p);
   PNR_LAUNCH_CHECK("wgrad_kernel");
   return PNR_OK;
@@ -269,8 +247,8 @@ extern "C" int pnr_wgrad(const float* dz, int64_t ld_dz, int32_t No, const float
   PNR_CHECK_ARG(S >= 0, "pnr_wgrad: S = %lld", (long long)S);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   int dev = 0;
-  PNR_CUDA(cudaGetDevice(&dev));
-  PNR_CHECK_ARG(dev >= 0 && dev < kMaxDevices, "pnr_wgrad: device ordinal %d >= %d", dev, kMaxDevices);
+  int rc = current_device("pnr_wgrad", &dev);
+  if (rc != PNR_OK) return rc;
   const int mh = No > 128 ? 2 : 1, NP = (Ni + 15) / 16 * 16;
   const int grid = S > 0 ? wgrad_grid(S, mh, dev) : 0;
   const size_t need = (size_t)grid * ((size_t)mh * 128 * NP + kWgRows) * sizeof(float);
@@ -287,7 +265,7 @@ extern "C" int pnr_wgrad(const float* dz, int64_t ld_dz, int32_t No, const float
   p.vec_a = (reinterpret_cast<uintptr_t>(dz) & 15) == 0 && (ld_dz & 3) == 0;
   p.vec_b = (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (ld_x & 3) == 0;
   if (grid > 0) {
-    const int rc = precision == PNR_PREC_FP16X3 ? wgrad_launch<kFmtF16>(p, grid, dev, st) : wgrad_launch<kFmtBF16>(p, grid, dev, st);
+    rc = precision == PNR_PREC_FP16X3 ? wgrad_launch<kFmtF16>(p, grid, dev, st) : wgrad_launch<kFmtBF16>(p, grid, dev, st);
     if (rc != PNR_OK) return rc;
   }
   const int n = No * NP;
