@@ -168,3 +168,9 @@ def ptr(t: Optional[torch.Tensor], dtype: Optional[torch.dtype] = None, name: st
     if not t.is_contiguous():
         raise PnrError(f"{name}: expected a contiguous tensor")
     return t.data_ptr()
+
+
+def ptr_struct(cls, tensors):
+    """A struct of device pointers (PnrCompositeOut, PnrCompositeGrads) from tensors by field name; a field missing
+    from `tensors` or None there is NULL."""
+    return cls(**{k: ptr(tensors.get(k)) for k, _ in cls._fields_})

@@ -1,6 +1,7 @@
 // composite_math.cuh — the per-sample arithmetic of alpha compositing (SURVEY.md 8(a) a9), shared by the standalone
-// compositing kernel (stream_kernels.cu) and the compositing epilogue of the fused MLP kernel (mlp_tc05.cu), so
-// that both produce the same per-sample weights bit for bit (the fine sampler consumes them).
+// compositing kernel and its backward (stream_kernels.cu) and the compositing epilogue of the fused MLP kernel
+// (mlp_wgmma.cu), so that all three produce the same per-sample weights bit for bit (the fine sampler consumes them,
+// the backward differentiates them).
 //
 // A ray's samples are handled in aligned groups of 32 (one warp, lane = sample index mod 32):
 //   alpha_i = 1 - exp(-relu(sigma_i) * dist_i),   t_i = 1 - alpha_i + 1e-10,

@@ -237,7 +237,8 @@ __global__ void __launch_bounds__(kCompWarps * 32) composite_kernel(CompositeArg
 //   dL/dalpha_i = G_i T_i - (sum_{j>i} G_j w_j) / t_i,   dalpha/dsigma = delta_i exp(-sigma_i delta_i),
 //   dL/dc_i = w_i g_rgb (through the sigmoid), dL/ds_i = w_i g_sem, dL/du_i = w_i g_inst.
 // Same work distribution as the forward kernel: one warp per ray, lanes stride samples for the scans and
-// channels for the logits; T is recomputed with the forward's scan so that w matches it bit for bit.
+// channels for the logits; T is recomputed with the forward's arithmetic (composite_math.cuh) so that w matches it
+// bit for bit.
 struct CompositeBwdArgs {
   const float* raw; const float* z; const float* rays;
   int64_t R; int N, C, K, CH;
@@ -256,7 +257,7 @@ __global__ void __launch_bounds__(kCompWarps * 32) composite_backward_kernel(Com
   float* d_raw = a.d_raw + r * N * CH;
   const float* z = a.z + r * N;
   const float dx = a.rays[r * 6 + 3], dy = a.rays[r * 6 + 4], dz = a.rays[r * 6 + 5];
-  const float dnorm = sqrtf(dx * dx + dy * dy + dz * dz);
+  const float dnorm = comp_dnorm(dx, dy, dz);
   float g_r = 0.f, g_g = 0.f, g_b = 0.f;
   if (a.g.rgb_map) { g_r = a.g.rgb_map[r * 3 + 0]; g_g = a.g.rgb_map[r * 3 + 1]; g_b = a.g.rgb_map[r * 3 + 2]; }
   const float g_depth = a.g.depth_map ? a.g.depth_map[r] : 0.f;
@@ -278,19 +279,19 @@ __global__ void __launch_bounds__(kCompWarps * 32) composite_backward_kernel(Com
     float cr = 0.f, cg = 0.f, cb = 0.f;
     if (i < N) {
       const float zi = z[i];
-      const float dist = ((i + 1 < N) ? (z[i + 1] - zi) : 1e10f) * dnorm;
+      const float dist = comp_dist(zi, (i + 1 < N) ? z[i + 1] : 0.f, i + 1 < N, dnorm);
       const float* q = raw + (int64_t)i * CH;
       float sig = fmaxf(q[3], 0.f);
       bool live = q[3] > 0.f;
       int32_t sb = -1;
       if (a.sample_box != nullptr) sb = a.sample_box[r * N + i];
       if (a.mask_outside && a.sample_box != nullptr && sb < 0) { sig = 0.f; live = false; }
-      const float e = expf(-sig * dist);
+      const float e = expf(-sig * dist);   // comp_alpha's exp, kept: 1 - alpha is not e in fp32
       alpha = 1.0f - e;
       ds = live ? dist * e : 0.f;                       // dalpha / draw_sigma
-      cr = 1.0f / (1.0f + expf(-q[0]));
-      cg = 1.0f / (1.0f + expf(-q[1]));
-      cb = 1.0f / (1.0f + expf(-q[2]));
+      cr = comp_sigmoid(q[0]);
+      cg = comp_sigmoid(q[1]);
+      cb = comp_sigmoid(q[2]);
       Gi = g_r * cr + g_g * cg + g_b * cb + g_depth * zi + g_acc;
       if (a.g.weights) Gi += a.g.weights[r * N + i];
       if (sb >= 0 && sb < a.B) {
@@ -300,16 +301,9 @@ __global__ void __launch_bounds__(kCompWarps * 32) composite_backward_kernel(Com
     }
     const float t = (i < N) ? (1.0f - alpha + 1e-10f) : 1.0f;
     tv[j] = t;
-    float incl = t;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const float o = __shfl_up_sync(0xffffffffu, incl, d);
-      if (lane >= d) incl *= o;
-    }
-    float excl = __shfl_up_sync(0xffffffffu, incl, 1);
-    if (lane == 0) excl = 1.0f;
-    T[j] = carry * excl;
-    carry *= __shfl_sync(0xffffffffu, incl, 31);
+    float total;
+    T[j] = carry * comp_scan32(t, lane, &total);
+    carry *= total;
     w[j] = alpha * T[j];
     G[j] = Gi;
     dsig[j] = ds;

@@ -27,6 +27,7 @@ import torch.nn as nn
 
 from panopticnerf_b200 import _capi
 from panopticnerf_b200.lib.networks.encoding import HashGrid
+from panopticnerf_b200.lib.networks.renderer.panopticnerf_renderer import empty_composite_maps, primitive_tables
 
 
 def embed_dim(L: int) -> int:
@@ -230,27 +231,16 @@ class Network(nn.Module):
                           mask_outside: bool = False, sample_box: Optional[torch.Tensor] = None,
                           box_sem: Optional[torch.Tensor] = None, box_inst: Optional[torch.Tensor] = None):
         """Network.forward + raw2outputs in ONE kernel (pnr_mlp_composite): the compositing runs in the MLP's epilogue
-        and `raw` is never written.  Returns the dict raw2outputs returns.  Needs N % 32 == 0."""
+        and `raw` is never written.  Returns the dict raw2outputs returns.  Needs N % 32 == 0; the primitive tables are
+        refused, as by raw2outputs, when they live on another device or the id tables differ in length."""
         R, N = z.shape
         dev = rays.device
         ctx = self.pack(dev if rays.is_cuda else None)
         rp, zp = _capi.ptr(rays, torch.float32, "rays"), _capi.ptr(z, torch.float32, "z")
-        e = lambda *shape: torch.empty(*shape, dtype=torch.float32, device=dev)
-        out = {"rgb_map": e(R, 3), "depth_map": e(R), "acc_map": e(R), "disp_map": e(R), "weights": e(R, N)}
-        if self.C > 0:
-            out["semantic_map"] = e(R, self.C)
-        if self.K > 0:
-            out["instance_map"] = e(R, self.K)
-        sb = sample_box.to(dev, torch.int32).contiguous() if sample_box is not None else None
-        bs = box_sem.to(dev, torch.int32).contiguous() if box_sem is not None else None
-        bi = box_inst.to(dev, torch.int32).contiguous() if box_inst is not None else None
-        B = 0
-        if sb is not None and bs is not None and self.C > 0:
-            out["fixed_semantic_map"], B = e(R, self.C), bs.shape[0]
-        if sb is not None and bi is not None and self.K > 0:
-            out["fixed_instance_map"], B = e(R, self.K), bi.shape[0]
-        co = _capi.PnrCompositeOut(**{k: _capi.ptr(out[k]) if k in out else None
-                                      for k, _ in _capi.PnrCompositeOut._fields_})
+        sb, bs, bi, B = primitive_tables(rays, sample_box, box_sem, box_inst)
+        out = empty_composite_maps(R, N, self.C, self.K, sb is not None and bs is not None,
+                                   sb is not None and bi is not None, dev)
+        co = _capi.ptr_struct(_capi.PnrCompositeOut, out)
         with torch.cuda.device(dev):
             _capi.check(_capi.lib().pnr_mlp_composite(ctx, rp, zp, R, N, int(bool(white_bkgd)), int(bool(mask_outside)),
                                                       _capi.ptr(sb), _capi.ptr(bs), _capi.ptr(bi), B, C.byref(co),

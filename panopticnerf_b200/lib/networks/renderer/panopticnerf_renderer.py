@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import ctypes as C
 import functools
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import torch
 
@@ -40,10 +40,57 @@ def _on_tensor_device(fn):
     return wrapper
 
 
-def _same_device(ref: torch.Tensor, **tensors) -> None:
-    for name, t in tensors.items():
+# ------------------------------------------------------------------------------------------------
+# what every compositing call (pnr_composite, pnr_composite_backward, pnr_mlp_composite, pnr_render_fused) shares
+# ------------------------------------------------------------------------------------------------
+def composite_map_keys(C: int, K: int, fixed_sem: bool, fixed_inst: bool) -> List[str]:
+    """The maps a compositing call produces, in the order it returns them: rgb / depth / acc / disp / weights always,
+    semantic_map if C > 0, instance_map if K > 0, and a fixed (bounding-box) map when it is wanted (per-sample
+    primitive ids and that id table given) and its head exists."""
+    keys = ["rgb_map", "depth_map", "acc_map", "disp_map", "weights"]
+    if C > 0:
+        keys.append("semantic_map")
+    if K > 0:
+        keys.append("instance_map")
+    if fixed_sem and C > 0:
+        keys.append("fixed_semantic_map")
+    if fixed_inst and K > 0:
+        keys.append("fixed_instance_map")
+    return keys
+
+
+def _map_shapes(R: int, n: int, C: int, K: int) -> Dict[str, tuple]:
+    return {"rgb_map": (R, 3), "depth_map": (R,), "acc_map": (R,), "disp_map": (R,), "weights": (R, n),
+            "semantic_map": (R, C), "instance_map": (R, K), "fixed_semantic_map": (R, C), "fixed_instance_map": (R, K)}
+
+
+def empty_composite_maps(R: int, n: int, C: int, K: int, fixed_sem: bool, fixed_inst: bool,
+                         device) -> Dict[str, torch.Tensor]:
+    """Uninitialised float32 maps of `composite_map_keys` for R rays of n samples on `device`."""
+    shapes = _map_shapes(R, n, C, K)
+    return {k: torch.empty(shapes[k], dtype=_F32, device=device) for k in composite_map_keys(C, K, fixed_sem, fixed_inst)}
+
+
+def primitive_tables(ref: torch.Tensor, sample_box, box_sem, box_inst):
+    """(sample_box, box_sem, box_inst, B) as the compositing kernels take them: each table int32 and contiguous (None
+    stays None) and B, the one bound of both id tables, which sample_box indexes (0 without sample_box).  The tables
+    must live on ref's device and, with sample_box, the id tables must have the same length."""
+    for name, t in (("sample_box", sample_box), ("box_sem", box_sem), ("box_inst", box_inst)):
         if t is not None and t.device != ref.device:
             raise _capi.PnrError(f"{name} is on {t.device}, expected {ref.device}")
+    B = 0
+    if sample_box is not None:
+        sizes = {int(t.shape[0]) for t in (box_sem, box_inst) if t is not None}
+        if len(sizes) > 1:
+            raise ValueError(f"box_sem and box_inst must have one entry per primitive each, got lengths {sorted(sizes)}")
+        B = sizes.pop() if sizes else 0
+    sb, bs, bi = (t.to(_I32).contiguous() if t is not None else None for t in (sample_box, box_sem, box_inst))
+    return sb, bs, bi, B
+
+
+def _rays(rays_d: torch.Tensor) -> torch.Tensor:
+    """rays [R,6] for the compositing kernels, which read only the directions: rays_d [R,3] gets zero origins."""
+    return _f(torch.cat([torch.zeros_like(rays_d), rays_d], -1) if rays_d.shape[-1] == 3 else rays_d, "rays")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -164,18 +211,6 @@ def embed(x: torch.Tensor, L: int) -> torch.Tensor:
     return out.reshape(*x.shape[:-1], 3 + 6 * L)
 
 
-def _box_table_size(raw, sample_box, box_sem, box_inst) -> int:
-    """One B bounds both id tables in the kernel (sample_box indexes them): they must have the same length and
-    live on raw's device."""
-    _same_device(raw, sample_box=sample_box, box_sem=box_sem, box_inst=box_inst)
-    if sample_box is None:
-        return 0
-    sizes = {int(t.shape[0]) for t in (box_sem, box_inst) if t is not None}
-    if len(sizes) > 1:
-        raise ValueError(f"box_sem and box_inst must have one entry per primitive each, got lengths {sorted(sizes)}")
-    return sizes.pop() if sizes else 0
-
-
 @_on_tensor_device
 def raw2outputs(raw, z_vals, rays_d, raw_noise_std: float = 0.0, white_bkgd: bool = False,
                 num_classes: int = 0, num_instances: int = 0, sem_activation: str = "none",
@@ -192,33 +227,14 @@ def raw2outputs(raw, z_vals, rays_d, raw_noise_std: float = 0.0, white_bkgd: boo
         nz = noise if noise is not None else torch.randn(R, N, device=raw.device)
         raw = raw.clone()
         raw[..., 3] += nz.to(raw.device, _F32) * raw_noise_std
-    if rays_d.shape[-1] == 3:
-        rays = torch.cat([torch.zeros_like(rays_d), rays_d], -1)
-    else:
-        rays = rays_d
-    rays = _f(rays, "rays")
-    dev = raw.device
-    out = {"rgb_map": torch.empty(R, 3, dtype=_F32, device=dev), "depth_map": torch.empty(R, dtype=_F32, device=dev),
-           "acc_map": torch.empty(R, dtype=_F32, device=dev), "disp_map": torch.empty(R, dtype=_F32, device=dev),
-           "weights": torch.empty(R, N, dtype=_F32, device=dev)}
-    if Cn > 0:
-        out["semantic_map"] = torch.empty(R, Cn, dtype=_F32, device=dev)
-    if Kn > 0:
-        out["instance_map"] = torch.empty(R, Kn, dtype=_F32, device=dev)
-    B = _box_table_size(raw, sample_box, box_sem, box_inst)
-    if sample_box is not None and box_sem is not None and Cn > 0:
-        out["fixed_semantic_map"] = torch.empty(R, Cn, dtype=_F32, device=dev)
-    if sample_box is not None and box_inst is not None and Kn > 0:
-        out["fixed_instance_map"] = torch.empty(R, Kn, dtype=_F32, device=dev)
-    co = _capi.PnrCompositeOut(**{k: _capi.ptr(out[k]) if k in out else None
-                                  for k, _ in _capi.PnrCompositeOut._fields_})
-    sb = sample_box.to(_I32).contiguous() if sample_box is not None else None
-    bs = box_sem.to(_I32).contiguous() if box_sem is not None else None
-    bi = box_inst.to(_I32).contiguous() if box_inst is not None else None
+    rays = _rays(rays_d)
+    sb, bs, bi, B = primitive_tables(raw, sample_box, box_sem, box_inst)
+    out = empty_composite_maps(R, N, Cn, Kn, sb is not None and bs is not None, sb is not None and bi is not None,
+                               raw.device)
     _capi.check(_capi.lib().pnr_composite(
         _capi.ptr(raw), _capi.ptr(z_vals), _capi.ptr(rays), R, N, Cn, Kn, int(bool(white_bkgd)),
         int(sem_activation == "softmax"), int(bool(mask_outside)), _capi.ptr(sb), _capi.ptr(bs), _capi.ptr(bi),
-        B, C.byref(co), _capi.stream_ptr()), "pnr_composite")
+        B, C.byref(_capi.ptr_struct(_capi.PnrCompositeOut, out)), _capi.stream_ptr()), "pnr_composite")
     return out
 
 
@@ -238,10 +254,8 @@ def raw2outputs_backward(raw, z_vals, rays_d, grads: Dict[str, torch.Tensor], wh
         raise ValueError(f"raw2outputs_backward: raw has {raw.shape[-1]} channels, expected {4 + Cn + Kn}")
     if "disp_map" in grads:
         raise ValueError("raw2outputs_backward: disp_map is not differentiated")
-    rays = torch.cat([torch.zeros_like(rays_d), rays_d], -1) if rays_d.shape[-1] == 3 else rays_d
-    rays = _f(rays, "rays")
-    shapes = {"rgb_map": (R, 3), "depth_map": (R,), "acc_map": (R,), "weights": (R, N), "semantic_map": (R, Cn),
-              "instance_map": (R, Kn), "fixed_semantic_map": (R, Cn), "fixed_instance_map": (R, Kn)}
+    rays = _rays(rays_d)
+    shapes = _map_shapes(R, N, Cn, Kn)
     held = {}
     for k, g in grads.items():
         if k not in shapes:
@@ -252,32 +266,26 @@ def raw2outputs_backward(raw, z_vals, rays_d, grads: Dict[str, torch.Tensor], wh
         if tuple(g.shape) != shapes[k]:
             raise ValueError(f"raw2outputs_backward: grad of {k} has shape {tuple(g.shape)}, expected {shapes[k]}")
         held[k] = g
-    cg = _capi.PnrCompositeGrads(**{k: _capi.ptr(held[k]) if k in held else None
-                                    for k, _ in _capi.PnrCompositeGrads._fields_})
-    B = _box_table_size(raw, sample_box, box_sem, box_inst)
-    sb = sample_box.to(_I32).contiguous() if sample_box is not None else None
-    bs = box_sem.to(_I32).contiguous() if box_sem is not None else None
-    bi = box_inst.to(_I32).contiguous() if box_inst is not None else None
+    sb, bs, bi, B = primitive_tables(raw, sample_box, box_sem, box_inst)
     d_raw = torch.empty_like(raw)
     _capi.check(_capi.lib().pnr_composite_backward(
         _capi.ptr(raw), _capi.ptr(z_vals), _capi.ptr(rays), R, N, Cn, Kn, int(bool(white_bkgd)),
         int(sem_activation == "softmax"), int(bool(mask_outside)), _capi.ptr(sb), _capi.ptr(bs), _capi.ptr(bi),
-        B, C.byref(cg), _capi.ptr(d_raw), _capi.stream_ptr()), "pnr_composite_backward")
+        B, C.byref(_capi.ptr_struct(_capi.PnrCompositeGrads, held)), _capi.ptr(d_raw), _capi.stream_ptr()),
+        "pnr_composite_backward")
     return d_raw
 
 
 class _Raw2OutputsFn(torch.autograd.Function):
     """`raw2outputs` as an autograd node: losses written in torch on the composited maps back-propagate to `raw`
-    through `pnr_composite_backward`.  The maps are returned in a fixed key order."""
-    KEYS = ("rgb_map", "depth_map", "acc_map", "weights", "semantic_map", "instance_map",
-            "fixed_semantic_map", "fixed_instance_map")
+    through `pnr_composite_backward`.  The maps are returned in the order of `composite_map_keys`, disp_map last."""
 
     @staticmethod
     def forward(ctx, raw, z_vals, rays_d, kw):
         out = raw2outputs(raw.detach(), z_vals, rays_d, **kw)
         ctx.save_for_backward(raw.detach(), z_vals, rays_d)
         ctx.kw = kw
-        ctx.present = [k for k in _Raw2OutputsFn.KEYS if k in out]
+        ctx.present = [k for k in out if k != "disp_map"]
         ctx.mark_non_differentiable(out["disp_map"])
         return tuple(out[k] for k in ctx.present) + (out["disp_map"],)
 
@@ -298,16 +306,8 @@ def raw2outputs_autograd(raw, z_vals, rays_d, white_bkgd: bool = False, num_clas
               sem_activation=sem_activation, sample_box=sample_box, box_sem=box_sem, box_inst=box_inst,
               mask_outside=mask_outside)
     res = _Raw2OutputsFn.apply(raw, z_vals, rays_d, kw)
-    Cn, Kn = int(num_classes), int(num_instances)
-    present = ["rgb_map", "depth_map", "acc_map", "weights"]
-    if Cn > 0:
-        present.append("semantic_map")
-    if Kn > 0:
-        present.append("instance_map")
-    if sample_box is not None and box_sem is not None and Cn > 0:
-        present.append("fixed_semantic_map")
-    if sample_box is not None and box_inst is not None and Kn > 0:
-        present.append("fixed_instance_map")
+    fixed = [sample_box is not None and t is not None for t in (box_sem, box_inst)]
+    present = [k for k in composite_map_keys(int(num_classes), int(num_instances), *fixed) if k != "disp_map"]
     out = dict(zip(present, res[:-1]))
     out["disp_map"] = res[-1]
     return out
@@ -502,23 +502,9 @@ class Renderer:
         ctx = self.net.pack(dev)
         ctx_fine = self.net_fine.pack(dev) if self.net_fine is not self.net else None
         e = lambda *shape, dtype=_F32: torch.empty(*shape, dtype=dtype, device=dev)
-
-        def maps(n_samples):
-            m = {"rgb_map": e(R, 3), "depth_map": e(R), "acc_map": e(R), "disp_map": e(R), "weights": e(R, n_samples)}
-            if Cn > 0:
-                m["semantic_map"] = e(R, Cn)
-            if Kn > 0:
-                m["instance_map"] = e(R, Kn)
-            if has_boxes and batch.get("box_sem") is not None and Cn > 0:
-                m["fixed_semantic_map"] = e(R, Cn)
-            if has_boxes and batch.get("box_inst") is not None and Kn > 0:
-                m["fixed_instance_map"] = e(R, Kn)
-            return m
-
-        def cstruct(m):
-            return _capi.PnrCompositeOut(**{k: _capi.ptr(m[k]) if k in m else None
-                                            for k, _ in _capi.PnrCompositeOut._fields_})
-        final, coarse = maps(Nt), (maps(N) if Ni > 0 else {})
+        fixed = [has_boxes and batch.get(k) is not None for k in ("box_sem", "box_inst")]
+        final = empty_composite_maps(R, Nt, Cn, Kn, *fixed, dev)
+        coarse = empty_composite_maps(R, N, Cn, Kn, *fixed, dev) if Ni > 0 else {}
         keep = [rays, near, far]                      # tensors the call reads: alive until it is enqueued
         a = _capi.PnrRenderArgs()
         a.rays, a.R, a.near, a.far = _capi.ptr(rays), R, _capi.ptr(near), _capi.ptr(far)
@@ -526,14 +512,13 @@ class Renderer:
         out: Dict[str, torch.Tensor] = {}
         if has_boxes:
             bc, bh, br = _f(batch["box_center"], "box_center"), _f(batch["box_half"], "box_half"), _f(batch["box_rot"], "box_rot")
-            bs = batch["box_sem"].to(dev, _I32).contiguous() if batch.get("box_sem") is not None else None
-            bi = batch["box_inst"].to(dev, _I32).contiguous() if batch.get("box_inst") is not None else None
-            _box_table_size(rays, torch.empty(0, device=dev), bs, bi)
+            out.update(box_id=e(R, M, dtype=_I32), t_in=e(R, M), t_out=e(R, M), sample_box=e(R, Nt, dtype=_I32))
+            tables = [batch[k].to(dev) if batch.get(k) is not None else None for k in ("box_sem", "box_inst")]
+            _, bs, bi, _ = primitive_tables(rays, out["sample_box"], *tables)
             keep += [bc, bh, br, bs, bi]
             a.box_center, a.box_half, a.box_rot = _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br)
             a.box_sem, a.box_inst, a.B, a.M = _capi.ptr(bs), _capi.ptr(bi), bc.shape[0], M
             hit8 = e(R, dtype=torch.uint8)
-            out.update(box_id=e(R, M, dtype=_I32), t_in=e(R, M), t_out=e(R, M), sample_box=e(R, Nt, dtype=_I32))
             a.hit_mask, a.box_id, a.t_in, a.t_out = _capi.ptr(hit8), _capi.ptr(out["box_id"]), _capi.ptr(out["t_in"]), _capi.ptr(out["t_out"])
             a.sample_box = _capi.ptr(out["sample_box"])
         a.N, a.Ni = N, Ni
@@ -561,7 +546,7 @@ class Renderer:
         a.sem_softmax = int(str(getattr(cfg, "sem_activation", "none")) == "softmax")
         a.mask_outside = int(bool(getattr(cfg, "mask_outside", False)))
         a.bound_by_primitives = int(bool(getattr(cfg, "bound_by_primitives", False)))
-        a.out, a.out0 = cstruct(final), cstruct(coarse)
+        a.out, a.out0 = _capi.ptr_struct(_capi.PnrCompositeOut, final), _capi.ptr_struct(_capi.PnrCompositeOut, coarse)
         out["z_vals"] = e(R, Nt)
         a.z_vals = _capi.ptr(out["z_vals"])
         if Ni > 0:

@@ -315,6 +315,27 @@ def test_compositing_epilogue_needs_whole_groups():
     assert out["rgb_map"].shape == (10, 3) and torch.isfinite(out["rgb_map"]).all()
 
 
+def test_compositing_epilogue_refuses_bad_primitive_tables():
+    """forward_composite takes the primitive tables as raw2outputs does: id tables of different lengths (one B bounds
+    both in the kernel, so the shorter one would be read past its end) and tables on another device are refused before
+    any launch."""
+    cfg = PN.make_cfg("cfg1", num_classes=5, num_instances=6)
+    net = S.init_network_weights(PN.make_network(cfg), seed=2).to(DEV)
+    rays = S.make_rays(cfg, rows=1)[:10].to(DEV)
+    z = torch.sort(torch.rand(10, 32, device=DEV) * 20 + 1, -1).values
+    sb = torch.randint(-1, 10, (10, 32), dtype=torch.int32, device=DEV)
+    ids = torch.arange(10, dtype=torch.int32, device=DEV) % 5
+    ok = net.forward_composite(rays, z, sample_box=sb, box_sem=ids, box_inst=ids)     # packs the weights
+    assert "fixed_semantic_map" in ok and "fixed_instance_map" in ok
+    torch.cuda.synchronize()
+    _capi.lib().pnr_launch_count(1)
+    with pytest.raises(ValueError, match=r"got lengths \[3, 10\]"):
+        net.forward_composite(rays, z, sample_box=sb, box_sem=ids[:3], box_inst=ids)
+    with pytest.raises(_capi.PnrError, match="box_sem is on cpu, expected cuda:0"):
+        net.forward_composite(rays, z, sample_box=sb, box_sem=ids.cpu(), box_inst=ids)
+    assert _capi.lib().pnr_launch_count(0) == 0
+
+
 def test_cuda_graph_capture_and_replay():
     """The kernels take everything they need as launch parameters (the per-tile program travels as a __grid_constant__
     argument, nothing is uploaded at launch time), so a forward or a fused MLP + compositing call can be captured in a
