@@ -11,11 +11,12 @@
 //     mbarrier complete_tx;
 //   * the consumer warpgroup issues wgmma m64nNk16 (N <= 128 per half of a step), both operands in shared memory:
 //     A = an embedding or the previous layer's activations, B = the weight stage; fp32 accumulators in registers;
-//   * once a step's MMAs have retired, its accumulators pass through a 64 x 128 fp32 staging tile in shared memory
-//     (one 128-column window at a time) to the row epilogue: two threads per row (column shares) add the bias, apply
-//     the ReLU, split into hi/lo and store the next layer's A operand over the one the step has just consumed.  The
-//     sigma head (N=1) and rgb head (N=3) are CUDA-core dot products inside the epilogue; semantic / instance logits
-//     are written straight to `raw`.
+//   * once a step's MMAs have retired, its epilogue adds the bias, applies the ReLU, splits into hi/lo and stores the
+//     next layer's A operand over the one the step has just consumed.  A trunk step does this straight from the
+//     accumulator registers (epi_regs_act); every other step passes its accumulators through a 64 x 128 fp32 staging
+//     tile in shared memory (one 128-column window at a time) to a row epilogue with two threads per row (column
+//     shares).  The sigma head (N=1) and rgb head (N=3) are CUDA-core dot products inside the row epilogue; semantic /
+//     instance logits are written straight to `raw`.
 //
 // The per-tile program (mlp_program.h) is built on the host once per weight load.  This kernel runs its steps in
 // order, each one's epilogue after all of its MMAs, and takes from the program the stage list (weight bytes, N,
@@ -471,6 +472,46 @@ __device__ __forceinline__ void mma_half_n(float (&d)[64], int n, const MlpProgr
 #undef PNR_MMA_N
 }
 
+// ------------------------------------------------------------------------------------------------
+// Trunk steps in registers.  A trunk step (ReLU hand-over without the sigma head, N = 256 as two N = 128 halves, output
+// to the activation columns; 7 of the 9 steps of an 8 x 256 network's tile) runs its epilogue straight from the
+// accumulator fragments: no staging tile, no barrier per 128-column window, no column shares.  The values and the
+// bytes stored are those of the staged epilogue (epi_group_act + epi_group_store): the same fp32 operations on the same
+// elements, the same range check.
+// ------------------------------------------------------------------------------------------------
+// Half HALF of a trunk step, held in `d` (its output always goes to the activation columns kColAHi / kColALo) ->
+// relu(acc + bias), split, stored.  Each thread holds rows r0 = 16w + t/4 and r0 + 8, columns 8j + 2(t%4) + {0, 1}:
+// one packed 32-bit word per row and part, and a quad of lanes covers one 16-byte core-matrix row (conflict-free: a
+// warp stores 8 consecutive 16-byte rows).  `bias` = the step's bias + 2(t%4), `op_t` = the operand region + this
+// thread's byte offset r0 * 16 + (t%4) * 4.
+template <int PASSES, int FMT, int HALF>
+__device__ __forceinline__ void epi_regs_act(const float (&d)[64], const float* bias, uint8_t* op_t, uint32_t& vmax) {
+  constexpr int kHi = ((kColAHi - kColOpBase) / 4 + 16 * HALF) * kOpKCoreBytes;
+  constexpr int kLo = ((kColALo - kColOpBase) / 4 + 16 * HALF) * kOpKCoreBytes;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float2 b = *reinterpret_cast<const float2*>(bias + 128 * HALF + 8 * j);
+    uint32_t h0, l0, h1, l1;
+    split_x2<FMT>(fmaxf(d[4 * j + 0] + b.x, 0.f), fmaxf(d[4 * j + 1] + b.y, 0.f), h0, l0);
+    split_x2<FMT>(fmaxf(d[4 * j + 2] + b.x, 0.f), fmaxf(d[4 * j + 3] + b.y, 0.f), h1, l1);
+#ifndef PNR_ABL_NOVMAX
+    vmax = __vimax3_u16x2(vmax, h0, h1);   // range check, as in epi_group_act
+#endif
+    *reinterpret_cast<uint32_t*>(op_t + kHi + j * kOpKCoreBytes) = h0;
+    *reinterpret_cast<uint32_t*>(op_t + kHi + j * kOpKCoreBytes + 8 * 16) = h1;
+    if (PASSES == 3) {
+      *reinterpret_cast<uint32_t*>(op_t + kLo + j * kOpKCoreBytes) = l0;
+      *reinterpret_cast<uint32_t*>(op_t + kLo + j * kOpKCoreBytes + 8 * 16) = l1;
+    }
+  }
+}
+
+// Can step `ed` run its epilogue in registers?  (Its halves are N = 128 whenever ed.n = 256 and ed.n0 = 128.)
+__device__ __forceinline__ bool trunk_in_regs(const EpiDesc& ed) {
+  return ed.kind == EPI_RELU_TO_A && !ed.sigma && ed.n == 256 && ed.n0 == 128 && ed.dst_col == kColAHi &&
+         ed.dst_lo_col == kColALo;
+}
+
 // Accumulator columns [c_base, c_base + n_h) of the step held in `d` (wgmma fragment: thread t of warp w holds rows
 // 16w + t/4 and 16w + t/4 + 8, columns 8j + 2(t%4) + {0, 1} in d[4j .. 4j+3]) -> the staging tile, for the columns
 // that fall into the window [w0, w0 + 128).
@@ -565,6 +606,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
     const int q = warp & 1, ch = warp >> 1;     // 32-row group (a "quarter" of the compositing code) ; column share
     const int row = q * 32 + lane;
     uint8_t* op = smem + kSmemOp;
+    uint8_t* op_t = op + (warp * 16 + (lane >> 2)) * 16 + (lane & 3) * 4;   // this thread's word of a trunk epilogue
     float* stg = reinterpret_cast<float*>(smem + kSmemStage);
     const uint32_t op_s = smem_u32(op), emb_s = smem_u32(smem + kSmemEmb), dir_s = smem_u32(smem + kSmemDir);
     RingPos rp{0u, -1};
@@ -591,6 +633,19 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
 #else
       constexpr bool kStreamOnly = false;
 #endif
+      // ablations (timing only, garbage outputs): no embeddings; no epilogue math or stores on the trunk steps (the
+      // staged path with its barriers, forward kernels).  (Skipping every epilogue is no ablation: with no accumulator
+      // ever read, ptxas serializes the wgmmas.)
+#ifdef PNR_ABL_NO_PROLOGUE
+      constexpr bool kAblNoPrologue = true;
+#else
+      constexpr bool kAblNoPrologue = false;
+#endif
+#ifdef PNR_ABL_NO_TRUNK_EPILOGUE
+      constexpr bool kAblNoTrunkEpi = true;
+#else
+      constexpr bool kAblNoTrunkEpi = false;
+#endif
       if (kStreamOnly || s_base >= s_end) {
         // no sample of this CTA in the tile: take the weight slots, compute nothing
 #pragma unroll 1
@@ -616,7 +671,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
         const int erow = threadIdx.x & (kRows - 1);
         const bool dir_thread = threadIdx.x >= kRows;
         const bool hashgrid = p.hash_table != nullptr;
-        if (!(BWD && dir_thread) || hashgrid) {
+        if (!kAblNoPrologue && (!(BWD && dir_thread) || hashgrid)) {
           int64_t se = s_base + erow;
           if (se >= p.S) se = p.S - 1;  // clamp: tail rows compute on a valid sample, results are discarded
           float x[3], d[3];
@@ -678,6 +733,16 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
           mma_half_n<PASSES, FMT>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
         si = end;
 
+        if (!BWD && !kAblNoTrunkEpi && trunk_in_regs(ed)) {   // ---- trunk epilogue in registers (see epi_regs_act)
+          named_bar_sync(1, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
+          const float* bias_t = consts + ed.bias_off + 2 * (lane & 3);
+          epi_regs_act<PASSES, FMT, 0>(acc0, bias_t, op_t, vmax);
+          epi_regs_act<PASSES, FMT, 1>(acc1, bias_t, op_t, vmax);
+          fence_proxy_async_smem();              // the next step's MMAs read what was just stored
+          named_bar_sync(1, kConsumerThreads);
+          continue;
+        }
+
         // ---- epilogue: accumulator columns [0, n0) are in acc0, [n0, n) in acc1
         const float* bias = consts + ed.bias_off;
         const float* aux = consts + ed.aux_off;
@@ -695,6 +760,11 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
           for (int c = ch * 32; c < (int)prog.ep[0].n; c += 2 * 32) prefetch_l2(g0 + c);
         }
         for (int w0 = 0; w0 < (int)ed.n; w0 += 128) {
+          if (kAblNoTrunkEpi && !BWD && trunk_in_regs(ed)) {
+            named_bar_sync(1, kConsumerThreads);
+            named_bar_sync(1, kConsumerThreads);
+            continue;
+          }
           stage_acc(acc0, 0, ed.n0, w0, stg, warp, lane);
           if (ed.n0 < ed.n) stage_acc(acc1, ed.n0, ed.n - ed.n0, w0, stg, warp, lane);
           named_bar_sync(1, kConsumerThreads);
