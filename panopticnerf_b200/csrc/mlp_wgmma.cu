@@ -37,16 +37,17 @@
 
 namespace pnr {
 
-// Write 8 consecutive K elements (one 16-byte core-matrix row) of this thread's row, split hi/lo.
+// Write 8 consecutive K elements (one 16-byte core-matrix row) of this thread's row, split hi/lo; returns the hi part.
 template <int PASSES, int FMT>
-__device__ __forceinline__ void store_core_row(uint8_t* hi_base, uint8_t* lo_base, int kcore, int row,
-                                               const float (&v)[8]) {
+__device__ __forceinline__ uint4 store_core_row(uint8_t* hi_base, uint8_t* lo_base, int kcore, int row,
+                                                const float (&v)[8]) {
   uint32_t h[4], l[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) split_x2<FMT>(v[2 * j], v[2 * j + 1], h[j], l[j]);
   const int off = (kcore * kRows + row) * 16;
   *reinterpret_cast<uint4*>(hi_base + off) = make_uint4(h[0], h[1], h[2], h[3]);
   if (PASSES == 3) *reinterpret_cast<uint4*>(lo_base + off) = make_uint4(l[0], l[1], l[2], l[3]);
+  return make_uint4(h[0], h[1], h[2], h[3]);
 }
 
 // gamma(p) = [p, sin(2^0 p), cos(2^0 p), ...] padded with zeros to KPAD, streamed out 8 at a time.
@@ -106,14 +107,9 @@ __device__ __forceinline__ void hash_rows(const MlpParams& p, const float (&v)[3
       for (int j = 0; j < 8; ++j)
         if (j / F == ll) acc[j] = f[j % F];
     }
-    uint32_t h[4], lo[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) split_x2<FMT>(acc[2 * j], acc[2 * j + 1], h[j], lo[j]);
-    const int off = (g * kRows + row) * 16;
-    *reinterpret_cast<uint4*>(hi_base + off) = make_uint4(h[0], h[1], h[2], h[3]);
-    if (PASSES == 3) *reinterpret_cast<uint4*>(lo_base + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    vmax = __vimax3_u16x2(vmax, h[0] & 0x7FFF7FFFu, h[1] & 0x7FFF7FFFu);
-    vmax = __vimax3_u16x2(vmax, h[2] & 0x7FFF7FFFu, h[3] & 0x7FFF7FFFu);
+    const uint4 h = store_core_row<PASSES, FMT>(hi_base, lo_base, g, row, acc);
+    vmax = __vimax3_u16x2(vmax, h.x & 0x7FFF7FFFu, h.y & 0x7FFF7FFFu);
+    vmax = __vimax3_u16x2(vmax, h.z & 0x7FFF7FFFu, h.w & 0x7FFF7FFFu);
   }
 }
 
@@ -132,6 +128,12 @@ __device__ __forceinline__ void hash_rows_f(const MlpParams& p, const float (&v)
 // Epilogue building blocks.  One thread owns one accumulator row; groups are 16 columns.
 // ------------------------------------------------------------------------------------------------
 
+// relu(acc + bias) of columns 4q .. 4q + 3 of a 16-column group, b = their bias
+__device__ __forceinline__ float4 relu_bias4(const uint32_t (&r)[16], int q, float4 b) {
+  return make_float4(fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f), fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f),
+                     fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f), fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f));
+}
+
 // activation -> next layer's A operand: v = act(acc + bias); [sigma += v . wsig]; split into hi / lo parts.
 // `vmax` collects the largest hi-part bit patterns seen (two 16-bit lanes; range check of the operand format).
 template <int PASSES, int FMT>
@@ -141,17 +143,13 @@ __device__ __forceinline__ void epi_group_act(const uint32_t (&r)[16], int g, co
   const float4* b4 = reinterpret_cast<const float4*>(bias + g * 16);
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    const float4 b = b4[q];
-    const float v0 = fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f);
-    const float v1 = fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f);
-    const float v2 = fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f);
-    const float v3 = fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f);
+    const float4 v = relu_bias4(r, q, b4[q]);
     if (ed.sigma) {
       const float4 w = reinterpret_cast<const float4*>(wsig + g * 16)[q];
-      sig += v0 * w.x + v1 * w.y + v2 * w.z + v3 * w.w;
+      sig += v.x * w.x + v.y * w.y + v.z * w.z + v.w * w.w;
     }
-    split_x2<FMT>(v0, v1, hi[2 * q], lo[2 * q]);
-    split_x2<FMT>(v2, v3, hi[2 * q + 1], lo[2 * q + 1]);
+    split_x2<FMT>(v.x, v.y, hi[2 * q], lo[2 * q]);
+    split_x2<FMT>(v.z, v.w, hi[2 * q + 1], lo[2 * q + 1]);
     // Range check on the packed hi parts (one 3-input 16x2 max per four values): v >= 0 after the ReLU, so the
     // 16-bit patterns order like the values, with +inf (what an overflowing conversion yields) and NaN on top.
     // (fmaxf turns a NaN accumulator into 0, but a NaN can only follow an overflow that was flagged where it
@@ -186,14 +184,11 @@ __device__ __forceinline__ void epi_group_rgb(const uint32_t (&r)[16], int g, co
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const float4 b = b4[q], a0 = w0[q], a1 = w1[q], a2 = w2[q];
-    const float v0 = fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f);
-    const float v1 = fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f);
-    const float v2 = fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f);
-    const float v3 = fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f);
-    c0 += v0 * a0.x; c1 += v0 * a1.x; c2 += v0 * a2.x;
-    c0 += v1 * a0.y; c1 += v1 * a1.y; c2 += v1 * a2.y;
-    c0 += v2 * a0.z; c1 += v2 * a1.z; c2 += v2 * a2.z;
-    c0 += v3 * a0.w; c1 += v3 * a1.w; c2 += v3 * a2.w;
+    const float4 v = relu_bias4(r, q, b);
+    c0 += v.x * a0.x; c1 += v.x * a1.x; c2 += v.x * a2.x;
+    c0 += v.y * a0.y; c1 += v.y * a1.y; c2 += v.y * a2.y;
+    c0 += v.z * a0.z; c1 += v.z * a1.z; c2 += v.z * a2.z;
+    c0 += v.w * a0.w; c1 += v.w * a1.w; c2 += v.w * a2.w;
   }
 }
 
@@ -230,11 +225,8 @@ __device__ __forceinline__ void epi_group_bwd(const uint32_t (&r)[16], int g, co
     uint32_t m = 0;
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const float4 b = b4[q];
-      v[4 * q + 0] = fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f);
-      v[4 * q + 1] = fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f);
-      v[4 * q + 2] = fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f);
-      v[4 * q + 3] = fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f);
+      const float4 x = relu_bias4(r, q, b4[q]);
+      v[4 * q + 0] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
     }
 #pragma unroll
     for (int j = 0; j < 16; ++j) m |= (v[j] > 0.f ? 1u : 0u) << j;
@@ -273,11 +265,7 @@ __device__ __forceinline__ void epi_group_actout(const uint32_t (&r)[16], int g,
   const float4* b4 = reinterpret_cast<const float4*>(bias + g * 16);
   float4* d4 = reinterpret_cast<float4*>(dst + g * 16);
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const float4 b = b4[q];
-    d4[q] = make_float4(fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f), fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f),
-                        fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f), fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f));
-  }
+  for (int q = 0; q < 4; ++q) d4[q] = relu_bias4(r, q, b4[q]);
 }
 
 // gradient w.r.t. the embedded input: accumulator columns [0, n_valid) of this group -> the sample's output row
@@ -357,6 +345,9 @@ __device__ __forceinline__ constexpr uint32_t inf_bits16() {
 constexpr int kSlots = 4;
 constexpr int kSlotBytes = kRing * kStageBytes / kSlots;
 static_assert(2 * kSlotBytes == kStageBytes, "a program stage is two ring slots");
+// ring slot and barrier phase of the gs-th slot taken (the weight stream and the consumers count alike)
+__device__ __forceinline__ uint32_t ring_slot(uint32_t gs) { return gs % kSlots; }
+__device__ __forceinline__ uint32_t ring_phase(uint32_t gs) { return (gs / kSlots) & 1; }
 
 __device__ __forceinline__ int stage_slots(const StageDesc& sd) { return sd.ksteps > 1 ? 2 : 1; }
 // the K16 steps [k0, k0 + kn) of slot j of the stage (the first K-half is the larger one)
@@ -421,7 +412,7 @@ __device__ __forceinline__ void mma_slot(float (&d)[64], const StageDesc& sd, in
   }
   int k0, kn;
   slot_ksteps(sd, j, k0, kn);
-  const uint32_t slot = rp.gs % kSlots, ph = (rp.gs / kSlots) & 1;
+  const uint32_t slot = ring_slot(rp.gs), ph = ring_phase(rp.gs);
   const uint32_t b = ring_s + slot * (uint32_t)kSlotBytes;
   const uint64_t ad_hi = make_smem_desc_noswz(a_hi, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
   const uint64_t ad_lo = make_smem_desc_noswz(a_lo, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
@@ -527,6 +518,144 @@ __device__ __forceinline__ void stage_acc(const float (&d)[64], int c_base, int 
   }
 }
 
+// Ablation builds (timing only, garbage outputs): the weight stream alone; no embeddings; no epilogue math or stores on
+// the trunk steps (the staged path with its barriers, forward kernels).  (Skipping every epilogue is no ablation: with
+// no accumulator ever read, ptxas serializes the wgmmas.)
+#ifdef PNR_ABL_STREAM_ONLY
+constexpr bool kStreamOnly = true;
+#else
+constexpr bool kStreamOnly = false;
+#endif
+#ifdef PNR_ABL_NO_PROLOGUE
+constexpr bool kAblNoPrologue = true;
+#else
+constexpr bool kAblNoPrologue = false;
+#endif
+#ifdef PNR_ABL_NO_TRUNK_EPILOGUE
+constexpr bool kAblNoTrunkEpi = true;
+#else
+constexpr bool kAblNoTrunkEpi = false;
+#endif
+
+// Embeddings of the tile from s_base: threads 0-63 gamma(x) of row t, threads 64-127 gamma(d) of row t - 64.  A
+// hash-grid trunk input (p.hash_table set) replaces gamma(x) by h(x): both threads of a row form its point, the xyz
+// thread gathers the first half of the feature core rows, the dir thread (after gamma(d), if any) the second half.
+template <int PASSES, int FMT, bool BWD>
+__device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgram& prog, uint8_t* smem, int64_t s_base,
+                                              uint32_t& vmax) {
+  named_bar_sync(1, kConsumerThreads);    // the previous tile's end-of-tile reads are done
+  const int erow = threadIdx.x & (kRows - 1);
+  const bool dir_thread = threadIdx.x >= kRows;
+  const bool hashgrid = p.hash_table != nullptr;
+  if (!kAblNoPrologue && (!(BWD && dir_thread) || hashgrid)) {
+    int64_t se = s_base + erow;
+    if (se >= p.S) se = p.S - 1;  // clamp: tail rows compute on a valid sample, results are discarded
+    float x[3], d[3];
+    if (p.pts != nullptr) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { x[c] = p.pts[se * 3 + c]; d[c] = BWD ? 0.f : p.viewdirs[se * 3 + c]; }
+    } else {
+      const int64_t ray = se / p.N;
+      const float zi = p.z[se];
+      const float* rr = p.rays + ray * 6;
+      float dn2 = 0.f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float dc = rr[3 + c];
+        x[c] = __fadd_rn(rr[c], __fmul_rn(dc, zi));  // pts = o + d*z, separately rounded like the oracle
+        dn2 = (c == 0) ? __fmul_rn(dc, dc) : __fadd_rn(dn2, __fmul_rn(dc, dc));
+        d[c] = dc;
+      }
+      const float nrm = sqrtf(dn2);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(d[c], nrm);
+    }
+    if (dir_thread) {
+      if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow);
+    } else if (!hashgrid) {
+      encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow);
+    }
+    if (hashgrid) {
+      float v[3];
+      hash_normalize(x, p.hash_aabb, v);
+      const int nc = ((p.hash_L * p.hash_F + 15) & ~15) / 8, half = (nc + 1) / 2;   // core rows the MMAs read
+      hash_rows_f<PASSES, FMT>(p, v, dir_thread ? half : 0, dir_thread ? nc : half, smem + kSmemEmb,
+                               smem + kSmemEmb + kEmbPartBytes, erow, vmax);
+    }
+  }
+  fence_proxy_async_smem();   // generic-proxy stores -> visible to the MMAs' async proxy
+  named_bar_sync(1, kConsumerThreads);
+}
+
+// The MMAs of step `ed` from stage si on: its stages up to the one that closes it, those of the first half (accumulator
+// column ed.acc_col) into acc0, the rest into acc1; a ring slot is released when the MMAs that read it have retired.
+// Returns the next step's first stage.
+template <int PASSES, int FMT>
+__device__ __forceinline__ int step_mmas(float (&acc0)[64], float (&acc1)[64], const MlpProgram& prog, const EpiDesc& ed,
+                                         int si, uint32_t ring_s, uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s,
+                                         uint32_t dir_s, uint32_t op_s, RingPos& rp, bool leader) {
+  int h1 = si, end = si;
+  for (;;) {
+    const uint32_t flags = prog.st[end].flags;
+    if (prog.st[end].acc_col == ed.acc_col) h1 = end + 1;
+    ++end;
+    if (flags & (F_COMMIT_ACC1 | F_COMMIT_VIEW)) break;
+  }
+  // each half's first stage (F_FIRST) overwrites its accumulator, so the old values are dead: clearing them (before
+  // any of the step's wgmmas) says so to the compiler, which can then use those registers between steps without moving
+  // live accumulators - a move in a divergent path would serialize every wgmma
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
+  mma_half_n<PASSES, FMT>(acc0, prog.st[si].n, prog, si, h1, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+  if (h1 < end)
+    mma_half_n<PASSES, FMT>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+  return end;
+}
+
+// A trunk step's epilogue in registers: both halves through epi_regs_act (bias_t, op_t as there) between two barriers.
+template <int PASSES, int FMT>
+__device__ __forceinline__ void trunk_epilogue(const float (&acc0)[64], const float (&acc1)[64], const float* bias_t,
+                                               uint8_t* op_t, uint32_t& vmax) {
+  named_bar_sync(1, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
+  epi_regs_act<PASSES, FMT, 0>(acc0, bias_t, op_t, vmax);
+  epi_regs_act<PASSES, FMT, 1>(acc1, bias_t, op_t, vmax);
+  fence_proxy_async_smem();              // the next step's MMAs read what was just stored
+  named_bar_sync(1, kConsumerThreads);
+}
+
+// End of a COMP tile (one warp, lanes stride channels): fold its per-quarter sums (qsum half `par`) into the open ray's
+// running sums racc, in ray order; a ray is written out when the next one starts or the CTA's range ends.
+__device__ __forceinline__ void comp_flush_tile(const MlpParams& p, float* racc, const float* qsum, int nch, int par,
+                                                int64_t s_base, int64_t s_end, int64_t cta_first, int lane) {
+  auto flush = [&](int64_t r) {
+    const float depth = racc[3], acc = racc[4];
+    __syncwarp();
+    for (int c = lane; c < nch; c += 32) {
+      const float v = racc[c];
+      if (c < 3) { if (p.rgb_map) p.rgb_map[r * 3 + c] = v + (p.white_bkgd ? (1.0f - acc) : 0.f); }
+      else if (c == 3) {
+        if (p.depth_map) p.depth_map[r] = v;
+        if (p.disp_map) p.disp_map[r] = comp_disp(depth, acc);
+      }
+      else if (c == 4) { if (p.acc_map) p.acc_map[r] = v; }
+      else if (c < 5 + p.C) { if (p.sem_map) p.sem_map[r * p.C + (c - 5)] = v; }
+      else { if (p.inst_map) p.inst_map[r * p.K + (c - 5 - p.C)] = v; }
+      racc[c] = 0.f;
+    }
+    __syncwarp();
+  };
+#pragma unroll 1
+  for (int qq = 0; qq < kQuarters; ++qq) {
+    const int64_t sq = s_base + 32 * qq;
+    if (sq >= s_end) break;
+    if (sq > cta_first && sq % p.N == 0) flush(sq / p.N - 1);    // the previous ray ended right before sq
+    const float* src = qsum + (par * kQuarters + qq) * kCompChPad;
+    for (int c = lane; c < nch; c += 32) racc[c] += src[c];
+    __syncwarp();
+  }
+  if (s_base < s_end && s_base + kRows >= s_end) flush(s_end / p.N - 1);   // the CTA's last ray
+}
+
 // COMP = false: tiles are dealt round-robin to the CTAs and the network outputs go to `raw`.
 // COMP = true : every CTA owns a contiguous range of whole rays and walks it tile by tile; the epilogue composites
 // on chip - per-sample alpha / transmittance / weight right after the sigma-producing layer (warp scan over aligned
@@ -588,7 +717,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
           for (int j = 0; j < nslots; ++j, ++gs) {
             int k0, kn;
             slot_ksteps(sd, j, k0, kn);
-            const uint32_t slot = gs % kSlots, ph = (gs / kSlots) & 1;
+            const uint32_t slot = ring_slot(gs), ph = ring_phase(gs);
             const uint32_t part = (uint32_t)kn * step_bytes;   // bytes of one image in this slot
             const uint32_t dst = ring_s + slot * (uint32_t)kSlotBytes, bar = bar_full + 8 * slot;
             const uint8_t* hi = p.wpacked + sd.gofs + (uint32_t)k0 * step_bytes;
@@ -628,32 +757,14 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       const int64_t s = s_base + row;
       const int64_t s_end = cta_end();
       const bool valid = s < s_end;
-#ifdef PNR_ABL_STREAM_ONLY
-      constexpr bool kStreamOnly = true;    // ablation (timing only, garbage outputs): the weight stream alone
-#else
-      constexpr bool kStreamOnly = false;
-#endif
-      // ablations (timing only, garbage outputs): no embeddings; no epilogue math or stores on the trunk steps (the
-      // staged path with its barriers, forward kernels).  (Skipping every epilogue is no ablation: with no accumulator
-      // ever read, ptxas serializes the wgmmas.)
-#ifdef PNR_ABL_NO_PROLOGUE
-      constexpr bool kAblNoPrologue = true;
-#else
-      constexpr bool kAblNoPrologue = false;
-#endif
-#ifdef PNR_ABL_NO_TRUNK_EPILOGUE
-      constexpr bool kAblNoTrunkEpi = true;
-#else
-      constexpr bool kAblNoTrunkEpi = false;
-#endif
       if (kStreamOnly || s_base >= s_end) {
         // no sample of this CTA in the tile: take the weight slots, compute nothing
 #pragma unroll 1
         for (int si = 0; si < n_stages; ++si) {
 #pragma unroll 1
           for (int j = 0; j < stage_slots(prog.st[si]); ++j, ++rp.gs) {
-            mbar_wait(bar_full + 8 * (rp.gs % kSlots), (rp.gs / kSlots) & 1);
-            release_slot(bar_empty, (int)(rp.gs % kSlots), lane == 0);
+            mbar_wait(bar_full + 8 * ring_slot(rp.gs), ring_phase(rp.gs));
+            release_slot(bar_empty, (int)ring_slot(rp.gs), lane == 0);
           }
         }
         continue;
@@ -663,83 +774,13 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       float w_mine = 0.f;                                            // this row's compositing weight (COMP)
       float sig = 0.f;
 
-      // ---- embeddings of this tile: threads 0-63 gamma(x) of row t, threads 64-127 gamma(d) of row t - 64.  A hash-grid
-      // trunk input (p.hash_table set) replaces gamma(x) by h(x): both threads of a row form its point, the xyz thread
-      // gathers the first half of the feature core rows, the dir thread (after gamma(d), if any) the second half.
-      named_bar_sync(1, kConsumerThreads);    // the previous tile's end-of-tile reads are done
-      {
-        const int erow = threadIdx.x & (kRows - 1);
-        const bool dir_thread = threadIdx.x >= kRows;
-        const bool hashgrid = p.hash_table != nullptr;
-        if (!kAblNoPrologue && (!(BWD && dir_thread) || hashgrid)) {
-          int64_t se = s_base + erow;
-          if (se >= p.S) se = p.S - 1;  // clamp: tail rows compute on a valid sample, results are discarded
-          float x[3], d[3];
-          if (p.pts != nullptr) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) { x[c] = p.pts[se * 3 + c]; d[c] = BWD ? 0.f : p.viewdirs[se * 3 + c]; }
-          } else {
-            const int64_t ray = se / p.N;
-            const float zi = p.z[se];
-            const float* rr = p.rays + ray * 6;
-            float dn2 = 0.f;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              const float dc = rr[3 + c];
-              x[c] = __fadd_rn(rr[c], __fmul_rn(dc, zi));  // pts = o + d*z, separately rounded like the oracle
-              dn2 = (c == 0) ? __fmul_rn(dc, dc) : __fadd_rn(dn2, __fmul_rn(dc, dc));
-              d[c] = dc;
-            }
-            const float nrm = sqrtf(dn2);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(d[c], nrm);
-          }
-          if (dir_thread) {
-            if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow);
-          } else if (!hashgrid) {
-            encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow);
-          }
-          if (hashgrid) {
-            float v[3];
-            hash_normalize(x, p.hash_aabb, v);
-            const int nc = ((p.hash_L * p.hash_F + 15) & ~15) / 8, half = (nc + 1) / 2;   // core rows the MMAs read
-            hash_rows_f<PASSES, FMT>(p, v, dir_thread ? half : 0, dir_thread ? nc : half, smem + kSmemEmb,
-                                     smem + kSmemEmb + kEmbPartBytes, erow, vmax);
-          }
-        }
-        fence_proxy_async_smem();   // generic-proxy stores -> visible to the MMAs' async proxy
-        named_bar_sync(1, kConsumerThreads);
-      }
-
+      tile_prologue<PASSES, FMT, BWD>(p, prog, smem, s_base, vmax);
       int si = 0;
       for (int st = 0; st < n_steps; ++st) {
         const EpiDesc ed = prog.ep[st];
-        // ---- the step's MMAs: its stages up to the one that closes it, those of the first half (accumulator column
-        // ed.acc_col) into acc0, the rest into acc1; a ring slot is released when the MMAs that read it have retired
-        int h1 = si, end = si;
-        for (;;) {
-          const uint32_t flags = prog.st[end].flags;
-          if (prog.st[end].acc_col == ed.acc_col) h1 = end + 1;
-          ++end;
-          if (flags & (F_COMMIT_ACC1 | F_COMMIT_VIEW)) break;
-        }
-        // each half's first stage (F_FIRST) overwrites its accumulator, so the old values are dead: clearing them
-        // (before any of the step's wgmmas) says so to the compiler, which can then use those registers between
-        // steps without moving live accumulators - a move in a divergent path would serialize every wgmma
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
-        mma_half_n<PASSES, FMT>(acc0, prog.st[si].n, prog, si, h1, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
-        if (h1 < end)
-          mma_half_n<PASSES, FMT>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
-        si = end;
-
-        if (!BWD && !kAblNoTrunkEpi && trunk_in_regs(ed)) {   // ---- trunk epilogue in registers (see epi_regs_act)
-          named_bar_sync(1, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
-          const float* bias_t = consts + ed.bias_off + 2 * (lane & 3);
-          epi_regs_act<PASSES, FMT, 0>(acc0, bias_t, op_t, vmax);
-          epi_regs_act<PASSES, FMT, 1>(acc1, bias_t, op_t, vmax);
-          fence_proxy_async_smem();              // the next step's MMAs read what was just stored
-          named_bar_sync(1, kConsumerThreads);
+        si = step_mmas<PASSES, FMT>(acc0, acc1, prog, ed, si, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
+        if (!BWD && !kAblNoTrunkEpi && trunk_in_regs(ed)) {
+          trunk_epilogue<PASSES, FMT>(acc0, acc1, consts + ed.bias_off + 2 * (lane & 3), op_t, vmax);
           continue;
         }
 
@@ -901,38 +942,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
         }
       }
       if (COMP) {
-        // ---- end of tile: fold this tile's per-quarter sums into the running sums of the open ray, in ray order;
-        // a ray is written out when the next one starts (or the CTA's range ends).  One warp, lanes stride channels.
         named_bar_sync(1, kConsumerThreads);            // every quarter's partial sums are in shared memory
-        if (warp == 0) {
-          auto flush = [&](int64_t r) {
-            const float depth = racc[3], acc = racc[4];
-            __syncwarp();
-            for (int c = lane; c < nch; c += 32) {
-              const float v = racc[c];
-              if (c < 3) { if (p.rgb_map) p.rgb_map[r * 3 + c] = v + (p.white_bkgd ? (1.0f - acc) : 0.f); }
-              else if (c == 3) {
-                if (p.depth_map) p.depth_map[r] = v;
-                if (p.disp_map) p.disp_map[r] = comp_disp(depth, acc);
-              }
-              else if (c == 4) { if (p.acc_map) p.acc_map[r] = v; }
-              else if (c < 5 + p.C) { if (p.sem_map) p.sem_map[r * p.C + (c - 5)] = v; }
-              else { if (p.inst_map) p.inst_map[r * p.K + (c - 5 - p.C)] = v; }
-              racc[c] = 0.f;
-            }
-            __syncwarp();
-          };
-#pragma unroll 1
-          for (int qq = 0; qq < kQuarters; ++qq) {
-            const int64_t sq = s_base + 32 * qq;
-            if (sq >= s_end) break;
-            if (sq > cta_first() && sq % p.N == 0) flush(sq / p.N - 1);    // the previous ray ended right before sq
-            const float* src = qsum + (par * kQuarters + qq) * kCompChPad;
-            for (int c = lane; c < nch; c += 32) racc[c] += src[c];
-            __syncwarp();
-          }
-          if (s_base < s_end && s_base + kRows >= s_end) flush(s_end / p.N - 1);   // the CTA's last ray
-        }
+        if (warp == 0) comp_flush_tile(p, racc, qsum, nch, par, s_base, s_end, cta_first(), lane);
       }
     }
     if (p.status != nullptr && ((vmax & 0xFFFFu) >= inf_bits16<FMT>() || (vmax >> 16) >= inf_bits16<FMT>()))
