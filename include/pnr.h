@@ -192,7 +192,15 @@ int pnr_label_tiles(const float* rgb_map, const float* depth_map, const float* s
  * per_ray [R,4] receives the four unweighted values; the caller sums them.  Every gradient is already multiplied by
  * the term's weight w_* and normaliser inv_n_* (1 / number of elements or valid rays, which the caller knows), i.e.
  * it is dL/dmap of L = w_rgb*mean_rgb + w_depth*mean_depth + w_sem*mean_sem + w_fix*mean_fix, ready for
- * pnr_composite_backward.  (Terms as in the paper; the reference's NetworkWrapper is not in the mount.) */
+ * pnr_composite_backward.  (Terms as in the paper; the reference's NetworkWrapper is not in the mount.)
+ *
+ * Instance term (on when instance_map != NULL; the fields after d_fixed_semantic_map, zero = off): the target of ray r
+ * is the lowest slot k whose fixed_instance_map[r,k] [R,K] equals the row maximum; the ray counts when that maximum is
+ * >= inst_min_weight (in (0,1]; a NaN maximum or a ray without primitives does not count).  inst_label [R] receives k
+ * or -1 and n_inst (one device int) the number of counted rays, both written by a label pass before the loss pass, so
+ * no host synchronisation is needed.  per_ray_inst [R] (nullable) = lse(instance_map[r]) - instance_map[r,k] (0 when
+ * not counted); d_instance_map [R,K] (nullable) = (softmax - onehot(k)) * w_inst / n_inst, i.e. the gradient of
+ * w_inst * (mean over counted rays).  No gradient flows into fixed_instance_map (the target is piecewise constant). */
 typedef struct pnr_loss_args {
   int64_t R; int32_t C; int32_t sem_is_prob;
   const float* rgb_map; const float* rgb_map0; const float* rgb_gt;
@@ -203,6 +211,14 @@ typedef struct pnr_loss_args {
   float eps;
   float* per_ray;
   float* d_rgb_map; float* d_rgb_map0; float* d_depth_map; float* d_semantic_map; float* d_fixed_semantic_map;
+  int32_t K;
+  const float* instance_map; const float* fixed_instance_map;
+  float w_inst;
+  float inst_min_weight;
+  float* per_ray_inst;
+  int32_t* inst_label;
+  int32_t* n_inst;
+  float* d_instance_map;
 } pnr_loss_args;
 int pnr_losses(const pnr_loss_args* args, void* stream);
 

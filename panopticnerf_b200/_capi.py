@@ -47,7 +47,10 @@ class PnrLossArgs(C.Structure):
                                           "fixed_semantic_map", "label", "label_weight")] + \
                [(k, C.c_float) for k in ("w_rgb", "w_depth", "w_sem", "w_fix", "inv_n_rgb", "inv_n_depth", "inv_n_sem", "eps")] + \
                [(k, C.c_void_p) for k in ("per_ray", "d_rgb_map", "d_rgb_map0", "d_depth_map", "d_semantic_map",
-                                          "d_fixed_semantic_map")]
+                                          "d_fixed_semantic_map")] + \
+               [("K", C.c_int32), ("instance_map", C.c_void_p), ("fixed_instance_map", C.c_void_p),
+                ("w_inst", C.c_float), ("inst_min_weight", C.c_float)] + \
+               [(k, C.c_void_p) for k in ("per_ray_inst", "inst_label", "n_inst", "d_instance_map")]
 
 
 class PnrCompositeGrads(C.Structure):

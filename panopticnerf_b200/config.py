@@ -40,6 +40,11 @@ _DEFAULTS = dict(
     render_path="fused", workspace_mb=0,
     # raise if the fp16 operands overflowed in this render (costs one 4-byte D2H read per render)
     check_range=True,
+    # training (lib/train/network_wrapper.py): loss weights of the photometric (fine + coarse), depth, pseudo-label
+    # semantic, fixed-semantic and instance terms; a ray supervises the instance head when its dominant primitive
+    # holds at least inst_min_weight of its rendering weight
+    trainer_module="panopticnerf_b200.lib.train.network_wrapper",
+    w_rgb=1.0, w_depth=0.1, w_sem=1.0, w_fix=1.0, w_inst=1.0, inst_min_weight=0.5,
 )
 
 # BASELINE.json "configs", in order.

@@ -239,7 +239,9 @@ extern "C" int pnr_hashgrid_backward(const float* x, int64_t n, const float* aab
 // ------------------------------------------------------------------------------------------------ losses
 // SURVEY 8(f) rank 2, the loss side (the reference's NetworkWrapper computes these with torch ops on the rendered
 // maps; its exact terms are not in the mount - the four below are the paper's: photometric, depth, 2D pseudo-label
-// cross-entropy on the rendered semantics, and the cross-entropy of the fixed (bounding-primitive) semantics).
+// cross-entropy on the rendered semantics, and the cross-entropy of the fixed (bounding-primitive) semantics), plus the
+// instance term (softmax cross-entropy of the rendered instance logits against the dominant primitive's slot; rule
+// chosen here, DESIGN 3.4).
 // One pass per ray: the per-ray value of every term and the gradient w.r.t. every map it reads, already scaled by
 // the term's weight and normaliser, so that `pnr_composite_backward` can consume them directly.
 namespace pnr {
@@ -258,6 +260,57 @@ __device__ __forceinline__ float warp_add(float v) {
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
   return v;
+}
+
+// Softmax cross-entropy of the logits s[0, n) against `label` (0 <= label < n), one warp, lanes stride the logits.
+// Returns lse(s) - s[label] on every lane; when d != null writes d[c] = scale(softmax(s)[c] - [c == label]).
+template <class Scale>
+__device__ __forceinline__ float softmax_xent(const float* __restrict__ s, int n, int label, int lane,
+                                              float* __restrict__ d, Scale scale) {
+  float m = -INFINITY;
+  for (int c = lane; c < n; c += 32) m = fmaxf(m, s[c]);
+  m = warp_max(m);
+  float z = 0.f;
+  for (int c = lane; c < n; c += 32) z += expf(s[c] - m);
+  z = warp_add(z);
+  // lse - s[label] and softmax = exp(s - lse) are not formed through lse = m + log(z): with logits of ~1e4, lse
+  // rounds at ~1e-3 and that error would go straight into the loss and every probability.  m - s[c] is exact
+  // or rounded relative to itself, so both stay within a few ulps of their own value.
+  if (d != nullptr)
+    for (int c = lane; c < n; c += 32) d[c] = scale(expf(s[c] - m) / z - (c == label ? 1.f : 0.f));
+  return (m - s[label]) + logf(z);
+}
+
+// Instance targets, before the loss pass: inst_label[r] = the lowest slot holding the maximum of fixed_instance_map[r]
+// when that maximum is >= inst_min_weight, else -1 (a NaN anywhere in the row makes the maximum NaN: not counted).
+// *n_inst (zeroed before the launch) += the block's count: one integer atomic per block, so the count is exact.
+__global__ void __launch_bounds__(256) instance_labels_kernel(LossArgs L) {
+  const pnr_loss_args& a = L.a;
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  bool counted = false;
+  if (r < a.R) {
+    const float* v = a.fixed_instance_map + r * a.K;
+    float best = -INFINITY;
+    int arg = 0x7fffffff;
+    bool nan = false;
+    for (int c = lane; c < a.K; c += 32) {
+      const float x = v[c];
+      if (x != x) nan = true;
+      else if (x > best || arg == 0x7fffffff) { best = x; arg = c; }
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+      const float ob = __shfl_xor_sync(0xffffffffu, best, d);
+      const int oa = __shfl_xor_sync(0xffffffffu, arg, d);
+      if (ob > best || (ob == best && oa < arg)) { best = ob; arg = oa; }
+    }
+    nan = __any_sync(0xffffffffu, nan);
+    counted = !nan && best >= a.inst_min_weight;
+    if (lane == 0) a.inst_label[r] = counted ? arg : -1;
+  }
+  const int n = __syncthreads_count(lane == 0 && counted);
+  if (threadIdx.x == 0 && n > 0) atomicAdd(a.n_inst, n);
 }
 
 __global__ void __launch_bounds__(256) losses_kernel(LossArgs L) {
@@ -303,21 +356,25 @@ __global__ void __launch_bounds__(256) losses_kernel(LossArgs L) {
       if (a.d_semantic_map)
         for (int c = lane; c < a.C; c += 32)
           a.d_semantic_map[r * a.C + c] = (has && c == label && p >= a.eps) ? -conf * a.w_sem * a.inv_n_sem / pc : 0.f;
-    } else {                 // the map is rendered logits: softmax cross-entropy
-      float m = -INFINITY;
-      for (int c = lane; c < a.C; c += 32) m = fmaxf(m, s[c]);
-      m = warp_max(m);
-      float z = 0.f;
-      for (int c = lane; c < a.C; c += 32) z += expf(s[c] - m);
-      z = warp_add(z);
-      // lse - s[label] and softmax = exp(s - lse) are not formed through lse = m + log(z): with logits of ~1e4, lse
-      // rounds at ~1e-3 and that error would go straight into the loss and every probability.  m - s[c] is exact
-      // or rounded relative to itself, so both stay within a few ulps of their own value.
-      l_sem = has ? ((m - s[label]) + logf(z)) * conf : 0.f;
-      if (a.d_semantic_map)
-        for (int c = lane; c < a.C; c += 32)
-          a.d_semantic_map[r * a.C + c] = has ? (expf(s[c] - m) / z - (c == label ? 1.f : 0.f)) * conf * a.w_sem * a.inv_n_sem : 0.f;
+    } else if (has) {        // the map is rendered logits: softmax cross-entropy
+      l_sem = softmax_xent(s, a.C, label, lane, a.d_semantic_map ? a.d_semantic_map + r * a.C : nullptr,
+                           [&](float g) { return g * conf * a.w_sem * a.inv_n_sem; }) * conf;
+    } else if (a.d_semantic_map) {
+      for (int c = lane; c < a.C; c += 32) a.d_semantic_map[r * a.C + c] = 0.f;
     }
+  }
+  // instance: softmax cross-entropy of the rendered instance logits against the label pass's target
+  if (a.instance_map != nullptr) {
+    const int k = a.inst_label[r];
+    float* d = a.d_instance_map ? a.d_instance_map + r * a.K : nullptr;
+    float l_inst = 0.f;
+    if (k >= 0) {
+      const float n = (float)*a.n_inst;     // >= 1: this ray is counted
+      l_inst = softmax_xent(a.instance_map + r * a.K, a.K, k, lane, d, [&](float g) { return g * a.w_inst / n; });
+    } else if (d != nullptr) {
+      for (int c = lane; c < a.K; c += 32) d[c] = 0.f;
+    }
+    if (a.per_ray_inst != nullptr && lane == 0) a.per_ray_inst[r] = l_inst;
   }
   // fixed (bounding-primitive) semantics: a rendered probability by construction
   if (a.fixed_semantic_map != nullptr && a.C > 0) {
@@ -343,8 +400,23 @@ extern "C" int pnr_losses(const pnr_loss_args* args, void* stream) {
   PNR_CHECK_ARG(!(args->semantic_map || args->fixed_semantic_map) || (args->label && args->C > 0),
                 "pnr_losses: semantic maps need label [R] and C > 0");
   PNR_CHECK_ARG(args->eps > 0.f, "pnr_losses: eps must be > 0");
+  const bool inst = args->instance_map != nullptr;
+  if (inst) {
+    PNR_CHECK_ARG(args->K >= 1 && args->K <= 32767, "pnr_losses: K=%d outside [1,32767] with instance_map", args->K);
+    PNR_CHECK_ARG(args->fixed_instance_map, "pnr_losses: instance_map without fixed_instance_map");
+    PNR_CHECK_ARG(args->inst_label, "pnr_losses: instance_map needs inst_label [R]");
+    PNR_CHECK_ARG(args->n_inst, "pnr_losses: instance_map needs n_inst");
+    PNR_CHECK_ARG(args->inst_min_weight > 0.f && args->inst_min_weight <= 1.f,
+                  "pnr_losses: inst_min_weight=%g outside (0,1]", (double)args->inst_min_weight);
+  }
   LossArgs L{*args};
-  losses_kernel<<<(unsigned)((args->R + 7) / 8), 256, 0, (cudaStream_t)stream>>>(L);
+  const unsigned blocks = (unsigned)((args->R + 7) / 8);
+  if (inst) {
+    PNR_CUDA(cudaMemsetAsync(args->n_inst, 0, sizeof(int32_t), (cudaStream_t)stream));
+    instance_labels_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(L);
+    PNR_LAUNCH_CHECK("instance_labels_kernel");
+  }
+  losses_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(L);
   PNR_LAUNCH_CHECK("losses_kernel");
   return PNR_OK;
 }

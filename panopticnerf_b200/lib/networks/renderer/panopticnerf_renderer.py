@@ -384,7 +384,10 @@ class Renderer:
                                          batch, sl))
         return {k: torch.cat([o[k] for o in outs], 0) for k in outs[0]}
 
-    def render_rays(self, rays, near, far, batch, sl):
+    def render_rays(self, rays, near, far, batch, sl, grad: bool = False):
+        """Both passes for the rays `sl` of the batch.  grad=True: the maps carry gradients to the parameters of both
+        networks (network_forward_rays_autograd + raw2outputs_autograd); the sampler is not differentiated (the fine
+        pass reads the coarse weights detached), and cfg.raw_noise_std adds noise to sigma before compositing."""
         cfg = self.cfg
         N, Ni = int(cfg.N_samples), int(getattr(cfg, "N_importance", 0))
         Cn, Kn = int(getattr(cfg, "num_classes", 0)), int(getattr(cfg, "num_instances", 0))
@@ -411,17 +414,15 @@ class Renderer:
                   mask_outside=bool(getattr(cfg, "mask_outside", False)))
         if has_boxes:
             kw.update(box_sem=batch.get("box_sem"), box_inst=batch.get("box_inst"))
-        raw = self.net.forward_rays(rays, z)
-        res = raw2outputs(raw, z, rays, sample_box=sb, **kw)
+        raw, res = self._pass(self.net, rays, z, sb, kw, batch.get("noise"), sl, grad)
         if Ni > 0:
             for k, v in res.items():
                 out[k + "_0"] = v
             out["z_vals_0"] = z
             u_f = batch["u_fine"][sl] if "u_fine" in batch else None
-            _, z = sample_pdf(z, res["weights"], Ni, det=(perturb == 0.0), u=u_f)
+            _, z = sample_pdf(z, res["weights"].detach(), Ni, det=(perturb == 0.0), u=u_f)
             sb = tag_samples(z, box_id, t_in, t_out) if has_boxes else None
-            raw = self.net_fine.forward_rays(rays, z)
-            res = raw2outputs(raw, z, rays, sample_box=sb, **kw)
+            raw, res = self._pass(self.net_fine, rays, z, sb, kw, batch.get("noise_fine"), sl, grad)
         out.update(res)
         out["z_vals"] = z
         if sb is not None:
@@ -430,9 +431,20 @@ class Renderer:
             out["raw"] = raw
         return out
 
-    # -- a3
-    @torch.no_grad()
-    def render(self, batch: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    def _pass(self, net, rays, z, sb, kw, noise, sl, grad: bool):
+        """raw and the composited maps of one pass over the depths z."""
+        if not grad:
+            raw = net.forward_rays(rays, z)
+            return raw, raw2outputs(raw, z, rays, sample_box=sb, **kw)
+        from ...train.mlp_backward import network_forward_rays_autograd
+        raw = network_forward_rays_autograd(net, rays, z)
+        std = float(getattr(self.cfg, "raw_noise_std", 0.0))
+        if std > 0.0:
+            nz = noise[sl] if noise is not None else torch.randn(z.shape, device=z.device)
+            raw = torch.cat([raw[..., :3], raw[..., 3:4] + _f(nz, "noise")[..., None] * std, raw[..., 4:]], -1)
+        return raw, raw2outputs_autograd(raw, z, rays, sample_box=sb, **kw)
+
+    def _rays_near_far(self, batch):
         cfg = self.cfg
         if "rays" not in batch and "c2w" in batch:     # camera given instead of rays: generate them on the device
             dev = next(self.net.parameters()).device
@@ -448,6 +460,19 @@ class Renderer:
         else:
             near = torch.full((rays.shape[0],), float(cfg.near), dtype=_F32, device=rays.device)
             far = torch.full((rays.shape[0],), float(cfg.far), dtype=_F32, device=rays.device)
+        return rays, near, far
+
+    def _check_range(self):
+        if bool(getattr(self.cfg, "check_range", True)):
+            self.net.check_range()
+            if self.net_fine is not self.net:
+                self.net_fine.check_range()
+
+    # -- a3
+    @torch.no_grad()
+    def render(self, batch: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        cfg = self.cfg
+        rays, near, far = self._rays_near_far(batch)
         staged = str(getattr(cfg, "render_path", "fused")) == "staged" or bool(getattr(cfg, "return_raw", False))
         with torch.cuda.device(rays.device):
             if staged:     # stage by stage from Python (one libpnr call per stage and chunk; keeps `raw`)
@@ -456,10 +481,20 @@ class Renderer:
                 out["near"], out["far"] = near, far
             else:          # the whole frame in ONE libpnr call (pnr_render_fused), chunked inside by the workspace
                 out = self.render_fused(rays, near, far, batch)
-            if bool(getattr(cfg, "check_range", True)):
-                self.net.check_range()
-                if self.net_fine is not self.net:
-                    self.net_fine.check_range()
+            self._check_range()
+        return out
+
+    def render_train(self, batch: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """The staged render of a training batch (all its rays in one pass) whose maps carry gradients back to the
+        parameters of both networks: the same keys as `render` with render_path "staged" (coarse maps with the
+        suffix _0, z_vals, sample_box and the fixed maps when box_inst / box_sem are given).  Jitter from batch u /
+        u_fine when given; with cfg.raw_noise_std > 0, batch noise [R,N] / noise_fine [R,N+Ni] (else torch.randn)
+        times the std is added to sigma before compositing."""
+        rays, near, far = self._rays_near_far(batch)
+        with torch.cuda.device(rays.device):
+            out = self.render_rays(rays, near, far, batch, slice(0, rays.shape[0]), grad=True)
+            out["near"], out["far"] = near, far
+            self._check_range()
         return out
 
     # -- a3/a4 through the single C-ABI entry point
