@@ -103,6 +103,18 @@ int pnr_intersect(const float* rays, int64_t R, const float* box_center, const f
                   const float* box_rot, int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id,
                   float* t_in, float* t_out, void* stream);
 
+/* a5 with mesh primitives (DESIGN 3.2).  mesh_tri_start [B+1] i32, non-decreasing, [0] = 0, [B] = T; mesh_tris
+ * [T,3,3] world-space vertices; primitive b owns the triangles [start[b], start[b+1]).  A primitive with an empty
+ * range is a cuboid (the slab test of pnr_intersect).  One with triangles is a closed mesh whose box is a cull volume
+ * containing all its vertices: a ray that misses the box misses the mesh, and the box's own interval is never
+ * reported; the mesh's inside intervals (watertight crossings, paired along the line) enter the M-nearest list, so
+ * one primitive may take several slots.  Ranges are clamped into [0, T].  Both mesh pointers NULL with T = 0 is
+ * pnr_intersect; otherwise both are set and 1 <= T < 2^31 (PNR_ERR_ARG before any launch). */
+int pnr_intersect_meshes(const float* rays, int64_t R, const float* box_center, const float* box_half,
+                         const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T,
+                         int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
+                         void* stream);
+
 /* a5 (AABB special case): per-ray near = max(tmin, near_min), far = tmax, or
  * (near_min, far_default) when the scene box is missed.  aabb_host = {lo.xyz, hi.xyz}. */
 int pnr_scene_near_far(const float* rays, int64_t R, const float* aabb_host, float near_min,
@@ -414,6 +426,9 @@ typedef struct pnr_render_args {
   float* far_out;               /* [R]                                                                            */
   void* workspace;              /* device scratch, caller-owned                                                   */
   size_t workspace_bytes;
+  const int32_t* mesh_tri_start;  /* [B+1] mesh primitives (pnr_intersect_meshes), or NULL with T = 0: cuboids only */
+  const float* mesh_tris;       /* [T,3,3]                                                                        */
+  int64_t T;
 } pnr_render_args;
 /* ctx_fine: the network of the fine pass (NULL = ctx), with the same num_classes and num_instances as ctx
  * (PNR_ERR_ARG otherwise: the maps are [R,C] / [R,K] of ctx). */

@@ -72,7 +72,8 @@ class PnrRenderArgs(C.Structure):
                 ("out", PnrCompositeOut), ("out0", PnrCompositeOut), ("z_vals", C.c_void_p), ("z_vals0", C.c_void_p),
                 ("hit_mask", C.c_void_p), ("box_id", C.c_void_p), ("t_in", C.c_void_p), ("t_out", C.c_void_p),
                 ("sample_box", C.c_void_p), ("near_out", C.c_void_p), ("far_out", C.c_void_p),
-                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+                ("mesh_tri_start", C.c_void_p), ("mesh_tris", C.c_void_p), ("T", C.c_int64)]
 
 
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
@@ -89,6 +90,7 @@ SIGNATURES = {
     "pnr_bind_hashgrid_table": (C.c_int, [_vp, _vp]),
     "pnr_load_weights": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32]),
     "pnr_intersect": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "pnr_intersect_meshes": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "pnr_scene_near_far": (C.c_int, [_vp, _i64, C.POINTER(_f32), _f32, _f32, _vp, _vp, _vp]),
     "pnr_bound_by_primitives": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "pnr_sample_stratified": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _f32, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),

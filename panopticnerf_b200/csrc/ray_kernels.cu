@@ -9,8 +9,13 @@
 namespace pnr {
 
 // ------------------------------------------------------------------------------------ a5 intersect
-constexpr int kBoxChunk = 512;  // boxes staged per shared-memory fill (15 floats each = 30 KB)
+constexpr int kBoxChunk = 512;  // boxes staged per shared-memory fill (15 floats each = 30 KB; 17 with meshes)
 
+// kMeshes = false: the slab test of every box (pnr_intersect).  kMeshes = true: a box whose triangle range
+// [tri_start[b], tri_start[b+1]) is not empty is the cull volume of a closed mesh (ray_math.h: pnr_tri_cross,
+// PnrMeshCross); on a cull hit its triangles are read from global memory (the same rows for the whole warp, so
+// L1/L2-resident broadcasts).  Every range is clamped into [0, T], so a malformed start table cannot read outside tris.
+template <bool kMeshes>
 __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict__ rays, int64_t R,
                                                         const float* __restrict__ bc,
                                                         const float* __restrict__ bh,
@@ -18,8 +23,11 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
                                                         uint8_t* __restrict__ hit_mask,
                                                         int32_t* __restrict__ box_id,
                                                         float* __restrict__ t_in,
-                                                        float* __restrict__ t_out) {
-  __shared__ float sb[kBoxChunk * 15];
+                                                        float* __restrict__ t_out,
+                                                        const int32_t* __restrict__ tri_start,
+                                                        const float* __restrict__ tris, int64_t T) {
+  constexpr int kS = kMeshes ? 17 : 15;   // floats per staged box: center, half, rot (+ the triangle range)
+  __shared__ float sb[kBoxChunk * kS];
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   float ox = 0, oy = 0, oz = 0, dx = 0, dy = 0, dz = 1;
   if (r < R) {
@@ -32,17 +40,42 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
   for (int b0 = 0; b0 < B; b0 += kBoxChunk) {
     const int nb = min(kBoxChunk, B - b0);
     __syncthreads();
-    for (int i = threadIdx.x; i < nb * 15; i += blockDim.x) {
-      const int b = i / 15, e = i % 15;
-      sb[i] = e < 3 ? bc[(b0 + b) * 3 + e] : (e < 6 ? bh[(b0 + b) * 3 + e - 3] : br[(b0 + b) * 9 + e - 6]);
+    for (int i = threadIdx.x; i < nb * kS; i += blockDim.x) {
+      const int b = i / kS, e = i % kS;
+      if (kMeshes && e >= 15) {
+        const int64_t lo = min(max((int64_t)tri_start[b0 + b], (int64_t)0), T);
+        const int64_t hi = min(max((int64_t)tri_start[b0 + b + 1], lo), T);
+        sb[i] = __int_as_float((int)(e == 15 ? lo : hi));
+      } else {
+        sb[i] = e < 3 ? bc[(b0 + b) * 3 + e] : (e < 6 ? bh[(b0 + b) * 3 + e - 3] : br[(b0 + b) * 9 + e - 6]);
+      }
     }
     __syncthreads();
     if (r < R) {
       for (int b = 0; b < nb; ++b) {
-        const float* q = sb + b * 15;
+        const float* q = sb + b * kS;
         float tmin, tmax;
-        if (pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax))
+        const bool hit = pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax);
+        if (kMeshes) {
+          const int k0 = __float_as_int(q[15]), k1 = __float_as_int(q[16]);
+          if (k0 == k1) {
+            if (hit) pnr_hits_insert(&L, M, tmin, tmax, b0 + b);
+          } else if (hit) {
+            const PnrShear S = pnr_shear(dx, dy, dz);
+            PnrMeshCross X;
+            pnr_cross_init(&X);
+            for (int k = k0; k < k1; ++k) {
+              float v[9];
+#pragma unroll
+              for (int e = 0; e < 9; ++e) v[e] = __ldg(tris + (int64_t)k * 9 + e);
+              float t;
+              if (pnr_tri_cross(ox, oy, oz, S, v, &t)) pnr_cross_add(&X, M, t);
+            }
+            pnr_cross_emit(&X, &L, M, b0 + b);
+          }
+        } else if (hit) {
           pnr_hits_insert(&L, M, tmin, tmax, b0 + b);
+        }
       }
     }
   }
@@ -313,20 +346,43 @@ using namespace pnr;
 
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
+// fn: the entry point's name in the error messages
+static int intersect_rays(const char* fn, const float* rays, int64_t R, const float* box_center, const float* box_half,
+                     const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T, int32_t B,
+                     int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out, void* stream) {
+  if (R == 0) return PNR_OK;  // empty input: nothing to do (pointers of empty tensors may be null)
+  PNR_CHECK_ARG(R >= 0 && B >= 0, "%s: R=%lld or B=%d < 0", fn, (long long)R, B);
+  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "%s: M=%d outside [1,%d]", fn, M, PNR_MAX_HITS);
+  PNR_CHECK_ARG(rays && hit_mask && box_id && t_in && t_out, "%s: null pointer", fn);
+  PNR_CHECK_ARG(B == 0 || (box_center && box_half && box_rot), "%s: null box table", fn);
+  const bool meshes = mesh_tri_start || mesh_tris || T != 0;
+  PNR_CHECK_ARG(!meshes || (mesh_tri_start && mesh_tris && T >= 1 && T < (int64_t(1) << 31)),
+                "%s: mesh_tri_start (%s), mesh_tris (%s) and T=%lld: both pointers null with T == 0, or both set "
+                "with 1 <= T < 2^31", fn, mesh_tri_start ? "set" : "null", mesh_tris ? "set" : "null", (long long)T);
+  if (meshes && B > 0)
+    intersect_kernel<true><<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
+        rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id, t_in, t_out, mesh_tri_start, mesh_tris, T);
+  else
+    intersect_kernel<false><<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
+        rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id, t_in, t_out, nullptr, nullptr, 0);
+  PNR_LAUNCH_CHECK("intersect_kernel");
+  return PNR_OK;
+}
+
+extern "C" int pnr_intersect_meshes(const float* rays, int64_t R, const float* box_center, const float* box_half,
+                                    const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris,
+                                    int64_t T, int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in,
+                                    float* t_out, void* stream) {
+  return intersect_rays("pnr_intersect_meshes", rays, R, box_center, box_half, box_rot, mesh_tri_start, mesh_tris, T, B, M,
+                        hit_mask, box_id, t_in, t_out, stream);
+}
+
 extern "C" int pnr_intersect(const float* rays, int64_t R, const float* box_center,
                              const float* box_half, const float* box_rot, int32_t B, int32_t M,
                              uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
                              void* stream) {
-  if (R == 0) return PNR_OK;  // empty input: nothing to do (pointers of empty tensors may be null)
-  PNR_CHECK_ARG(R >= 0 && B >= 0, "pnr_intersect: R=%lld or B=%d < 0", (long long)R, B);
-  PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "pnr_intersect: M=%d outside [1,%d]", M, PNR_MAX_HITS);
-  PNR_CHECK_ARG(rays && hit_mask && box_id && t_in && t_out, "pnr_intersect: null pointer");
-  PNR_CHECK_ARG(B == 0 || (box_center && box_half && box_rot), "pnr_intersect: null box table");
-  if (R == 0) return PNR_OK;
-  intersect_kernel<<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
-      rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id, t_in, t_out);
-  PNR_LAUNCH_CHECK("intersect_kernel");
-  return PNR_OK;
+  return intersect_rays("pnr_intersect", rays, R, box_center, box_half, box_rot, nullptr, nullptr, 0, B, M, hit_mask, box_id,
+                        t_in, t_out, stream);
 }
 
 extern "C" int pnr_scene_near_far(const float* rays, int64_t R, const float* aabb_host, float near_min,

@@ -21,6 +21,8 @@
 #define PNR_SUB(a, b) __fsub_rn((a), (b))
 #define PNR_DIV(a, b) __fdiv_rn((a), (b))
 #define PNR_DADD(a, b) __dadd_rn((a), (b))
+#define PNR_DSUB(a, b) __dsub_rn((a), (b))
+#define PNR_DMUL(a, b) __dmul_rn((a), (b))
 #define PNR_SQRT(a) __fsqrt_rn((a))
 #else
 #define PNR_MUL(a, b) ((a) * (b))
@@ -28,6 +30,8 @@
 #define PNR_SUB(a, b) ((a) - (b))
 #define PNR_DIV(a, b) ((a) / (b))
 #define PNR_DADD(a, b) ((a) + (b))
+#define PNR_DSUB(a, b) ((a) - (b))
+#define PNR_DMUL(a, b) ((a) * (b))
 #define PNR_SQRT(a) sqrtf((a))
 #endif
 
@@ -88,6 +92,161 @@ PNR_HD void pnr_hits_insert(PnrHitList* L, int M, float tmin, float tmax, int32_
   for (int m = 0; m < PNR_MAX_HITS; ++m)
     if (m == p) { L->key[m] = tmin; L->tout[m] = tmax; L->id[m] = b; }
   if (L->n < M) L->n += 1;
+}
+
+// a5, mesh primitives (DESIGN 3.2).  A primitive given as a closed triangle mesh: its box is only a cull volume, and
+// its hit intervals come from the crossings of the ray's line with the triangles.
+//
+// Crossing: the watertight ray/triangle test of Woop, Benthin and Wald (JCGT 2013).  The vertices are translated to
+// the ray origin, the axes permuted so that the largest |d| component is z (ties -> the lower axis), and sheared so
+// that the ray becomes the z axis.  The 2D edge functions U, V, W are individually rounded fp32; one that is exactly 0
+// is re-evaluated in double (the products of two floats are exact there, so its sign is exact).  One that is still 0
+// is resolved by a half-open tie rule that depends only on the edge's two sheared endpoints P -> Q: the sign the edge
+// function takes for the origin displaced to (eps, eps^2), i.e. sign(Py - Qy), else sign(Qx - Px).  The rule is
+// antisymmetric in P, Q, so across an edge or vertex that triangles of a closed mesh share, a ray crosses exactly one
+// of them, and a tangent touch counts an even number of times.  det = U + V + W == 0 (the ray in the triangle's
+// plane) is no crossing.  t = T / det in fp32, on the whole line (either sign); a NaN t is no crossing.
+struct PnrShear {
+  int kx, ky, kz;
+  float sx, sy, sz;
+};
+PNR_HD float pnr_pick3(float a, float b, float c, int k) { return k == 0 ? a : (k == 1 ? b : c); }
+PNR_HD PnrShear pnr_shear(float dx, float dy, float dz) {
+  const float ax = fabsf(dx), ay = fabsf(dy), az = fabsf(dz);
+  int kz = ay > ax ? 1 : 0;
+  if (az > (kz == 0 ? ax : ay)) kz = 2;
+  int kx = kz == 2 ? 0 : kz + 1;
+  int ky = kx == 2 ? 0 : kx + 1;
+  const float dk = pnr_pick3(dx, dy, dz, kz);
+  if (dk < 0.f) { const int s = kx; kx = ky; ky = s; }   // keeps the winding (the test is two-sided anyway)
+  PnrShear S;
+  S.kx = kx; S.ky = ky; S.kz = kz;
+  S.sx = PNR_DIV(pnr_pick3(dx, dy, dz, kx), dk);
+  S.sy = PNR_DIV(pnr_pick3(dx, dy, dz, ky), dk);
+  S.sz = PNR_DIV(1.0f, dk);
+  return S;
+}
+// sign of the edge function e = Px*Qy - Py*Qx of the sheared edge P -> Q, e its fp32 value and ed its double value
+// (used when e == 0); 0 only for a degenerate edge (P == Q)
+PNR_HD int pnr_edge_sign(float e, double ed, bool redo, float px, float py, float qx, float qy) {
+  if (redo) {
+    if (ed > 0.0) return 1;
+    if (ed < 0.0) return -1;
+  } else {
+    if (e > 0.f) return 1;
+    if (e < 0.f) return -1;
+  }
+  if (py != qy) return py > qy ? 1 : -1;
+  if (qx != px) return qx > px ? 1 : -1;
+  return 0;
+}
+// v = the triangle's 9 floats (v0, v1, v2).  Returns whether the line crosses it, and where (*t).
+PNR_HD bool pnr_tri_cross(float ox, float oy, float oz, const PnrShear& S, const float* v, float* t) {
+  float ax, ay, az, bx, by, bz, cx, cy, cz;
+  {
+    const float a0 = PNR_SUB(v[0], ox), a1 = PNR_SUB(v[1], oy), a2 = PNR_SUB(v[2], oz);
+    const float b0 = PNR_SUB(v[3], ox), b1 = PNR_SUB(v[4], oy), b2 = PNR_SUB(v[5], oz);
+    const float c0 = PNR_SUB(v[6], ox), c1 = PNR_SUB(v[7], oy), c2 = PNR_SUB(v[8], oz);
+    az = pnr_pick3(a0, a1, a2, S.kz); bz = pnr_pick3(b0, b1, b2, S.kz); cz = pnr_pick3(c0, c1, c2, S.kz);
+    ax = PNR_SUB(pnr_pick3(a0, a1, a2, S.kx), PNR_MUL(S.sx, az));
+    ay = PNR_SUB(pnr_pick3(a0, a1, a2, S.ky), PNR_MUL(S.sy, az));
+    bx = PNR_SUB(pnr_pick3(b0, b1, b2, S.kx), PNR_MUL(S.sx, bz));
+    by = PNR_SUB(pnr_pick3(b0, b1, b2, S.ky), PNR_MUL(S.sy, bz));
+    cx = PNR_SUB(pnr_pick3(c0, c1, c2, S.kx), PNR_MUL(S.sx, cz));
+    cy = PNR_SUB(pnr_pick3(c0, c1, c2, S.ky), PNR_MUL(S.sy, cz));
+  }
+  float U = PNR_SUB(PNR_MUL(cx, by), PNR_MUL(cy, bx));   // edge C -> B
+  float V = PNR_SUB(PNR_MUL(ax, cy), PNR_MUL(ay, cx));   // edge A -> C
+  float W = PNR_SUB(PNR_MUL(bx, ay), PNR_MUL(by, ax));   // edge B -> A
+  double Ud = 0.0, Vd = 0.0, Wd = 0.0;
+  const bool redo = U == 0.f || V == 0.f || W == 0.f;
+  if (redo) {
+    Ud = PNR_DSUB(PNR_DMUL((double)cx, (double)by), PNR_DMUL((double)cy, (double)bx));
+    Vd = PNR_DSUB(PNR_DMUL((double)ax, (double)cy), PNR_DMUL((double)ay, (double)cx));
+    Wd = PNR_DSUB(PNR_DMUL((double)bx, (double)ay), PNR_DMUL((double)by, (double)ax));
+    U = (float)Ud; V = (float)Vd; W = (float)Wd;
+  }
+  const int su = pnr_edge_sign(U, Ud, redo, cx, cy, bx, by);
+  const int sv = pnr_edge_sign(V, Vd, redo, ax, ay, cx, cy);
+  const int sw = pnr_edge_sign(W, Wd, redo, bx, by, ax, ay);
+  if (!((su > 0 && sv > 0 && sw > 0) || (su < 0 && sv < 0 && sw < 0))) return false;
+  const float det = PNR_ADD(PNR_ADD(U, V), W);
+  if (det == 0.f) return false;
+  const float T = PNR_ADD(PNR_ADD(PNR_MUL(U, PNR_MUL(S.sz, az)), PNR_MUL(V, PNR_MUL(S.sz, bz))),
+                          PNR_MUL(W, PNR_MUL(S.sz, cz)));
+  *t = PNR_DIV(T, det);
+  return *t == *t;
+}
+
+// Crossings of one mesh -> its hit intervals.  Sorted along the line, the crossings c0 <= c1 <= ... pair up as the
+// inside intervals (c0,c1), (c2,c3), ...; an odd count (an open mesh, a degenerate ray) gives the one hull interval
+// [first, last].  An interval (a, b) with b > 0 is a candidate; a mesh's first M candidates are kept, and of those the
+// ones with b > max(a, 0) are hits (zero-length ones are not), inserted in order with key a.  So only the parity and
+// the largest of the crossings at t <= 0, the 2M smallest at t > 0, the count and the extremes are needed: exact, in
+// registers.
+struct PnrMeshCross {
+  float pos[2 * PNR_MAX_HITS];   // the smallest crossings at t > 0, ascending
+  int npos;                      // entries of pos in use (<= 2M)
+  int n;                         // crossings in all
+  int nneg;                      // crossings at t <= 0
+  float neg_max;                 // the largest of them
+  float lo, hi;                  // the smallest and largest crossing
+};
+PNR_HD void pnr_cross_init(PnrMeshCross* S) {
+  S->npos = 0; S->n = 0; S->nneg = 0;
+  S->neg_max = 0.f; S->lo = 0.f; S->hi = 0.f;
+#pragma unroll
+  for (int m = 0; m < 2 * PNR_MAX_HITS; ++m) S->pos[m] = 0.f;
+}
+PNR_HD void pnr_cross_add(PnrMeshCross* S, int M, float t) {
+  S->lo = (S->n == 0 || t < S->lo) ? t : S->lo;
+  S->hi = (S->n == 0 || t > S->hi) ? t : S->hi;
+  S->n += 1;
+  if (t <= 0.f) {
+    S->neg_max = (S->nneg == 0 || t > S->neg_max) ? t : S->neg_max;
+    S->nneg += 1;
+    return;
+  }
+  const int cap = 2 * M;
+  int p = S->npos;   // first p with pos[p] > t
+#pragma unroll
+  for (int m = 2 * PNR_MAX_HITS - 1; m >= 0; --m)
+    if (m < S->npos && S->pos[m] > t) p = m;
+  if (p >= cap) return;
+#pragma unroll
+  for (int m = 2 * PNR_MAX_HITS - 1; m >= 1; --m)
+    if (m > p && m < cap) S->pos[m] = S->pos[m - 1];
+#pragma unroll
+  for (int m = 0; m < 2 * PNR_MAX_HITS; ++m)
+    if (m == p) S->pos[m] = t;
+  if (S->npos < cap) S->npos += 1;
+}
+PNR_HD void pnr_cross_emit(const PnrMeshCross* S, PnrHitList* L, int M, int32_t b) {
+  if (S->n == 0) return;
+  if (S->n & 1) {
+    if (S->hi > pnr_max_nan(S->lo, 0.f)) pnr_hits_insert(L, M, S->lo, S->hi, b);
+    return;
+  }
+  int j = 0, kept = 0;
+  if (S->nneg & 1) {   // the interval around the origin: its exit is the first crossing at t > 0
+    pnr_hits_insert(L, M, S->neg_max, S->pos[0], b);
+    j = 1;
+    kept = 1;
+  }
+#pragma unroll
+  for (int m = 0; m < PNR_MAX_HITS; ++m) {
+    const int i = j + 2 * m;
+    if (kept < M && i + 1 < S->npos) {
+      float a = 0.f, c = 0.f;
+#pragma unroll
+      for (int q = 0; q < 2 * PNR_MAX_HITS; ++q) {   // register-resident: no dynamic indexing
+        if (q == i) a = S->pos[q];
+        if (q == i + 1) c = S->pos[q];
+      }
+      if (c > a) pnr_hits_insert(L, M, a, c, b);
+      kept += 1;
+    }
+  }
 }
 
 // a6

@@ -164,6 +164,10 @@ extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_rende
   const bool boxes = a->B > 0;
   PNR_CHECK_ARG(!boxes || (a->box_center && a->box_half && a->box_rot && M >= 1 && M <= PNR_MAX_HITS),
                 "pnr_render_fused: bad primitive table (B=%d, M=%d)", a->B, M);
+  PNR_CHECK_ARG((!a->mesh_tri_start && !a->mesh_tris && a->T == 0) ||
+                    (a->mesh_tri_start && a->mesh_tris && a->T >= 1 && a->T < (int64_t(1) << 31)),
+                "pnr_render_fused: mesh_tri_start (%s), mesh_tris (%s) and T=%lld: both null with T == 0, or both set "
+                "with 1 <= T < 2^31", a->mesh_tri_start ? "set" : "null", a->mesh_tris ? "set" : "null", (long long)a->T);
   PNR_CHECK_ARG(a->sample_mode == PNR_SAMPLE_UNIFORM || (a->sample_mode == PNR_SAMPLE_INTERVALS && boxes),
                 "pnr_render_fused: sample_mode %d (interval sampling needs primitives)", a->sample_mode);
   PNR_CHECK_ARG(a->workspace && a->workspace_bytes > 0, "pnr_render_fused: no workspace (see pnr_workspace_bytes)");
@@ -219,7 +223,11 @@ extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_rende
       bid = L.have_hits ? a->box_id + r0 * M : bid_s;
       tin = L.have_hits ? a->t_in + r0 * M : tin_s;
       tout = L.have_hits ? a->t_out + r0 * M : tout_s;
-      PNR_TRY(pnr_intersect(rays, n, a->box_center, a->box_half, a->box_rot, a->B, M, hit, bid, tin, tout, stream));
+      if (a->T > 0)
+        PNR_TRY(pnr_intersect_meshes(rays, n, a->box_center, a->box_half, a->box_rot, a->mesh_tri_start, a->mesh_tris,
+                                     a->T, a->B, M, hit, bid, tin, tout, stream));
+      else
+        PNR_TRY(pnr_intersect(rays, n, a->box_center, a->box_half, a->box_rot, a->B, M, hit, bid, tin, tout, stream));
       if (a->bound_by_primitives) PNR_TRY(pnr_bound_by_primitives(hit, bid, tin, tout, n, M, near, far, stream));
     }
     // ---- a6: coarse depths + ids

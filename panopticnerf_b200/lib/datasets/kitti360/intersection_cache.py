@@ -18,6 +18,9 @@ def _key(prims: Dict[str, np.ndarray], c2w: np.ndarray, intrinsics, H: int, W: i
     for a in (prims["box_center"], prims["box_half"], prims["box_rot"], np.asarray(c2w, dtype=np.float32),
               np.asarray(intrinsics, dtype=np.float32), np.array([H, W, max_hits, _FORMAT], dtype=np.int64)):
         h.update(np.ascontiguousarray(a).tobytes())
+    if "mesh_tris" in prims:      # only then: a cache of cuboids keeps its key
+        for a in (np.asarray(prims["mesh_tri_start"], dtype=np.int32), np.asarray(prims["mesh_tris"], dtype=np.float32)):
+            h.update(np.ascontiguousarray(a).tobytes())
     return h.hexdigest()
 
 

@@ -97,8 +97,9 @@ def _rays(rays_d: torch.Tensor) -> torch.Tensor:
 # stage wrappers (one libpnr call each)
 # ------------------------------------------------------------------------------------------------
 @_on_tensor_device
-def intersect(rays, box_center, box_half, box_rot, max_hits: int):
-    """a5 -> hit_mask [R] bool, box_id [R,M] i32, t_in, t_out [R,M]."""
+def intersect(rays, box_center, box_half, box_rot, max_hits: int, mesh_tri_start=None, mesh_tris=None):
+    """a5 -> hit_mask [R] bool, box_id [R,M] i32, t_in, t_out [R,M].  With a mesh table (mesh_tri_start [B+1] int32,
+    mesh_tris [T,3,3]) the primitives that own triangles are closed meshes culled by their box (DESIGN 3.2)."""
     rays = _f(rays, "rays")
     R, B, M = rays.shape[0], box_center.shape[0], int(max_hits)
     dev = rays.device
@@ -107,10 +108,29 @@ def intersect(rays, box_center, box_half, box_rot, max_hits: int):
     t_in = torch.empty(R, M, dtype=_F32, device=dev)
     t_out = torch.empty(R, M, dtype=_F32, device=dev)
     bc, bh, br = _f(box_center, "box_center"), _f(box_half, "box_half"), _f(box_rot, "box_rot")
-    _capi.check(_capi.lib().pnr_intersect(_capi.ptr(rays), R, _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br), B, M,
-                                          _capi.ptr(hit), _capi.ptr(box_id), _capi.ptr(t_in), _capi.ptr(t_out),
-                                          _capi.stream_ptr()), "pnr_intersect")
+    if mesh_tri_start is None and mesh_tris is None:
+        _capi.check(_capi.lib().pnr_intersect(_capi.ptr(rays), R, _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br), B, M,
+                                              _capi.ptr(hit), _capi.ptr(box_id), _capi.ptr(t_in), _capi.ptr(t_out),
+                                              _capi.stream_ptr()), "pnr_intersect")
+        return hit.bool(), box_id, t_in, t_out
+    starts, tris = _mesh_table(mesh_tri_start, mesh_tris, B, dev)
+    _capi.check(_capi.lib().pnr_intersect_meshes(_capi.ptr(rays), R, _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br),
+                                                 _capi.ptr(starts), _capi.ptr(tris), tris.shape[0], B, M,
+                                                 _capi.ptr(hit), _capi.ptr(box_id), _capi.ptr(t_in), _capi.ptr(t_out),
+                                                 _capi.stream_ptr()), "pnr_intersect_meshes")
     return hit.bool(), box_id, t_in, t_out
+
+
+def _mesh_table(mesh_tri_start, mesh_tris, B: int, device):
+    """(mesh_tri_start int32 [B+1], mesh_tris fp32 [T,3,3]) on `device`, shapes checked."""
+    if mesh_tri_start is None or mesh_tris is None:
+        raise ValueError("mesh_tri_start and mesh_tris come together")
+    starts = mesh_tri_start.to(device=device, dtype=_I32).contiguous()
+    tris = _f(mesh_tris.to(device), "mesh_tris")
+    if tuple(starts.shape) != (B + 1,) or tris.dim() != 3 or tuple(tris.shape[1:]) != (3, 3):
+        raise ValueError(f"mesh table: mesh_tri_start {tuple(starts.shape)} (want ({B + 1},)), mesh_tris "
+                         f"{tuple(tris.shape)} (want (T, 3, 3))")
+    return starts, tris
 
 
 @_on_tensor_device
@@ -342,6 +362,7 @@ def sample_pdf(z, weights, N_importance: int, det: bool = True, u: Optional[torc
 class Renderer:
     """Renderer(cfg, net).render(batch) -> dict of per-ray maps (a3).  batch keys: rays [R,6] (o||d),
     optional near/far [R], scene_aabb [2,3], box_center/box_half [B,3], box_rot [B,3,3], box_sem/box_inst [B],
+    mesh_tri_start [B+1] int32 / mesh_tris [T,3,3] (mesh primitives: include/pnr.h pnr_intersect_meshes),
     u [R,N] / u_fine [R,Ni] (externally supplied jitter), perturb."""
 
     def __init__(self, cfg, net, net_fine=None):
@@ -398,7 +419,7 @@ class Renderer:
         box_id = t_in = t_out = None
         if has_boxes:
             hit, box_id, t_in, t_out = intersect(rays, batch["box_center"], batch["box_half"],
-                                                 batch["box_rot"], M)
+                                                 batch["box_rot"], M, batch.get("mesh_tri_start"), batch.get("mesh_tris"))
             out.update(hit_mask=hit, box_id=box_id, t_in=t_in, t_out=t_out)
             if bool(getattr(cfg, "bound_by_primitives", False)):
                 near, far = bound_by_primitives(hit, box_id, t_in, t_out, near, far)
@@ -556,6 +577,10 @@ class Renderer:
             hit8 = e(R, dtype=torch.uint8)
             a.hit_mask, a.box_id, a.t_in, a.t_out = _capi.ptr(hit8), _capi.ptr(out["box_id"]), _capi.ptr(out["t_in"]), _capi.ptr(out["t_out"])
             a.sample_box = _capi.ptr(out["sample_box"])
+            if batch.get("mesh_tri_start") is not None or batch.get("mesh_tris") is not None:
+                starts, tris = _mesh_table(batch.get("mesh_tri_start"), batch.get("mesh_tris"), bc.shape[0], dev)
+                keep += [starts, tris]
+                a.mesh_tri_start, a.mesh_tris, a.T = _capi.ptr(starts), _capi.ptr(tris), tris.shape[0]
         a.N, a.Ni = N, Ni
         tv = self._tv(N, dev)
         a.t_vals = _capi.ptr(tv)
