@@ -43,15 +43,17 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
     for (int i = threadIdx.x; i < nb * kS; i += blockDim.x) {
       const int b = i / kS, e = i % kS;
       if (kMeshes && e >= 15) {
-        const int64_t lo = min(max((int64_t)tri_start[b0 + b], (int64_t)0), T);
-        const int64_t hi = min(max((int64_t)tri_start[b0 + b + 1], lo), T);
-        sb[i] = __int_as_float((int)(e == 15 ? lo : hi));
+        int k0, k1;
+        pnr_tri_range(tri_start, b0 + b, T, &k0, &k1);
+        sb[i] = __int_as_float(e == 15 ? k0 : k1);
       } else {
         sb[i] = e < 3 ? bc[(b0 + b) * 3 + e] : (e < 6 ? bh[(b0 + b) * 3 + e - 3] : br[(b0 + b) * 9 + e - 6]);
       }
     }
     __syncthreads();
     if (r < R) {
+      // the per-primitive step; tests/host_emu.cpp writes it out again, because as a shared function it changes the
+      // mesh instantiation's SASS
       for (int b = 0; b < nb; ++b) {
         const float* q = sb + b * kS;
         float tmin, tmax;
@@ -79,17 +81,7 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
       }
     }
   }
-  if (r < R) {
-    hit_mask[r] = L.n > 0 ? 1 : 0;
-#pragma unroll
-    for (int m = 0; m < PNR_MAX_HITS; ++m)
-      if (m < M) {
-        const bool v = m < L.n;
-        box_id[r * M + m] = v ? L.id[m] : -1;
-        t_in[r * M + m] = v ? pnr_max_nan(L.key[m], 0.f) : 0.f;
-        t_out[r * M + m] = v ? L.tout[m] : 0.f;
-      }
-  }
+  if (r < R) pnr_hits_store(&L, M, r, hit_mask, box_id, t_in, t_out);
 }
 
 struct Aabb { float c[3], h[3]; };
@@ -146,12 +138,12 @@ __global__ void __launch_bounds__(256) stratified_kernel(
     const bool live = i < N;
     float zi = 0.f;
     if (live) {
-      const int64_t idx = r * N + i;
-      zi = (perturb > 0.f) ? pnr_strat_z_jitter(nr, fr, t_vals, i, N, u[idx]) : pnr_strat_z(nr, fr, t_vals[i]);
-      z[idx] = zi;
+      zi = pnr_sample_z(nr, fr, t_vals, u + r * N, i, N, perturb);
+      z[r * N + i] = zi;
     }
     if (sample_box != nullptr) {
       int32_t tag = -1;
+      // pnr_tag's rule, written out: sharing it changes the SASS of this kernel or of pnr_tag's callers
       for (int m = M - 1; m >= 0; --m) {   // first (nearest) containing interval wins
         const int32_t id = __shfl_sync(0xffffffffu, my_id, m);
         const float a = __shfl_sync(0xffffffffu, my_in, m), b = __shfl_sync(0xffffffffu, my_out, m);
@@ -184,7 +176,7 @@ __global__ void __launch_bounds__(kIvWarps * 32) interval_kernel(
   if (P.kept == 0) {   // no primitive on this ray: the uniform rule (already ascending)
     for (int i = lane; i < N; i += 32) {
       const int64_t idx = r * N + i;
-      z[idx] = (perturb > 0.f) ? pnr_strat_z_jitter(nr, fr, t_vals, i, N, u[idx]) : pnr_strat_z(nr, fr, t_vals[i]);
+      z[idx] = pnr_sample_z(nr, fr, t_vals, u + r * N, i, N, perturb);
       if (sample_box != nullptr) sample_box[idx] = -1;
     }
     return;
@@ -192,7 +184,7 @@ __global__ void __launch_bounds__(kIvWarps * 32) interval_kernel(
   int Pw = 1;
   while (Pw < N) Pw <<= 1;
   for (int k = lane; k < Pw; k += 32)
-    all[k] = k < N ? pnr_interval_z(&P, k, (perturb > 0.f) ? u[r * N + k] : 0.5f) : __int_as_float(0x7f800000);
+    all[k] = k < N ? pnr_interval_slot_z(&P, u + r * N, k, perturb) : __int_as_float(0x7f800000);
   __syncwarp();
   for (int k = 2; k <= Pw; k <<= 1)
     for (int j = k >> 1; j > 0; j >>= 1) {

@@ -1,6 +1,10 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
-// kernels (ray_kernels.cu) and a host build used by the CPU tests (tests/host_emu.cpp) to prove the
-// order matches the oracle bit for bit without a GPU.
+// kernels (ray_kernels.cu, rays_kernel in stream_kernels.cu) and a host build used by the CPU tests
+// (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep
+// only layout here (staging, shuffles, sorts); the rules they apply per ray - range clamps, sample depths,
+// output slots, camera directions - are the functions below, called by both builds.  Two pieces stay written
+// out in the kernels and again in host_emu.cpp, because moving them into a function changes the SASS:
+// intersect_kernel's per-primitive step and stratified_kernel's interval test (pnr_tag's rule).
 //
 // Rules (SURVEY.md 7.3 item 3): every multiply/add/subtract/divide is individually rounded (no FMA
 // contraction: __f*_rn intrinsics on device, -ffp-contract=off on host), true division, and min/max
@@ -249,6 +253,31 @@ PNR_HD void pnr_cross_emit(const PnrMeshCross* S, PnrHitList* L, int M, int32_t 
   }
 }
 
+// Triangle range [*k0, *k1) of primitive b, clamped into [0, T], so a malformed start table cannot read outside the
+// triangle table.  T < 2^31 (pnr_intersect_meshes checks it), so the range fits in int.
+PNR_HD void pnr_tri_range(const int32_t* tri_start, int b, int64_t T, int* k0, int* k1) {
+  const int64_t s0 = tri_start[b], s1 = tri_start[b + 1];
+  int64_t lo = s0 > 0 ? s0 : 0;
+  lo = lo < T ? lo : T;
+  int64_t hi = s1 > lo ? s1 : lo;
+  hi = hi < T ? hi : T;
+  *k0 = (int)lo;
+  *k1 = (int)hi;
+}
+// Output slots of ray r: the M nearest hits, then padding (id -1, depths 0); t_in starts at the origin.
+PNR_HD void pnr_hits_store(const PnrHitList* L, int M, int64_t r, uint8_t* hit, int32_t* box_id, float* t_in,
+                           float* t_out) {
+  hit[r] = L->n > 0 ? 1 : 0;
+#pragma unroll
+  for (int m = 0; m < PNR_MAX_HITS; ++m)
+    if (m < M) {
+      const bool v = m < L->n;
+      box_id[r * M + m] = v ? L->id[m] : -1;
+      t_in[r * M + m] = v ? pnr_max_nan(L->key[m], 0.f) : 0.f;
+      t_out[r * M + m] = v ? L->tout[m] : 0.f;
+    }
+}
+
 // a6
 PNR_HD float pnr_strat_z(float near, float far, float t) {
   return PNR_ADD(PNR_MUL(near, PNR_SUB(1.0f, t)), PNR_MUL(far, t));
@@ -259,6 +288,11 @@ PNR_HD float pnr_strat_z_jitter(float near, float far, const float* t_vals, int 
   if (i > 0) lower = PNR_MUL(0.5f, PNR_ADD(zi, pnr_strat_z(near, far, t_vals[i - 1])));
   if (i < N - 1) upper = PNR_MUL(0.5f, PNR_ADD(pnr_strat_z(near, far, t_vals[i + 1]), zi));
   return PNR_ADD(lower, PNR_MUL(PNR_SUB(upper, lower), u));
+}
+// depth of sample i of a ray (u_row: the ray's jitter row, read only when perturb > 0)
+PNR_HD float pnr_sample_z(float near, float far, const float* t_vals, const float* u_row, int i, int N,
+                          float perturb) {
+  return (perturb > 0.f) ? pnr_strat_z_jitter(near, far, t_vals, i, N, u_row[i]) : pnr_strat_z(near, far, t_vals[i]);
 }
 PNR_HD int32_t pnr_tag(float z, const int32_t* box_id, const float* t_in, const float* t_out, int M) {
   for (int m = 0; m < M; ++m)
@@ -336,6 +370,10 @@ PNR_HD float pnr_interval_z(const PnrIntervalPlan* P, int k, float c) {
   }
   return z;
 }
+// the same with the slot's c chosen (u_row: the ray's jitter row, read only when perturb > 0)
+PNR_HD float pnr_interval_slot_z(const PnrIntervalPlan* P, const float* u_row, int k, float perturb) {
+  return pnr_interval_z(P, k, (perturb > 0.f) ? u_row[k] : 0.5f);
+}
 
 // a10: cdf over the Nb = N-1 bin edges from coarse weights[0..N-1] (uses weights[1..N-2]).
 // Sequential running sums with a double accumulator rounded to fp32 per element (= torch.cumsum CPU).
@@ -402,4 +440,16 @@ PNR_HD void pnr_fisheye_dir(float u, float v, float g1, float g2, float u0, floa
   *x = PNR_MUL(fac, px);
   *y = PNR_MUL(fac, py);
   *z = PNR_SUB(fac, xi);
+}
+// Pinhole camera: pixel (u, v) -> unnormalised direction (x, y, 1) in the camera frame.
+PNR_HD void pnr_pinhole_dir(float u, float v, float fx, float fy, float cx, float cy, float* x, float* y, float* z) {
+  *x = PNR_DIV(PNR_SUB(u, cx), fx);
+  *y = PNR_DIV(PNR_SUB(v, cy), fy);
+  *z = 1.0f;
+}
+// Camera-frame direction -> world frame by the rotation of c2w (row-major 3x4 [R|t]).
+PNR_HD void pnr_cam_to_world(const float* c2w, float x, float y, float z, float* d0, float* d1, float* d2) {
+  *d0 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[0], x), PNR_MUL(c2w[1], y)), PNR_MUL(c2w[2], z));
+  *d1 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[4], x), PNR_MUL(c2w[5], y)), PNR_MUL(c2w[6], z));
+  *d2 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[8], x), PNR_MUL(c2w[9], y)), PNR_MUL(c2w[10], z));
 }

@@ -50,13 +50,11 @@ __global__ void __launch_bounds__(256) rays_kernel(CamArgs a, float* __restrict_
   if (i >= (int64_t)a.rows * a.W) return;
   const int v = a.row0 + (int)(i / a.W), u = (int)(i % a.W);
   float x, y, z;
-  if (a.camera == 0) {  // pinhole; every op separately rounded so the result equals the oracle's bit for bit
-    x = __fdiv_rn(__fsub_rn((float)u, a.cx), a.fx);
-    y = __fdiv_rn(__fsub_rn((float)v, a.cy), a.fy);
-    z = 1.0f;
-  } else if (a.camera == 2) {   // KITTI-360 fisheye (MEI): ray_math.h, also compiled for the host by the CPU tests
+  if (a.camera == 0) {   // pinhole and KITTI-360 fisheye (MEI): ray_math.h, also compiled for the host by the CPU tests
+    pnr_pinhole_dir((float)u, (float)v, a.fx, a.fy, a.cx, a.cy, &x, &y, &z);
+  } else if (a.camera == 2) {
     pnr_fisheye_dir((float)u, (float)v, a.fx, a.fy, a.cx, a.cy, a.xi, a.k1, a.k2, &x, &y, &z);
-  } else {
+  } else {   // equirect: device-only, sincosf rounds differently on the host
     const float lon = __fmul_rn(__fsub_rn(__fdiv_rn((float)u, (float)a.W), 0.5f), 6.2831853071795864769f);
     const float lat = __fmul_rn(__fsub_rn(0.5f, __fdiv_rn((float)v, (float)a.H)), 3.14159265358979323846f);
     float sl, cl, so, co;
@@ -65,9 +63,8 @@ __global__ void __launch_bounds__(256) rays_kernel(CamArgs a, float* __restrict_
     x = cl * so; y = -sl; z = cl * co;
   }
   float2* o = reinterpret_cast<float2*>(rays + i * 6);
-  const float d0 = __fadd_rn(__fadd_rn(__fmul_rn(a.c2w[0], x), __fmul_rn(a.c2w[1], y)), __fmul_rn(a.c2w[2], z));
-  const float d1 = __fadd_rn(__fadd_rn(__fmul_rn(a.c2w[4], x), __fmul_rn(a.c2w[5], y)), __fmul_rn(a.c2w[6], z));
-  const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(a.c2w[8], x), __fmul_rn(a.c2w[9], y)), __fmul_rn(a.c2w[10], z));
+  float d0, d1, d2;
+  pnr_cam_to_world(a.c2w, x, y, z, &d0, &d1, &d2);
   o[0] = make_float2(a.c2w[3], a.c2w[7]);
   o[1] = make_float2(a.c2w[11], d0);
   o[2] = make_float2(d1, d2);

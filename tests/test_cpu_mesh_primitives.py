@@ -1,5 +1,5 @@
 """CPU tier of the mesh primitives of a5 (DESIGN 3.2): the routines of csrc/ray_math.h built for the host with
--ffp-contract=off (tests/host_emu_mesh.cpp) equal the torch oracle (tests/oracle_mesh.py) bit for bit; the intervals
+-ffp-contract=off (tests/host_emu.cpp) equal the torch oracle (tests/oracle_mesh.py) bit for bit; the intervals
 agree with exact geometry; a cuboid given as 12 triangles agrees with the slab test; the KITTI-360 reader's mesh
 primitives; the argument checks of pnr_intersect_meshes (refused with PNR_ERR_ARG before any CUDA call: the pointers
 are placeholders that are never dereferenced) and the ctypes layout of pnr_render_args against the header."""
@@ -14,6 +14,7 @@ import pytest
 import torch
 
 import oracle_mesh as OM
+from host_emu import emu  # noqa: F401  (fixture)
 from oracle import reference_renderer as O
 from panopticnerf_b200 import _capi, make_cfg, synthetic as S
 from panopticnerf_b200.lib.datasets import kitti360 as K
@@ -23,15 +24,6 @@ from panopticnerf_b200.lib.datasets.kitti360 import intersection_cache as KC
 ROOT = Path(__file__).resolve().parent.parent
 X = 64          # a non-null placeholder pointer
 ERR_ARG = -1
-
-
-@pytest.fixture(scope="module")
-def emu():
-    out = ROOT / "build" / "host_emu_mesh.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu_mesh.cpp")])
-    return C.CDLL(str(out))
 
 
 def _p(t):
@@ -44,9 +36,9 @@ def emu_intersect(emu, rays, prims, M):
     bid = torch.zeros(R, M, dtype=torch.int32)
     tin, tout = torch.zeros(R, M), torch.zeros(R, M)
     tris = prims["mesh_tris"].contiguous()
-    emu.emu_intersect_meshes(_p(rays), C.c_int64(R), _p(prims["box_center"]), _p(prims["box_half"]),
-                             _p(prims["box_rot"]), _p(prims["mesh_tri_start"]), _p(tris), C.c_int64(tris.shape[0]), B,
-                             M, _p(hit), _p(bid), _p(tin), _p(tout))
+    emu.emu_intersect(_p(rays), C.c_int64(R), _p(prims["box_center"]), _p(prims["box_half"]),
+                      _p(prims["box_rot"]), _p(prims["mesh_tri_start"]), _p(tris), C.c_int64(tris.shape[0]), B, M,
+                      _p(hit), _p(bid), _p(tin), _p(tout))
     return hit.bool(), bid, tin, tout
 
 

@@ -3,26 +3,15 @@
 stratified depths, per-sample ids and sample_pdf indices.  No GPU needed; the GPU tests repeat these
 comparisons through the C ABI."""
 import ctypes as C
-import subprocess
-from pathlib import Path
+import math
 
 import numpy as np
 import pytest
 import torch
 
+from host_emu import emu  # noqa: F401  (fixture)
 from oracle import reference_renderer as O
 from panopticnerf_b200 import make_cfg, synthetic as S
-
-ROOT = Path(__file__).resolve().parent.parent
-
-
-@pytest.fixture(scope="module")
-def emu():
-    out = ROOT / "build" / "host_emu.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu.cpp")])
-    return C.CDLL(str(out))
 
 
 def _p(t):
@@ -40,7 +29,7 @@ def test_intersect_order(emu, B, M):
     bid = torch.zeros(R, M, dtype=torch.int32)
     tin, tout = torch.zeros(R, M), torch.zeros(R, M)
     emu.emu_intersect(_p(rays), C.c_int64(R), _p(bx["box_center"]), _p(bx["box_half"]), _p(bx["box_rot"]),
-                      B, M, _p(hit), _p(bid), _p(tin), _p(tout))
+                      None, None, C.c_int64(0), B, M, _p(hit), _p(bid), _p(tin), _p(tout))
     assert torch.equal(hit.bool(), ref[0]) and torch.equal(bid, ref[1])
     assert torch.equal(tin, ref[2]) and torch.equal(tout, ref[3])
     assert B < 64 or ref[0].any()
@@ -148,10 +137,36 @@ def test_fisheye_unprojection_order(emu):
     k = (1336.3220825849971, 1335.7883350012958, 716.94323510126321, 705.76498308221585, 2.2134047507854890,
          1.6798235660113681e-02, 1.6548773243373522)
     H = W = 1400
-    out = torch.zeros(H * W, 3)
-    emu.emu_fisheye(H, W, (C.c_float * 7)(*k), _p(out))
-    ref = O.generate_rays(H, W, k, torch.eye(4)[:3], "fisheye")
-    assert torch.equal(out, ref[:, 3:]) and torch.isfinite(out).all()
+    c2w = torch.eye(4)[:3].contiguous()
+    out = torch.zeros(H * W, 6)
+    assert emu.emu_generate_rays(H, W, 0, H, 2, (C.c_float * 7)(*k), _p(c2w), _p(out)) == 0
+    ref = O.generate_rays(H, W, k, c2w, "fisheye")
+    assert torch.equal(out[:, 3:], ref[:, 3:]) and torch.isfinite(out[:, 3:]).all()
+    assert torch.equal(out, ref)
+
+
+@pytest.mark.parametrize("camera,code", [("pinhole", 0), ("fisheye", 2)])
+def test_generate_rays_order(emu, camera, code):
+    """The ray generation the rays kernel runs (ray_math.h: pnr_pinhole_dir / pnr_fisheye_dir, then pnr_cam_to_world),
+    compiled for the host: origins and directions equal the oracle's bit for bit, for a rotated and translated camera
+    and a window of rows."""
+    cfg = make_cfg("cfg2")
+    k = (cfg.fx, cfg.fy, cfg.cx, cfg.cy) if camera == "pinhole" else \
+        (1336.3220825849971, 1335.7883350012958, 716.94323510126321, 705.76498308221585, 2.2134047507854890,
+         1.6798235660113681e-02, 1.6548773243373522)
+    H, W = (cfg.H, cfg.W_img) if camera == "pinhole" else (1400, 1400)
+    row0, rows = H // 3, 9
+    yaw, pitch = 0.3, -0.2
+    cy, sy, cp, sp = math.cos(yaw), math.sin(yaw), math.cos(pitch), math.sin(pitch)
+    rot = torch.tensor([[cy, 0.0, sy], [0.0, 1.0, 0.0], [-sy, 0.0, cy]], dtype=torch.float64) @ \
+        torch.tensor([[1.0, 0.0, 0.0], [0.0, cp, -sp], [0.0, sp, cp]], dtype=torch.float64)
+    c2w = torch.cat([rot, torch.tensor([[1.5], [-2.25], [0.75]], dtype=torch.float64)], 1).float().contiguous()
+    intr = (C.c_float * 7)(*(list(k) + [0.0] * (7 - len(k))))
+    out = torch.zeros(rows * W, 6)
+    assert emu.emu_generate_rays(H, W, row0, rows, code, intr, _p(c2w), _p(out)) == 0
+    ref = O.generate_rays(H, W, k, c2w, camera, row0=row0, rows=rows)
+    assert torch.equal(out, ref)
+    assert not torch.equal(ref[:, 3:], O.generate_rays(H, W, k, torch.eye(4)[:3], camera, row0=row0, rows=rows)[:, 3:])
 
 
 def test_pdf_cdf_sums_are_order_independent():
