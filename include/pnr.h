@@ -70,8 +70,12 @@ int pnr_create(const pnr_config* cfg, pnr_ctx** out);
 int pnr_destroy(pnr_ctx* ctx);
 
 /* a8 range check: sticky status of the fused-MLP launches enqueued so far on `stream` (synchronises it).
- * bit 0 (PNR_STATUS_RANGE): an activation left the range of the 16-bit operand format (fp16 modes: |x| > 65504)
- * or was not finite - the outputs of that launch are not trustworthy, re-run with PNR_PREC_BF16X3.
+ * bit 0 (PNR_STATUS_RANGE): a value written into a 16-bit operand - an embedding (gamma(x), gamma(d), hash-grid
+ * features), a trunk activation, a head's hidden activation, a scaled gradient of the backward program - had a hi
+ * part that rounds to inf (fp16 modes: |x| >= 65520; 65519 is carried exactly as 65504 + 15) or was NaN, or a
+ * hash-grid sample point was not finite.  Outputs of that launch are not trustworthy: a finite overflow, re-run with
+ * PNR_PREC_BF16X3.  The ReLU keeps NaN (as torch.relu does), so a NaN input or parameter also reaches the outputs.
+ * bit 1: pnr_update_weights packed a weight outside the fp16 range (fp16 modes; see there).
  * reset != 0 clears the word after reading it. */
 #define PNR_STATUS_RANGE 1u
 int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, void* stream);
@@ -94,7 +98,9 @@ int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
  * format (fp16 or bf16, cfg.precision), laid out as the no-swizzle K-major wgmma stage images of the packed weight
  * stream (csrc/mlp_program.h) and uploaded, together with the weights themselves, from which the programs built later
  * and pnr_update_weights pack on the device.  In the fp16 modes a packed weight with |w| > 65504 (after the
- * feature_linear fold) or not finite is rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode. */
+ * feature_linear fold) or not finite is rejected (PNR_ERR_UNSUPPORTED): use a bf16 mode.  The bf16 modes accept a
+ * NaN weight, and no mode checks the fp32 biases: a NaN there propagates to the outputs and sets bit 0 of pnr_status
+ * where it enters an operand. */
 int pnr_load_weights(pnr_ctx* ctx, const float* const* tensors_host, const int64_t* shapes, int32_t n);
 
 /* a5: ray / oriented-box slab test.  rays [R,6] (o||d); box_center, box_half [B,3]; box_rot [B,3,3]

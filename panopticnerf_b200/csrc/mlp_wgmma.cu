@@ -26,8 +26,9 @@
 // as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo with x = hi + lo split in the operand format: ~2^-21 relative
 // per product for fp16x3 (default; what the 1e-4 parity tolerance needs with margin), ~2^-17 for
 // bf16x3 (fp32 exponent range).  The 1-pass modes keep the first term only (fast, out of tolerance).
-// An activation outside the operand format's range (|x| > 65504 in the fp16 modes, non-finite in any) sets
-// bit 0 of the context's sticky status word: overflow is reported (pnr_status), never silent.
+// Range check: a value written into an operand (the embeddings included) whose hi part rounds to inf (fp16 modes:
+// |x| >= 65520) or that is NaN sets bit 0 of the context's sticky status word (pnr_status): overflow is reported, never
+// silent.  The ReLU keeps a NaN, as torch.relu does, so a NaN input or parameter reaches the outputs as well.
 #include <cstddef>
 #include "common.cuh"
 #include "composite_math.cuh"
@@ -51,9 +52,10 @@ __device__ __forceinline__ uint4 store_core_row(uint8_t* hi_base, uint8_t* lo_ba
 }
 
 // gamma(p) = [p, sin(2^0 p), cos(2^0 p), ...] padded with zeros to KPAD, streamed out 8 at a time.
+// The values carry a sign: `vmax` collects the magnitudes of the hi parts (range check), as in hash_rows.
 template <int PASSES, int FMT, int LMAX, int KPAD>
 __device__ __forceinline__ void encode_row(const float (&p)[3], int L, uint8_t* hi_base,
-                                           uint8_t* lo_base, int row) {
+                                           uint8_t* lo_base, int row, uint32_t& vmax) {
   float v[KPAD];
 #pragma unroll
   for (int i = 0; i < KPAD; ++i) v[i] = 0.f;
@@ -77,7 +79,9 @@ __device__ __forceinline__ void encode_row(const float (&p)[3], int L, uint8_t* 
     float w8[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) w8[j] = v[g * 8 + j];
-    store_core_row<PASSES, FMT>(hi_base, lo_base, g, row, w8);
+    const uint4 h = store_core_row<PASSES, FMT>(hi_base, lo_base, g, row, w8);
+    vmax = __vimax3_u16x2(vmax, h.x & 0x7FFF7FFFu, h.y & 0x7FFF7FFFu);
+    vmax = __vimax3_u16x2(vmax, h.z & 0x7FFF7FFFu, h.w & 0x7FFF7FFFu);
   }
 }
 
@@ -128,10 +132,18 @@ __device__ __forceinline__ void hash_rows_f(const MlpParams& p, const float (&v)
 // Epilogue building blocks.  One thread owns one accumulator row; groups are 16 columns.
 // ------------------------------------------------------------------------------------------------
 
+// relu(x) that keeps a NaN, as torch.relu does (fmaxf(NaN, 0) = 0 would hide a NaN input or parameter from the range
+// check and from the outputs): one FMNMX.NAN, the instruction count of fmaxf.
+__device__ __forceinline__ float relu_nan(float x) {
+  float y;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 // relu(acc + bias) of columns 4q .. 4q + 3 of a 16-column group, b = their bias
 __device__ __forceinline__ float4 relu_bias4(const uint32_t (&r)[16], int q, float4 b) {
-  return make_float4(fmaxf(__uint_as_float(r[4 * q + 0]) + b.x, 0.f), fmaxf(__uint_as_float(r[4 * q + 1]) + b.y, 0.f),
-                     fmaxf(__uint_as_float(r[4 * q + 2]) + b.z, 0.f), fmaxf(__uint_as_float(r[4 * q + 3]) + b.w, 0.f));
+  return make_float4(relu_nan(__uint_as_float(r[4 * q + 0]) + b.x), relu_nan(__uint_as_float(r[4 * q + 1]) + b.y),
+                     relu_nan(__uint_as_float(r[4 * q + 2]) + b.z), relu_nan(__uint_as_float(r[4 * q + 3]) + b.w));
 }
 
 // activation -> next layer's A operand: v = act(acc + bias); [sigma += v . wsig]; split into hi / lo parts.
@@ -150,10 +162,10 @@ __device__ __forceinline__ void epi_group_act(const uint32_t (&r)[16], int g, co
     }
     split_x2<FMT>(v.x, v.y, hi[2 * q], lo[2 * q]);
     split_x2<FMT>(v.z, v.w, hi[2 * q + 1], lo[2 * q + 1]);
-    // Range check on the packed hi parts (one 3-input 16x2 max per four values): v >= 0 after the ReLU, so the
-    // 16-bit patterns order like the values, with +inf (what an overflowing conversion yields) and NaN on top.
-    // (fmaxf turns a NaN accumulator into 0, but a NaN can only follow an overflow that was flagged where it
-    // happened - which is why the check sits in every layer and not only on the outputs.)
+    // Range check on the packed hi parts (one 3-input 16x2 max per four values): v >= +0 or the canonical (positive)
+    // NaN after the ReLU, so the 16-bit patterns order like the values, with +inf (what an overflowing conversion
+    // yields, fp16: v >= 65520) and NaN on top.  The ReLU keeps a NaN accumulator (a NaN input, bias or weight), so it
+    // is seen here and reaches the outputs.
 #ifndef PNR_ABL_NOVMAX
     vmax = __vimax3_u16x2(vmax, hi[2 * q], hi[2 * q + 1]);
 #endif
@@ -483,8 +495,8 @@ __device__ __forceinline__ void epi_regs_act(const float (&d)[64], const float* 
   for (int j = 0; j < 16; ++j) {
     const float2 b = *reinterpret_cast<const float2*>(bias + 128 * HALF + 8 * j);
     uint32_t h0, l0, h1, l1;
-    split_x2<FMT>(fmaxf(d[4 * j + 0] + b.x, 0.f), fmaxf(d[4 * j + 1] + b.y, 0.f), h0, l0);
-    split_x2<FMT>(fmaxf(d[4 * j + 2] + b.x, 0.f), fmaxf(d[4 * j + 3] + b.y, 0.f), h1, l1);
+    split_x2<FMT>(relu_nan(d[4 * j + 0] + b.x), relu_nan(d[4 * j + 1] + b.y), h0, l0);
+    split_x2<FMT>(relu_nan(d[4 * j + 2] + b.x), relu_nan(d[4 * j + 3] + b.y), h1, l1);
 #ifndef PNR_ABL_NOVMAX
     vmax = __vimax3_u16x2(vmax, h0, h1);   // range check, as in epi_group_act
 #endif
@@ -571,11 +583,14 @@ __device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgr
       for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(d[c], nrm);
     }
     if (dir_thread) {
-      if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow);
+      if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow, vmax);
     } else if (!hashgrid) {
-      encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow);
+      encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow, vmax);
     }
     if (hashgrid) {
+      // a non-finite point is flagged here: the clamp below sends a NaN to the corner (0,0,0), whose features are
+      // finite (the clamp stays: a NaN must never become a table index)
+      if (!(isfinite(x[0]) && isfinite(x[1]) && isfinite(x[2]))) vmax |= 0xFFFFu;
       float v[3];
       hash_normalize(x, p.hash_aabb, v);
       const int nc = ((p.hash_L * p.hash_F + 15) & ~15) / 8, half = (nc + 1) / 2;   // core rows the MMAs read

@@ -532,8 +532,8 @@ extern "C" int pnr_destroy(pnr_ctx* ctx) {
   return PNR_OK;
 }
 
-// Sticky status of the fused MLP launches enqueued so far on `stream` (synchronises that stream): bit 0 = an
-// activation left the range of the 16-bit operand format (fp16 modes: |x| > 65504) or was not finite - the
+// Sticky status of the fused MLP launches enqueued so far on `stream` (synchronises that stream): bit 0 = a value
+// written into a 16-bit operand rounded to inf (fp16 modes: |x| >= 65520) or was NaN (include/pnr.h) - the
 // results of that launch are not trustworthy; re-run with PNR_PREC_BF16X3.  reset != 0 clears the word.
 extern "C" int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, void* stream) {
   PNR_CHECK_ARG(ctx && status_host, "pnr_status: null pointer");

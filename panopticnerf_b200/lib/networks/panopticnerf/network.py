@@ -308,8 +308,10 @@ class Network(nn.Module):
 
     def range_status(self, reset: bool = True) -> int:
         """Sticky range-check word of this network's fused-MLP launches (synchronises the current stream).
-        Bit 0 set: an activation left the range of the 16-bit operand format (fp16 modes: |x| > 65504) or was not
-        finite - those outputs are wrong; use precision='bf16x3' for this network."""
+        Bit 0 set: a value written into a 16-bit operand (an embedding, an activation, a scaled gradient) rounded to inf
+        in that format (fp16 modes: |x| >= 65520) or was NaN - those outputs are wrong; for a finite overflow use
+        precision='bf16x3' for this network.  A NaN input or parameter also reaches the outputs as NaN.
+        Bit 1 set: pnr_update_weights packed a weight outside the fp16 range."""
         if self._ctx is None:
             return 0
         dev = torch.device(self._ctx_key[0])
@@ -327,5 +329,5 @@ class Network(nn.Module):
                                  "the packed weights are invalid; use cfg.precision = 'bf16x3'")
         if st & 1:
             raise _capi.PnrError(
-                f"Network: an activation left the range of the {self.precision} tensor-core operands (|x| > 65504 "
-                "or non-finite) - the MLP outputs of this call are invalid; use cfg.precision = 'bf16x3'")
+                f"Network: an activation left the range of the {self.precision} tensor-core operands (|x| >= 65520 in "
+                "fp16, or NaN) - the MLP outputs of this call are invalid; use cfg.precision = 'bf16x3'")

@@ -18,13 +18,20 @@ def _net(cfg, seed=3):
     return S.init_network_weights(make_network(cfg), seed=seed)
 
 
-@pytest.mark.parametrize("value", [1e5, float("nan")], ids=["1e5", "nan"])
+WEIGHTS = [1e5, float("nan"), 65504.0, -65504.0, 65505.0, -65505.0, float("inf"), float("-inf")]
+
+
+@pytest.mark.parametrize("value", WEIGHTS, ids=["1e5", "nan", "65504", "-65504", "65505", "-65505", "inf", "-inf"])
 @pytest.mark.parametrize("precision", ["fp16x3", "fp16"])
 def test_trunk_weight_outside_fp16_is_refused(precision, value):
+    """|w| <= 65504 is packed; 65505, +-Inf and NaN are refused (the host twin of pnr_update_weights' bit 1)."""
     cfg = make_cfg("cfg2", precision=precision)
     net = _net(cfg)
     with torch.no_grad():
         net.pts_linears[3].weight[5, 7] = value
+    if abs(value) <= 65504.0:
+        build(cfg, net)
+        return
     with pytest.raises(_capi.PnrError, match=rf"rc={ERR_UNSUPPORTED}\).*outside the fp16 range"):
         build(cfg, net)
     build(make_cfg("cfg2", precision="bf16x3"), net)          # the bf16 range holds it
