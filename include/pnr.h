@@ -84,7 +84,9 @@ int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, void* stream)
  * fp32, a caller-owned DEVICE pointer.  It is not copied: every fused-MLP launch of the context (pnr_mlp_forward,
  * pnr_mlp_composite, pnr_mlp_trunk_forward, pnr_mlp_backward_trunk, pnr_render_fused) reads it when it executes, so an
  * in-place update on the same stream is seen by the next launch.  Those entry points return PNR_ERR_STATE on a
- * hash-grid context without a table; NULL unbinds.  PNR_ERR_STATE on a frequency context. */
+ * hash-grid context without a table; NULL unbinds.  PNR_ERR_STATE on a frequency context.  A table that is not
+ * aligned to one corner's features when they are read as a vector (8 bytes at F = 2, 16 at F = 4) is refused
+ * (PNR_ERR_ARG), here and by pnr_hashgrid_encode. */
 int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
 
 /* a2: load a Network state_dict.  `tensors_host[i]` are HOST fp32 pointers in this fixed order:
@@ -462,6 +464,34 @@ int pnr_comm_unique_id(uint8_t* id_out);
 int pnr_comm_init(pnr_comm** out, const uint8_t* id, int32_t rank, int32_t world, int32_t device);
 int pnr_comm_destroy(pnr_comm* comm);
 int pnr_allgather_outputs(pnr_comm* comm, const void* send, void* recv, size_t bytes_per_rank, void* stream);
+/* buf [bytes] on every rank <- root's buf, asynchronously on `stream` (data-parallel training starts every replica from
+ * rank 0's parameters and optimiser state with it). */
+int pnr_broadcast(pnr_comm* comm, void* buf, size_t bytes, int32_t root, void* stream);
+
+/* Adam over one flat fp32 parameter vector param [P] with moments exp_avg, exp_avg_sq [P], whose gradient is the sum of
+ * G slices grads[g * ld_grad + i] (the all-gathered gradients of G data-parallel ranks), added in rank order
+ * g = 0, 1, ..., G-1 in fp32 starting from slice 0 (G = 1 uses the slice as it is).  The update is torch.optim.Adam's
+ * single-tensor path (foreach=False), operation for operation, every operation rounded to fp32 (no FMA contraction):
+ *   g += weight_decay * p                                      (only when weight_decay != 0)
+ *   m  = lerp(m, g, w1), w1 = (float)(1 - beta1):  m + w1 * (g - m) when w1 < 0.5, else g - (g - m) * (1 - w1)
+ *   v  = v * (float)beta2 + ((float)(1 - beta2) * g) * g
+ *   denom = sqrt(v) / bc2_sqrt + eps
+ *   p  = p + (-step_size) * (m / denom)
+ * beta1, beta2: as the user set them (double; rounded as torch's kernels receive them); step_size = lr / (1 - beta1^t)
+ * and bc2_sqrt = sqrt(1 - beta2^t), computed by the caller in double for step t and rounded to float.
+ * grad_sum [P] (nullable) receives the summed gradient (before weight decay).  NaN and Inf propagate, unsuppressed.
+ * HBM-bound: (G + 3) reads and 3 writes of 4P bytes (+ one write with grad_sum); 16-byte accesses when ld_grad % 4 == 0
+ * and every buffer is 16-byte aligned.  Refused before any launch (PNR_ERR_ARG): G < 1, P < 0, ld_grad < P, a null
+ * buffer when P > 0, a hyper-parameter that is not finite, betas outside [0, 1), eps, weight_decay or step_size < 0,
+ * bc2_sqrt <= 0. */
+typedef struct pnr_adam_args {
+  int64_t P, ld_grad;
+  int32_t G;
+  double beta1, beta2;
+  float eps, weight_decay, step_size, bc2_sqrt;
+} pnr_adam_args;
+int pnr_adam_step(const float* grads, float* param, float* exp_avg, float* exp_avg_sq, const pnr_adam_args* args,
+                  float* grad_sum, void* stream);
 
 /* Evaluation of rendered frames against their ground truth (the step after pnr_panoptic_fuse; the reference's
  * evaluator is not in the mount, so these rules are chosen here - DESIGN.md 3.4, oracle/reference_eval.py).

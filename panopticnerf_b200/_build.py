@@ -14,7 +14,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libpnr.so"
-SOURCES = ["pnr_api.cu", "ray_kernels.cu", "stream_kernels.cu", "mlp_wgmma.cu", "render.cu", "comm.cu", "panoptic_kernels.cu", "wgrad_wgmma.cu", "linear_wgmma.cu", "eval_kernels.cu"]
+SOURCES = ["pnr_api.cu", "ray_kernels.cu", "stream_kernels.cu", "mlp_wgmma.cu", "render.cu", "comm.cu", "panoptic_kernels.cu", "wgrad_wgmma.cu", "linear_wgmma.cu", "eval_kernels.cu", "optim_kernels.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC"] + os.environ.get("PNR_NVCC_FLAGS", "").split()
 

@@ -76,6 +76,13 @@ class PnrRenderArgs(C.Structure):
                 ("mesh_tri_start", C.c_void_p), ("mesh_tris", C.c_void_p), ("T", C.c_int64)]
 
 
+class PnrAdamArgs(C.Structure):
+    """pnr_adam_args of include/pnr.h."""
+    _fields_ = [("P", C.c_int64), ("ld_grad", C.c_int64), ("G", C.c_int32), ("beta1", C.c_double),
+                ("beta2", C.c_double), ("eps", C.c_float), ("weight_decay", C.c_float), ("step_size", C.c_float),
+                ("bc2_sqrt", C.c_float)]
+
+
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
 COMM_ID_BYTES = 128
 
@@ -128,6 +135,8 @@ SIGNATURES = {
     "pnr_comm_init": (C.c_int, [C.POINTER(_vp), C.POINTER(C.c_uint8), _i32, _i32, _i32]),
     "pnr_comm_destroy": (C.c_int, [_vp]),
     "pnr_allgather_outputs": (C.c_int, [_vp, _vp, _vp, C.c_size_t, _vp]),
+    "pnr_broadcast": (C.c_int, [_vp, _vp, C.c_size_t, _i32, _vp]),
+    "pnr_adam_step": (C.c_int, [_vp, _vp, _vp, _vp, C.POINTER(PnrAdamArgs), _vp, _vp]),
     "pnr_launch_count": (_i64, [_i32]),
     "pnr_eval_workspace_bytes": (C.c_size_t, [_i64]),
     "pnr_eval_semantic": (C.c_int, [_vp, _vp, _i64, _i32, _vp, _i32, _vp, _vp]),

@@ -1,6 +1,8 @@
 // comm.cu — the multi-GPU entry points of the C ABI (SURVEY.md 8(b) "Multi-GPU entry", 8(e)): one NCCL
 // communicator per context and ONE all-gather of the rendered per-ray tiles (image / label tiles) over NVLink.
-// Rays shard with no data-path collective; this gather is the only exchange step on the path.
+// Rays shard with no data-path collective; this gather is the only exchange step on the path.  Data-parallel
+// training (lib/train/data_parallel.py) reuses the same all-gather for its gradients and counts, and a broadcast once
+// at start-up.
 //
 // NCCL is bound at run time (dlopen of libnccl.so.2, the soname both the system package and the PyTorch wheel
 // install): libpnr keeps loading on boxes without NCCL, and inside a PyTorch process the already-loaded copy is
@@ -11,7 +13,7 @@
 
 namespace pnr {
 
-// Minimal NCCL surface, declared here so that no NCCL header version is baked in (the ABI of these five
+// Minimal NCCL surface, declared here so that no NCCL header version is baked in (the ABI of these six
 // functions has been stable across NCCL 2.x).
 struct NcclUniqueId { char internal[PNR_COMM_ID_BYTES]; };
 typedef struct ncclComm* NcclComm;
@@ -23,6 +25,7 @@ struct NcclApi {
   NcclResult (*CommInitRank)(NcclComm*, int, NcclUniqueId, int) = nullptr;
   NcclResult (*CommDestroy)(NcclComm) = nullptr;
   NcclResult (*AllGather)(const void*, void*, size_t, int, NcclComm, cudaStream_t) = nullptr;
+  NcclResult (*Broadcast)(const void*, void*, size_t, int, int, NcclComm, cudaStream_t) = nullptr;
   const char* (*GetErrorString)(NcclResult) = nullptr;
   NcclResult (*GetVersion)(int*) = nullptr;
   bool ok = false;
@@ -48,9 +51,11 @@ static NcclApi& nccl() {
     api.CommInitRank = (decltype(api.CommInitRank))sym("ncclCommInitRank");
     api.CommDestroy = (decltype(api.CommDestroy))sym("ncclCommDestroy");
     api.AllGather = (decltype(api.AllGather))sym("ncclAllGather");
+    api.Broadcast = (decltype(api.Broadcast))sym("ncclBroadcast");
     api.GetErrorString = (decltype(api.GetErrorString))sym("ncclGetErrorString");
     api.GetVersion = (decltype(api.GetVersion))sym("ncclGetVersion");
-    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.GetErrorString;
+    api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllGather && api.Broadcast &&
+             api.GetErrorString;
   });
   return api;
 }
@@ -122,5 +127,16 @@ extern "C" int pnr_allgather_outputs(pnr_comm* comm, const void* send, void* rec
   PNR_CHECK_ARG(send && recv, "pnr_allgather_outputs: null pointer");
   DeviceGuard guard(comm->device);
   PNR_NCCL(nccl().AllGather(send, recv, bytes_per_rank, kNcclUint8, comm->comm, (cudaStream_t)stream));
+  return PNR_OK;
+}
+
+// buf [bytes] <- root's buf on every rank, in place.  Asynchronous on `stream`.
+extern "C" int pnr_broadcast(pnr_comm* comm, void* buf, size_t bytes, int32_t root, void* stream) {
+  PNR_CHECK_ARG(comm, "pnr_broadcast: null communicator");
+  PNR_CHECK_ARG(root >= 0 && root < comm->world, "pnr_broadcast: root %d of %d", root, comm->world);
+  if (bytes == 0) return PNR_OK;
+  PNR_CHECK_ARG(buf, "pnr_broadcast: null pointer");
+  DeviceGuard guard(comm->device);
+  PNR_NCCL(nccl().Broadcast(buf, buf, bytes, kNcclUint8, root, comm->comm, (cudaStream_t)stream));
   return PNR_OK;
 }

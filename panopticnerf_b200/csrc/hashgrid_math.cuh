@@ -15,6 +15,12 @@ namespace pnr {
 
 constexpr int kHashMaxLevels = 32;
 
+// Byte alignment the table needs: a corner's F = 2 / 4 features are read as one float2 / float4
+inline bool hash_table_aligned(const float* table, int F) {
+  const uintptr_t a = F == 4 ? 16 : F == 2 ? 8 : 4;
+  return (reinterpret_cast<uintptr_t>(table) & (a - 1)) == 0;
+}
+
 // res_l = floor(base * scale^l), evaluated in double
 inline void hash_level_resolutions(int L, float base, float scale, uint32_t* res) {
   for (int l = 0; l < L; ++l) res[l] = (uint32_t)floor((double)base * pow((double)scale, (double)l));

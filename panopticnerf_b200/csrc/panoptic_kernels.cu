@@ -193,6 +193,7 @@ extern "C" int pnr_hashgrid_encode(const float* x, int64_t n, const float* aabb,
   if (n == 0) return PNR_OK;
   PNR_CHECK_ARG(x && table && out && n > 0, "pnr_hashgrid_encode: null pointer");
   PNR_CHECK_ARG(L >= 1 && L <= 32 && (F == 1 || F == 2 || F == 4 || F == 8), "pnr_hashgrid_encode: L=%d F=%d (L in [1,32], F in {1,2,4,8})", L, F);
+  PNR_CHECK_ARG(hash_table_aligned(table, F), "pnr_hashgrid_encode: table not aligned to its %d features (a float%d per corner)", F, F);
   PNR_CHECK_ARG(T_log2 >= 4 && T_log2 <= 28, "pnr_hashgrid_encode: T_log2=%d outside [4,28]", T_log2);
   PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "pnr_hashgrid_encode: base_resolution / per_level_scale < 1");
   const double finest = (double)base_resolution * pow((double)per_level_scale, (double)(L - 1));

@@ -860,6 +860,9 @@ extern "C" int pnr_program_host(const pnr_config* cfg, const float* const* t, co
 extern "C" int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table) {
   PNR_CHECK_ARG(ctx, "pnr_bind_hashgrid_table: null context");
   if (!is_hashgrid(ctx->cfg)) return set_error(PNR_ERR_STATE, "pnr_bind_hashgrid_table: not a hash-grid context");
+  PNR_CHECK_ARG(!table || hash_table_aligned(table, ctx->cfg.hash_features),
+                "pnr_bind_hashgrid_table: table not aligned to its %d features (a float%d per corner)",
+                ctx->cfg.hash_features, ctx->cfg.hash_features);
   ctx->hash_table = table;
   return PNR_OK;
 }

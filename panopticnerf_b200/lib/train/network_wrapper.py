@@ -53,6 +53,11 @@ class NetworkWrapper(torch.nn.Module):
 
 
 def make_network_wrapper(cfg, net, net_fine=None):
-    """The NetworkWrapper of cfg.trainer_module (the reference's make_trainer resolves its wrapper the same way)."""
+    """The NetworkWrapper of cfg.trainer_module (the reference's make_trainer resolves its wrapper the same way); with
+    cfg.distributed set and the torch.distributed process group up, the DataParallelWrapper of this rank (train it
+    with FusedAdam(wrapper.parameters(), comm=wrapper.comm))."""
+    from .data_parallel import DataParallelWrapper, is_data_parallel
+    if is_data_parallel(cfg) and not getattr(cfg, "trainer_module", None):
+        return DataParallelWrapper(cfg, net, net_fine)
     module = importlib.import_module(getattr(cfg, "trainer_module", None) or DEFAULT_MODULE)
     return module.NetworkWrapper(cfg, net, net_fine)

@@ -37,6 +37,27 @@ def shard_batch(batch: Dict[str, torch.Tensor], rank: int, world: int) -> Dict[s
     return out
 
 
+TRAIN_RAY_KEYS = ("rays", "near", "far", "u", "u_fine", "noise", "noise_fine", "rgb", "depth", "pseudo_label",
+                  "pseudo_weight")
+
+
+def shard_training_batch(batch: Dict[str, torch.Tensor], rank: int, world: int) -> Dict[str, torch.Tensor]:
+    """A training batch's shard for data-parallel training: the rays and every per-ray target and random draw
+    (TRAIN_RAY_KEYS) are sliced to `shard_range`; scene tensors (primitives, meshes, aabb) are replicated.  A rank past
+    the last ray gets an empty shard (zero rows)."""
+    R = batch["rays"].shape[0]
+    lo, hi = shard_range(R, rank, world)
+    out = {}
+    for k, v in batch.items():
+        if k in TRAIN_RAY_KEYS and torch.is_tensor(v):
+            if v.dim() < 1 or v.shape[0] != R:
+                raise ValueError(f"shard_training_batch: {k} has shape {tuple(v.shape)}, expected a leading dim of R={R}")
+            out[k] = v[lo:hi].contiguous()
+        else:
+            out[k] = v
+    return out
+
+
 def all_gather_maps(local: Dict[str, torch.Tensor], R: int, keys: Iterable[str] = DEFAULT_KEYS,
                     group: Optional[dist.ProcessGroup] = None) -> Dict[str, torch.Tensor]:
     """One all_gather_into_tensor of the selected per-ray maps, packed as a single [per, F] fp32 tile
@@ -69,7 +90,9 @@ class TileGather:
     label tiles : pnr_label_tiles first - rgb as u8, depth f32, semantic / instance argmax as i16 = 11 B per ray
                   (13 with both labels) instead of 4*(5+C+K): what a consumer of the rendered image / label tiles
                   needs (north_star), ~35x fewer bytes over NVLink than the logits at cfg3 / cfg5.
-    torch.distributed is used once, to hand rank 0's NCCL unique id to the other ranks."""
+    torch.distributed is used once, to hand rank 0's NCCL unique id to the other ranks.
+    Data-parallel training (lib/train/data_parallel.py) uses the same communicator: `allgather` of tensors (gradients,
+    counts) and `broadcast` of the start-up state."""
 
     def __init__(self, device, group: Optional[dist.ProcessGroup] = None):
         import ctypes as C
@@ -111,6 +134,21 @@ class TileGather:
                 self._h, tile.data_ptr(), full.data_ptr(), tile.numel(), self._capi.stream_ptr()),
                 "pnr_allgather_outputs")
         return full
+
+    def allgather(self, t: torch.Tensor) -> torch.Tensor:
+        """[world, *t.shape] <- every rank's t (contiguous, on self.device, any dtype), in rank order; asynchronous on
+        the current stream."""
+        full = self._gather_bytes(t.contiguous().reshape(-1).view(torch.uint8))
+        return full.view(t.dtype).reshape((self.world,) + tuple(t.shape))
+
+    def broadcast(self, t: torch.Tensor, root: int = 0) -> torch.Tensor:
+        """t (contiguous, on self.device) <- root's t, in place (pnr_broadcast)."""
+        if not t.is_contiguous() or t.device != self.device:
+            raise self._capi.PnrError(f"broadcast: expected a contiguous tensor on {self.device}")
+        with torch.cuda.device(self.device):
+            self._capi.check(self._capi.lib().pnr_broadcast(self._h, t.data_ptr(), t.numel() * t.element_size(), root,
+                                                            self._capi.stream_ptr()), "pnr_broadcast")
+        return t
 
     def gather_maps(self, local: Dict[str, torch.Tensor], R: int, keys: Iterable[str] = DEFAULT_KEYS):
         """fp32 maps (same result as all_gather_maps, through the C ABI)."""
