@@ -166,6 +166,55 @@ int pnr_tag_samples(const float* z, int64_t R, int32_t N, const int32_t* box_id,
 int pnr_generate_rays(int32_t H, int32_t W, int32_t row0, int32_t rows, int32_t camera, const float* intr_host,
                       const float* c2w_host, float* rays, void* stream);
 
+/* A training batch of random pixels from a set of frames kept on the device (DESIGN 3.4): per ray the camera ray,
+ * its targets and its sampling jitter.
+ * Frame set (caller-owned, device): c2w [F, 12] (row-major 3x4 [R|t] as pnr_generate_rays), frame_cam [F] i32 (an
+ * entry of cams), pix_offset [F+1] i64: frame f owns the flat pixels [off[f], off[f+1]), row-major over (v, u) of its
+ * camera's W, off[0] = 0, off[F] = P (a malformed table is clamped, never read outside); per pixel rgb8 [P, 3] u8 and
+ * optionally label [P] i16 (-1 = ignore) and depth [P] f32 (<= 0 = none).  cams[0 .. num_cameras): model 0 pinhole
+ * (intr = fx, fy, cx, cy) or 2 fisheye (gamma1, gamma2, u0, v0, xi, k1, k2); the equirect model (1) is refused, its
+ * rays are device-only.
+ * Draws: Philox4x32-10 with key = seed (low word first) and counter (block, r, step low word, step high word) for the
+ * global ray index r.  Block 0: the pixel p = mulhi64(w0 << 32 | w1, P) (the high 64 bits of the 128-bit product), the
+ * frame f by an upper-bound search of pix_offset, (v, u) = divmod(p - off[f], W).  Blocks 1, 2, ...: jitter word k
+ * (k = 0 .. N+Ni) is word k % 4 of block 1 + k / 4, as (w >> 8) * 2^-24; u[r, j] = word j, u_fine[r, j] = word N + j.
+ * Every output row is a function of (seed, step, r) alone: the launch writes the rays r0 .. r1-1 into rows
+ * 0 .. r1-r0-1, equal bit for bit to the matching rows of [0, R).
+ * Outputs [r1 - r0, ...]: rays [., 6] (row v*W + u of pnr_generate_rays for that frame, bit for bit), rgb [., 3] =
+ * byte / 255 (true division), u [., N], u_fine [., Ni] (needed when Ni > 0); nullable: depth_out [.] (0 without a depth
+ * table), pseudo_label [.] i32 (-1 without a label table), pixel [.] i64 (the flat index p).
+ * Refused before any launch (PNR_ERR_ARG, by name): F < 1 or >= 2^31 - 1, P < 1, r0 < 0, r1 < r0, r1 > 2^32, N outside
+ * [1, 256], Ni < 0 or N + Ni > 256, num_cameras outside [1, PNR_RAY_BATCH_MAX_CAMERAS], a camera model other than 0 / 2
+ * or H, W < 1, a null frame-set or required output pointer. */
+#define PNR_RAY_BATCH_MAX_CAMERAS 4
+typedef struct pnr_ray_camera {
+  int32_t model, H, W;
+  float intr[7];
+} pnr_ray_camera;
+typedef struct pnr_ray_batch_args {
+  const float* c2w;
+  const int32_t* frame_cam;
+  const int64_t* pix_offset;
+  int32_t F;
+  int64_t P;
+  const uint8_t* rgb8;
+  const int16_t* label;
+  const float* depth;
+  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
+  int32_t num_cameras;
+  uint64_t seed, step;
+  int64_t r0, r1;
+  int32_t N, Ni;
+  float* rays;
+  float* rgb;
+  float* depth_out;
+  int32_t* pseudo_label;
+  float* u;
+  float* u_fine;
+  int64_t* pixel;
+} pnr_ray_batch_args;
+int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream);
+
 /* a7: standalone positional encoding, out [n, 3+6L]. */
 int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void* stream);
 

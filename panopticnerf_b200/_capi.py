@@ -83,6 +83,24 @@ class PnrAdamArgs(C.Structure):
                 ("bc2_sqrt", C.c_float)]
 
 
+RAY_BATCH_MAX_CAMERAS = 4
+
+
+class PnrRayCamera(C.Structure):
+    """pnr_ray_camera of include/pnr.h."""
+    _fields_ = [("model", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("intr", C.c_float * 7)]
+
+
+class PnrRayBatchArgs(C.Structure):
+    """pnr_ray_batch_args of include/pnr.h (same field order)."""
+    _fields_ = [("c2w", C.c_void_p), ("frame_cam", C.c_void_p), ("pix_offset", C.c_void_p), ("F", C.c_int32),
+                ("P", C.c_int64), ("rgb8", C.c_void_p), ("label", C.c_void_p), ("depth", C.c_void_p),
+                ("cams", PnrRayCamera * RAY_BATCH_MAX_CAMERAS), ("num_cameras", C.c_int32),
+                ("seed", C.c_uint64), ("step", C.c_uint64), ("r0", C.c_int64), ("r1", C.c_int64),
+                ("N", C.c_int32), ("Ni", C.c_int32)] + \
+               [(k, C.c_void_p) for k in ("rays", "rgb", "depth_out", "pseudo_label", "u", "u_fine", "pixel")]
+
+
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
 COMM_ID_BYTES = 128
 
@@ -104,6 +122,7 @@ SIGNATURES = {
     "pnr_sample_intervals": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _f32, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "pnr_tag_samples": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
     "pnr_generate_rays": (C.c_int, [_i32, _i32, _i32, _i32, _i32, C.POINTER(_f32), C.POINTER(_f32), _vp, _vp]),
+    "pnr_sample_ray_batch": (C.c_int, [C.POINTER(PnrRayBatchArgs), _vp]),
     "pnr_encode": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_forward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_composite": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i32,

@@ -1,8 +1,9 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
-// kernels (ray_kernels.cu, rays_kernel in stream_kernels.cu) and a host build used by the CPU tests
-// (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep
-// only layout here (staging, shuffles, sorts); the rules they apply per ray - range clamps, sample depths,
-// output slots, camera directions - are the functions below, called by both builds.  Two pieces stay written
+// kernels (ray_kernels.cu, rays_kernel and ray_batch_kernel in stream_kernels.cu) and a host build used by the CPU tests
+// (tests/host_emu.cpp; tests/host_emu_ray_batch.cpp for the ray-batch routine) to prove the order matches the oracle
+// bit for bit without a GPU.  The kernels keep only layout here (staging, shuffles, sorts); the rules they apply per
+// ray - range clamps, sample depths, output slots, camera directions, batch draws - are the functions below, called by
+// both builds.  Two pieces stay written
 // out in the kernels and again in host_emu.cpp, because moving them into a function changes the SASS:
 // intersect_kernel's per-primitive step and stratified_kernel's interval test (pnr_tag's rule).
 //
@@ -12,6 +13,7 @@
 #pragma once
 #include <stdint.h>
 #include <math.h>
+#include "../../include/pnr.h"   // pnr_ray_batch_args: the ray-batch routine reads the entry point's own arguments
 
 #if defined(__CUDACC__)
 #define PNR_HD __host__ __device__ __forceinline__
@@ -452,4 +454,105 @@ PNR_HD void pnr_cam_to_world(const float* c2w, float x, float y, float z, float*
   *d0 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[0], x), PNR_MUL(c2w[1], y)), PNR_MUL(c2w[2], z));
   *d1 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[4], x), PNR_MUL(c2w[5], y)), PNR_MUL(c2w[6], z));
   *d2 = PNR_ADD(PNR_ADD(PNR_MUL(c2w[8], x), PNR_MUL(c2w[9], y)), PNR_MUL(c2w[10], z));
+}
+
+// ---------------------------------------------------------------------------------------------- training ray batches
+// pnr_sample_ray_batch (include/pnr.h; DESIGN 3.4): a random pixel of a frame set per ray, its camera ray, targets and
+// jitter, all a function of (seed, step, global ray index).  Integer work (Philox, the 64-bit multiply, the search) is
+// exact on both builds; the float work is the camera routines above and one true division per colour channel.
+
+// Philox4x32-10 (Salmon, Moraes, Dror, Shaw, SC 2011): 10 rounds of two 32x32 -> 64-bit multiplies, the key bumped by
+// the Weyl constants between rounds.
+PNR_HD void pnr_mulhilo32(uint32_t a, uint32_t b, uint32_t* hi, uint32_t* lo) {
+#if defined(__CUDA_ARCH__)
+  *hi = __umulhi(a, b);
+  *lo = a * b;
+#else
+  const uint64_t p = (uint64_t)a * b;
+  *hi = (uint32_t)(p >> 32);
+  *lo = (uint32_t)p;
+#endif
+}
+PNR_HD void pnr_philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1,
+                              uint32_t out[4]) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    if (i > 0) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    uint32_t hi0, lo0, hi1, lo1;
+    pnr_mulhilo32(0xD2511F53u, c0, &hi0, &lo0);
+    pnr_mulhilo32(0xCD9E8D57u, c2, &hi1, &lo1);
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
+}
+// block `block` of ray r: counter (block, r, step low word, step high word), key = the seed (low word first)
+PNR_HD void pnr_ray_draw(uint64_t seed, uint64_t step, int64_t r, uint32_t block, uint32_t out[4]) {
+  pnr_philox4x32_10(block, (uint32_t)r, (uint32_t)step, (uint32_t)(step >> 32), (uint32_t)seed, (uint32_t)(seed >> 32),
+                    out);
+}
+// high 64 bits of the 128-bit product a * b: a uniform 64-bit a gives an index in [0, b), biased by at most b / 2^64
+PNR_HD uint64_t pnr_mulhi64(uint64_t a, uint64_t b) {
+#if defined(__CUDA_ARCH__)
+  return __umul64hi(a, b);
+#else
+  return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+// a 32-bit word -> [0, 1) on the 2^-24 grid (exact in fp32)
+PNR_HD float pnr_u01(uint32_t w) { return (float)(w >> 8) * 5.9604644775390625e-08f; }
+// frame of flat pixel p: the last f with off[f] <= p (upper bound over off[0..F]), clamped into [0, F)
+PNR_HD int pnr_frame_of(const int64_t* off, int F, int64_t p) {
+  int lo = 0, hi = F + 1;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= p) lo = mid + 1; else hi = mid;
+  }
+  const int f = lo - 1;
+  return f < 0 ? 0 : (f >= F ? F - 1 : f);
+}
+// an 8-bit colour channel -> [0, 1], as torch's u8.float() / 255 on the CPU (true division)
+PNR_HD float pnr_u8_unit(uint8_t b) { return PNR_DIV((float)b, 255.0f); }
+
+// Row r - a.r0 of every output of pnr_sample_ray_batch for the global ray r (off: a.pix_offset or a copy of it).
+PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, int64_t r) {
+  const int64_t row = r - a.r0;
+  uint32_t w[4];
+  pnr_ray_draw(a.seed, a.step, r, 0u, w);
+  const int64_t p = (int64_t)pnr_mulhi64(((uint64_t)w[0] << 32) | w[1], (uint64_t)a.P);
+  const int f = pnr_frame_of(off, a.F, p);
+  int cam = a.frame_cam[f];
+  cam = cam < 0 ? 0 : (cam >= a.num_cameras ? a.num_cameras - 1 : cam);
+  pnr_ray_camera c = a.cams[0];   // selected with constant indices: the table stays in the kernel's parameters
+#pragma unroll
+  for (int k = 1; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k)
+    if (k == cam) c = a.cams[k];
+  const int64_t q = p - off[f];
+  const int v = (int)(q / c.W), u = (int)(q % c.W);
+  float x, y, z;
+  if (c.model == 0)
+    pnr_pinhole_dir((float)u, (float)v, c.intr[0], c.intr[1], c.intr[2], c.intr[3], &x, &y, &z);
+  else
+    pnr_fisheye_dir((float)u, (float)v, c.intr[0], c.intr[1], c.intr[2], c.intr[3], c.intr[4], c.intr[5], c.intr[6],
+                    &x, &y, &z);
+  float m[12];
+#pragma unroll
+  for (int i = 0; i < 12; ++i) m[i] = a.c2w[(int64_t)f * 12 + i];
+  float* o = a.rays + row * 6;
+  o[0] = m[3]; o[1] = m[7]; o[2] = m[11];
+  pnr_cam_to_world(m, x, y, z, o + 3, o + 4, o + 5);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) a.rgb[row * 3 + k] = pnr_u8_unit(a.rgb8[p * 3 + k]);
+  if (a.depth_out) a.depth_out[row] = a.depth ? a.depth[p] : 0.f;
+  if (a.pseudo_label) a.pseudo_label[row] = a.label ? (int32_t)a.label[p] : -1;
+  if (a.pixel) a.pixel[row] = p;
+  const int nw = a.N + a.Ni;
+  for (int k = 0; k < nw; k += 4) {
+    pnr_ray_draw(a.seed, a.step, r, 1u + (uint32_t)(k >> 2), w);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int i = k + j;
+      if (i < a.N) a.u[row * a.N + i] = pnr_u01(w[j]);
+      else if (i < nw) a.u_fine[row * a.Ni + (i - a.N)] = pnr_u01(w[j]);
+    }
+  }
 }

@@ -5,6 +5,8 @@
 //   composite : one warp per ray; lanes stride the sample axis; transmittance is an exclusive
 //               product scan done with warp shuffles; per-class logits are accumulated with lanes
 //               striding the (contiguous) channel axis so every raw row is read once, coalesced.
+//   ray batch : one thread per training ray: a seeded random pixel of a device frame set, its camera ray, targets
+//               and jitter (pnr_ray_batch_row of ray_math.h).
 #include "common.cuh"
 #include "composite_math.cuh"
 #include "ray_math.h"
@@ -68,6 +70,28 @@ __global__ void __launch_bounds__(256) rays_kernel(CamArgs a, float* __restrict_
   o[0] = make_float2(a.c2w[3], a.c2w[7]);
   o[1] = make_float2(a.c2w[11], d0);
   o[2] = make_float2(d1, d2);
+}
+
+// ------------------------------------------------------------------------------------ training ray batches
+// One thread per ray of [r0, r1), grid-strided over a grid of a few blocks per SM; each row is pnr_ray_batch_row
+// (ray_math.h, also compiled for the host by the CPU tests).  With kSmemOff the frame offsets are searched in a
+// shared-memory copy, loaded once per block.
+constexpr int kRayBatchThreads = 256;
+constexpr int kRayBatchSmemOff = 1024;   // F + 1 offsets (8 KB) or fewer: the shared copy
+
+template <bool kSmemOff>
+__global__ void __launch_bounds__(kRayBatchThreads) ray_batch_kernel(const pnr_ray_batch_args a) {
+  extern __shared__ int64_t s_off[];
+  const int64_t* off = a.pix_offset;
+  if (kSmemOff) {
+    for (int i = threadIdx.x; i <= a.F; i += kRayBatchThreads) s_off[i] = a.pix_offset[i];
+    __syncthreads();
+    off = s_off;
+  }
+  const int64_t n = a.r1 - a.r0;
+  for (int64_t i = (int64_t)blockIdx.x * kRayBatchThreads + threadIdx.x; i < n;
+       i += (int64_t)gridDim.x * kRayBatchThreads)
+    pnr_ray_batch_row(a, off, a.r0 + i);
 }
 
 // ------------------------------------------------------------------------------------ a9 composite
@@ -529,6 +553,50 @@ extern "C" int pnr_generate_rays(int32_t H, int32_t W, int32_t row0, int32_t row
   const int64_t n = (int64_t)rows * W;
   rays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a, rays);
   PNR_LAUNCH_CHECK("rays_kernel");
+  return PNR_OK;
+}
+
+extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream) {
+  PNR_CHECK_ARG(args, "pnr_sample_ray_batch: null args");
+  const pnr_ray_batch_args& a = *args;
+  PNR_CHECK_ARG(a.F >= 1 && a.F < INT32_MAX, "pnr_sample_ray_batch: F=%d outside [1, 2^31 - 1)", a.F);
+  PNR_CHECK_ARG(a.P >= 1, "pnr_sample_ray_batch: P=%lld < 1", (long long)a.P);
+  PNR_CHECK_ARG(a.r0 >= 0 && a.r1 >= a.r0 && a.r1 <= (int64_t(1) << 32),
+                "pnr_sample_ray_batch: range r0=%lld r1=%lld is not 0 <= r0 <= r1 <= 2^32", (long long)a.r0,
+                (long long)a.r1);
+  PNR_CHECK_ARG(a.N >= 1 && a.N <= 32 * kCompMaxPerLane, "pnr_sample_ray_batch: N=%d outside [1,%d]", a.N,
+                32 * kCompMaxPerLane);
+  PNR_CHECK_ARG(a.Ni >= 0 && a.Ni <= 32 * kCompMaxPerLane - a.N, "pnr_sample_ray_batch: Ni=%d outside [0,%d] (N + Ni <= %d)",
+                a.Ni, 32 * kCompMaxPerLane - a.N, 32 * kCompMaxPerLane);
+  PNR_CHECK_ARG(a.num_cameras >= 1 && a.num_cameras <= PNR_RAY_BATCH_MAX_CAMERAS,
+                "pnr_sample_ray_batch: num_cameras=%d outside [1,%d]", a.num_cameras, PNR_RAY_BATCH_MAX_CAMERAS);
+  for (int k = 0; k < a.num_cameras; ++k) {
+    const pnr_ray_camera& c = a.cams[k];
+    if (c.model == 1)
+      return set_error(PNR_ERR_ARG, "pnr_sample_ray_batch: camera %d is equirect (model 1): its rays are device-only "
+                       "(sincosf), so batches take pinhole (0) and fisheye (2) cameras", k);
+    PNR_CHECK_ARG(c.model == 0 || c.model == 2, "pnr_sample_ray_batch: camera %d model %d (0 pinhole, 2 fisheye)", k,
+                  c.model);
+    PNR_CHECK_ARG(c.H >= 1 && c.W >= 1, "pnr_sample_ray_batch: camera %d size H=%d W=%d < 1", k, c.H, c.W);
+  }
+  PNR_CHECK_ARG(a.c2w && a.frame_cam && a.pix_offset && a.rgb8,
+                "pnr_sample_ray_batch: null frame-set pointer (c2w, frame_cam, pix_offset and rgb8 are required)");
+  PNR_CHECK_ARG(a.rays && a.rgb && a.u, "pnr_sample_ray_batch: null output pointer (rays, rgb and u are required)");
+  PNR_CHECK_ARG(a.Ni == 0 || a.u_fine, "pnr_sample_ray_batch: null output pointer u_fine with Ni=%d", a.Ni);
+  const int64_t n = a.r1 - a.r0;
+  if (n == 0) return PNR_OK;
+  int dev = 0;
+  int rc = current_device("pnr_sample_ray_batch", &dev);
+  if (rc != PNR_OK) return rc;
+  const int64_t want = (n + kRayBatchThreads - 1) / kRayBatchThreads, cap = (int64_t)num_sms(dev) * 8;
+  const int64_t blocks = want < cap ? want : cap;
+  if (a.F + 1 <= kRayBatchSmemOff) {
+    ray_batch_kernel<true><<<(unsigned)blocks, kRayBatchThreads, (size_t)(a.F + 1) * sizeof(int64_t),
+                             (cudaStream_t)stream>>>(a);
+  } else {
+    ray_batch_kernel<false><<<(unsigned)blocks, kRayBatchThreads, 0, (cudaStream_t)stream>>>(a);
+  }
+  PNR_LAUNCH_CHECK("ray_batch_kernel");
   return PNR_OK;
 }
 

@@ -1,0 +1,121 @@
+"""KITTI-360 frames of one camera -> a device FrameSet (lib/datasets/ray_batch.py) for training-batch sampling.
+
+Layout under `root` (public KITTI-360 layout):
+  data_2d_raw/<seq>/image_00/data_rect/<frame:010d>.png     rectified perspective camera, 8-bit colour
+  data_2d_raw/<seq>/image_02|03/data_rgb/<frame:010d>.png   fisheye cameras, 8-bit colour
+  calibration/perspective.txt (P_rect_00, S_rect_00), calibration/image_02.yaml / image_03.yaml,
+  calibration/calib_cam_to_pose.txt, data_poses/<seq>/cam0_to_world.txt, data_poses/<seq>/poses.txt
+Poses: image_00 -> cam0_to_world[frame]; image_02 / image_03 -> poses.txt[frame] @ calib_cam_to_pose[camera].
+
+Targets (rules chosen here, one format per kind; the reference's preprocessing is not in the mount):
+  <pseudo_dir>/<frame:010d>.png   8-bit single channel, KITTI-360 semanticIds, mapped to class channels through
+                                  sem_to_train as primitive_batch maps box ids (an id without a channel -> -1; no
+                                  table: the id itself)
+  <depth_dir>/<frame:010d>.png    16-bit single channel, metres x 256, 0 = no depth (the KITTI depth encoding)
+A missing file, a wrong bit depth or channel count and an image whose size is not its camera's calibration are refused
+by name."""
+from __future__ import annotations
+
+from pathlib import Path
+from typing import Dict, Iterable, Optional
+
+import numpy as np
+import torch
+
+from ..ray_batch import Camera, FrameSet
+from .calib import (fisheye_to_world, load_cam0_to_world, load_cam_to_pose, load_fisheye_yaml, load_perspective,
+                    load_poses)
+
+CAMERAS = ("image_00", "image_02", "image_03")
+
+
+def _read(path: Path, what: str, dtype, channels: int) -> np.ndarray:
+    import cv2
+    if not path.is_file():
+        raise FileNotFoundError(f"{path}: missing {what}")
+    img = cv2.imread(str(path), cv2.IMREAD_UNCHANGED)
+    if img is None:
+        raise ValueError(f"{path}: not a readable image ({what})")
+    got = 1 if img.ndim == 2 else img.shape[2]
+    if got != channels:
+        raise ValueError(f"{path}: {what} must have {channels} channel(s), got {got}")
+    if img.dtype != dtype:
+        raise ValueError(f"{path}: {what} must be {np.dtype(dtype).itemsize * 8}-bit, got {img.dtype}")
+    return img
+
+
+def _sized(img: np.ndarray, cam: Camera, path: Path, what: str) -> np.ndarray:
+    if img.shape[:2] != (cam.H, cam.W):
+        raise ValueError(f"{path}: {what} is {img.shape[1]} x {img.shape[0]}, its camera's calibration says "
+                         f"{cam.W} x {cam.H}")
+    return img
+
+
+def camera_of(root, camera: str) -> Camera:
+    """The calibrated camera of `camera` (image_00: P_rect_00 and S_rect_00; image_02 / 03: the MEI yaml)."""
+    cal = Path(root) / "calibration"
+    if camera == "image_00":
+        p = load_perspective(cal / "perspective.txt", 0)
+        if p["size"] is None:
+            raise ValueError(f"{cal / 'perspective.txt'}: no S_rect_00 (the image size)")
+        K = p["K"]
+        return Camera("pinhole", p["size"][1], p["size"][0], (K[0, 0], K[1, 1], K[0, 2], K[1, 2]))
+    fe = load_fisheye_yaml(cal / f"{camera}.yaml")
+    if "image_width" not in fe or "image_height" not in fe:
+        raise ValueError(f"{cal / (camera + '.yaml')}: no image_width / image_height")
+    return Camera("fisheye", int(fe["image_height"]), int(fe["image_width"]),
+                  tuple(fe[k] for k in ("gamma1", "gamma2", "u0", "v0", "xi", "k1", "k2")))
+
+
+def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00", pseudo_dir=None, depth_dir=None,
+                sem_to_train: Optional[Dict[int, int]] = None, device="cuda") -> FrameSet:
+    """The frames `frames` of sequence `seq` seen by `camera`, on `device` (module docstring: layout and formats)."""
+    if camera not in CAMERAS:
+        raise ValueError(f"load_frames: camera {camera!r}; one of {CAMERAS}")
+    root = Path(root)
+    frames = [int(f) for f in frames]
+    if not frames:
+        raise ValueError("load_frames: no frames")
+    cam = camera_of(root, camera)
+    poses = root / "data_poses" / seq
+    if camera == "image_00":
+        table = load_cam0_to_world(poses / "cam0_to_world.txt")
+        pose_of = lambda f: table[f]
+        src = poses / "cam0_to_world.txt"
+    else:
+        imu = load_poses(poses / "poses.txt")
+        c2p = load_cam_to_pose(root / "calibration" / "calib_cam_to_pose.txt")
+        if camera not in c2p:
+            raise ValueError(f"{root / 'calibration' / 'calib_cam_to_pose.txt'}: no {camera}")
+        pose_of = lambda f: fisheye_to_world(c2p[camera], imu[f])
+        src = poses / "poses.txt"
+    images = root / "data_2d_raw" / seq / camera / ("data_rect" if camera == "image_00" else "data_rgb")
+    lut = None
+    if sem_to_train is not None:
+        lut = np.full(256, -1, dtype=np.int16)
+        for k, v in sem_to_train.items():
+            if 0 <= int(k) < 256:
+                lut[int(k)] = int(v)
+    c2w, rgb, lab, dep = [], [], [], []
+    for f in frames:
+        try:
+            c2w.append(np.asarray(pose_of(f), dtype=np.float64)[:3, :4])
+        except KeyError:
+            raise ValueError(f"{src}: no pose for frame {f}") from None
+        name = f"{f:010d}.png"
+        bgr = _sized(_read(images / name, "a colour image", np.uint8, 3), cam, images / name, "the colour image")
+        rgb.append(torch.from_numpy(np.ascontiguousarray(bgr[:, :, ::-1])))
+        if pseudo_dir is not None:
+            p = Path(pseudo_dir) / name
+            ids = _sized(_read(p, "a pseudo-label image", np.uint8, 1), cam, p, "the pseudo-label image")
+            lab.append(torch.from_numpy(lut[ids] if lut is not None else ids.astype(np.int16)))
+        if depth_dir is not None:
+            p = Path(depth_dir) / name
+            d = _sized(_read(p, "a depth image", np.uint16, 1), cam, p, "the depth image")
+            dep.append(torch.from_numpy(d.astype(np.float32) / np.float32(256.0)))
+    return FrameSet.from_images([cam], [0] * len(frames), np.stack(c2w).astype(np.float32), rgb,
+                                lab if pseudo_dir is not None else None, dep if depth_dir is not None else None,
+                                [(camera, f) for f in frames], device)
+
+
+__all__ = ["CAMERAS", "camera_of", "load_frames"]

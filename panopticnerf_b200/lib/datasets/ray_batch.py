@@ -1,0 +1,204 @@
+"""Training batches drawn on the device from frames kept there (DESIGN 3.4).
+
+FrameSet: the images of a sequence, resident on the GPU as one flat pixel table (rgb8 [P,3] u8, optional label [P] i16
+and depth [P] f32) with per-frame poses, cameras and pixel offsets: what `pnr_sample_ray_batch` reads.
+`kitti360.load_frames` builds one from a KITTI-360 sequence; `concat_frame_sets` joins sets of different cameras.
+
+RaySampler(frames, seed).batch(step, R, N, Ni): one launch of `pnr_sample_ray_batch` -> the dict NetworkWrapper /
+DataParallelWrapper take (rays, rgb, u, u_fine, depth and pseudo_label when the set has them, plus the scene block given
+at construction).  Every row is a function of (seed, step, ray index) alone, so every data-parallel rank that calls
+batch(step, R, ...) with the same seed holds the same global batch, with no exchange."""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass, field
+from typing import Dict, List, Optional, Sequence, Tuple
+
+import torch
+
+from ... import _capi
+
+CAMERA_MODEL = {"pinhole": 0, "fisheye": 2}   # the equirect camera (1) has device-only rays: not a batch camera
+MAX_SAMPLES_PER_RAY = 256                     # N + Ni, as render_train accepts
+
+
+@dataclass
+class Camera:
+    """model 'pinhole' (intr fx, fy, cx, cy) or 'fisheye' (gamma1, gamma2, u0, v0, xi, k1, k2); H x W pixels."""
+    model: str
+    H: int
+    W: int
+    intr: Tuple[float, ...]
+
+    def __post_init__(self):
+        if self.model not in CAMERA_MODEL:
+            raise ValueError(f"Camera: model {self.model!r}; a ray batch takes {sorted(CAMERA_MODEL)} cameras "
+                             "(equirect rays are device-only)")
+        want = 4 if self.model == "pinhole" else 7
+        self.intr = tuple(float(x) for x in self.intr)
+        if len(self.intr) != want:
+            raise ValueError(f"Camera: a {self.model} camera takes {want} intrinsics, got {len(self.intr)}")
+        if int(self.H) < 1 or int(self.W) < 1:
+            raise ValueError(f"Camera: size {self.H} x {self.W}")
+        self.H, self.W = int(self.H), int(self.W)
+
+
+@dataclass
+class FrameSet:
+    """Device buffers of F frames.  Frame f: camera cameras[frame_cam[f]], pose c2w[f] (row-major 3x4 camera -> world),
+    pixels [pix_offset[f], pix_offset[f+1]) of the flat tables, row-major over (v, u).  label: -1 = ignore; depth:
+    metres, <= 0 = none.  names: one (camera name, frame id) per frame."""
+    cameras: List[Camera]
+    c2w: torch.Tensor          # [F, 12] f32
+    frame_cam: torch.Tensor    # [F] i32
+    pix_offset: torch.Tensor   # [F + 1] i64
+    rgb8: torch.Tensor         # [P, 3] u8
+    label: Optional[torch.Tensor] = None   # [P] i16
+    depth: Optional[torch.Tensor] = None   # [P] f32
+    names: List[Tuple[str, int]] = field(default_factory=list)
+
+    @property
+    def num_frames(self) -> int:
+        return int(self.c2w.shape[0])
+
+    @property
+    def num_pixels(self) -> int:
+        return int(self.rgb8.shape[0])
+
+    @staticmethod
+    def from_images(cameras: Sequence[Camera], frame_cam: Sequence[int], c2w, rgb8: Sequence[torch.Tensor],
+                    label: Optional[Sequence[torch.Tensor]] = None, depth: Optional[Sequence[torch.Tensor]] = None,
+                    names: Optional[Sequence[Tuple[str, int]]] = None, device="cuda") -> "FrameSet":
+        """A set from per-frame images: rgb8[f] [H, W, 3] u8, label[f] [H, W] i16, depth[f] [H, W] f32 (each list None
+        or one per frame), every image of its camera's size; c2w [F, 3, 4] or [F, 12]."""
+        cams = list(cameras)
+        if not 1 <= len(cams) <= _capi.RAY_BATCH_MAX_CAMERAS:
+            raise ValueError(f"FrameSet: {len(cams)} cameras; a set holds 1..{_capi.RAY_BATCH_MAX_CAMERAS}")
+        F = len(rgb8)
+        fc = [int(c) for c in frame_cam]
+        if F < 1 or len(fc) != F:
+            raise ValueError(f"FrameSet: {F} images for {len(fc)} frame cameras")
+        for k, name in ((label, "label"), (depth, "depth")):
+            if k is not None and len(k) != F:
+                raise ValueError(f"FrameSet: {len(k)} {name} images for {F} frames")
+        off = [0]
+        for f in range(F):
+            if not 0 <= fc[f] < len(cams):
+                raise ValueError(f"FrameSet: frame {f} has camera {fc[f]} outside [0, {len(cams)})")
+            cam = cams[fc[f]]
+            want = (cam.H, cam.W)
+            checks = [("rgb", rgb8[f], want + (3,), torch.uint8)]
+            if label is not None:
+                checks.append(("label", label[f], want, torch.int16))
+            if depth is not None:
+                checks.append(("depth", depth[f], want, torch.float32))
+            for what, t, shape, dt in checks:
+                if tuple(t.shape) != shape or t.dtype != dt:
+                    raise ValueError(f"FrameSet: frame {f} {what} is {tuple(t.shape)} {t.dtype}, its camera wants "
+                                     f"{shape} {dt}")
+            off.append(off[-1] + cam.H * cam.W)
+        flat = lambda ts, *tail: torch.cat([t.reshape(-1, *tail) for t in ts]).to(device).contiguous()
+        c2w = torch.as_tensor(c2w, dtype=torch.float32).reshape(F, -1)
+        if c2w.shape[1] != 12:
+            raise ValueError(f"FrameSet: c2w has {c2w.shape[1]} values per frame, expected 12 (3x4)")
+        return FrameSet(cams, c2w.to(device).contiguous(), torch.tensor(fc, dtype=torch.int32, device=device),
+                        torch.tensor(off, dtype=torch.int64, device=device), flat(rgb8, 3),
+                        flat(label) if label is not None else None, flat(depth) if depth is not None else None,
+                        list(names) if names is not None else [])
+
+
+def concat_frame_sets(*sets: FrameSet) -> FrameSet:
+    """One set of the frames of several (e.g. the perspective and the fisheye cameras of a sequence), in order.  Equal
+    cameras are merged; a label or depth table that only some sets have is filled with -1 / 0 (none) for the others."""
+    if not sets:
+        raise ValueError("concat_frame_sets: no sets")
+    cams: List[Camera] = []
+    fcs, offs, base = [], [sets[0].pix_offset[:1]], 0
+    for s in sets:
+        remap = []
+        for c in s.cameras:
+            if c not in cams:
+                cams.append(c)
+            remap.append(cams.index(c))
+        fcs.append(torch.tensor(remap, dtype=torch.int32, device=s.frame_cam.device)[s.frame_cam.long()])
+        offs.append(s.pix_offset[1:] + base)
+        base += s.num_pixels
+    if len(cams) > _capi.RAY_BATCH_MAX_CAMERAS:
+        raise ValueError(f"concat_frame_sets: {len(cams)} distinct cameras; a set holds at most "
+                         f"{_capi.RAY_BATCH_MAX_CAMERAS}")
+
+    def table(key, fill, dtype):
+        if all(getattr(s, key) is None for s in sets):
+            return None
+        return torch.cat([getattr(s, key) if getattr(s, key) is not None else
+                          torch.full((s.num_pixels,), fill, dtype=dtype, device=s.rgb8.device) for s in sets])
+    return FrameSet(cams, torch.cat([s.c2w for s in sets]), torch.cat(fcs), torch.cat(offs),
+                    torch.cat([s.rgb8 for s in sets]), table("label", -1, torch.int16),
+                    table("depth", 0.0, torch.float32), [n for s in sets for n in s.names])
+
+
+def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N: int, Ni: int = 0,
+                     want_pixel: bool = False) -> Dict[str, torch.Tensor]:
+    """Rays r0 .. r1-1 of the batch (seed, step): one pnr_sample_ray_batch launch on the frames' device.  Returns
+    rays [n,6], rgb [n,3], u [n,N], u_fine [n,Ni] (Ni > 0), depth [n] / pseudo_label [n] i32 when the set has a depth /
+    label table, and pixel [n] i64 (the flat pixel index) when asked."""
+    if not (0 <= int(seed) < 1 << 64 and 0 <= int(step) < 1 << 64):
+        raise ValueError(f"sample_ray_batch: seed {seed} and step {step} must be in [0, 2^64)")
+    dev = frames.rgb8.device
+    n = int(r1) - int(r0)
+    e = lambda *shape, dtype=torch.float32: torch.empty(*shape, dtype=dtype, device=dev)
+    out = {"rays": e(max(n, 0), 6), "rgb": e(max(n, 0), 3), "u": e(max(n, 0), int(N))}
+    if int(Ni) > 0:
+        out["u_fine"] = e(max(n, 0), int(Ni))
+    if frames.depth is not None:
+        out["depth"] = e(max(n, 0))
+    if frames.label is not None:
+        out["pseudo_label"] = e(max(n, 0), dtype=torch.int32)
+    if want_pixel:
+        out["pixel"] = e(max(n, 0), dtype=torch.int64)
+    a = _capi.PnrRayBatchArgs()
+    a.c2w = _capi.ptr(frames.c2w, torch.float32, "c2w")
+    a.frame_cam = _capi.ptr(frames.frame_cam, torch.int32, "frame_cam")
+    a.pix_offset = _capi.ptr(frames.pix_offset, torch.int64, "pix_offset")
+    a.F, a.P = frames.num_frames, frames.num_pixels
+    a.rgb8 = _capi.ptr(frames.rgb8, torch.uint8, "rgb8")
+    a.label = _capi.ptr(frames.label, torch.int16, "label")
+    a.depth = _capi.ptr(frames.depth, torch.float32, "depth")
+    if len(frames.cameras) > _capi.RAY_BATCH_MAX_CAMERAS:
+        raise ValueError(f"sample_ray_batch: {len(frames.cameras)} cameras > {_capi.RAY_BATCH_MAX_CAMERAS}")
+    for k, cam in enumerate(frames.cameras):
+        a.cams[k].model, a.cams[k].H, a.cams[k].W = CAMERA_MODEL[cam.model], cam.H, cam.W
+        for i, x in enumerate(cam.intr):
+            a.cams[k].intr[i] = x
+    a.num_cameras = len(frames.cameras)
+    a.seed, a.step, a.r0, a.r1, a.N, a.Ni = int(seed), int(step), int(r0), int(r1), int(N), int(Ni)
+    a.rays, a.rgb, a.u = _capi.ptr(out["rays"]), _capi.ptr(out["rgb"]), _capi.ptr(out["u"])
+    a.u_fine = _capi.ptr(out.get("u_fine"))
+    a.depth_out, a.pseudo_label = _capi.ptr(out.get("depth")), _capi.ptr(out.get("pseudo_label"))
+    a.pixel = _capi.ptr(out.get("pixel"))
+    with torch.cuda.device(dev):
+        _capi.check(_capi.lib().pnr_sample_ray_batch(C.byref(a), _capi.stream_ptr()), "pnr_sample_ray_batch")
+    return out
+
+
+class RaySampler:
+    """RaySampler(frames, seed, scene).batch(step, R, N, Ni) -> a training batch of R random pixels of the frame set.
+    `scene`: the replicated block every batch carries (the static primitive table of `kitti360.primitive_batch`, a
+    mesh table, scene_aabb, ...).  One table serves rays of every frame, so it holds the static annotations
+    (boxes_to_primitives(frame=None)); per-frame dynamic boxes are not part of a sampled batch."""
+
+    def __init__(self, frames: FrameSet, seed: int, scene: Optional[Dict[str, torch.Tensor]] = None):
+        self.frames, self.seed = frames, int(seed)
+        self.scene = dict(scene or {})
+        clash = set(self.scene) & {"rays", "rgb", "u", "u_fine", "depth", "pseudo_label"}
+        if clash:
+            raise ValueError(f"RaySampler: the scene block may not carry the per-ray keys {sorted(clash)}")
+
+    def batch(self, step: int, R: int, N: int, Ni: int = 0) -> Dict[str, torch.Tensor]:
+        """The global batch of `step`: rays 0 .. R-1, identical on every rank that uses the same seed."""
+        out = sample_ray_batch(self.frames, self.seed, step, 0, R, N, Ni)
+        out.update(self.scene)
+        return out
+
+
+__all__ = ["Camera", "FrameSet", "concat_frame_sets", "sample_ray_batch", "RaySampler"]
