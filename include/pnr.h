@@ -123,6 +123,39 @@ int pnr_intersect_meshes(const float* rays, int64_t R, const float* box_center, 
                          int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
                          void* stream);
 
+/* a5 with a sequence table (DESIGN 3.2): one primitive table for the rays of many frames.  Primitives [0, S) are
+ * static; frame f owns the dynamic block frame_boxes [F,2] i32 row f = (begin, end), S <= begin <= end <= B (blocks may
+ * be shared, e.g. by the cameras of one timestamp).  Ray r is intersected with [0, S) and then with the block of its
+ * frame ray_frame [R] i32, in that order, so its outputs equal, bit for bit, those of pnr_intersect_meshes on the table
+ * cat(static, block) with the block's ids shifted by begin - S.  Box ids index the whole table (box_sem, box_inst and
+ * mesh_tri_start index it unchanged).  A block entry is clamped into [S, B] (end < begin: empty); a ray_frame outside
+ * [0, F) meets the static primitives only.  F = 0 is no frame table: ray_frame and frame_boxes NULL and S = 0, every
+ * primitive static (the bytes of pnr_intersect_meshes).  Refused before any launch (PNR_ERR_ARG, by name): F < 0, a
+ * null ray_frame or frame_boxes with F >= 1, either set or S != 0 with F = 0, S outside [0, B]; and whatever
+ * pnr_intersect_meshes refuses. */
+typedef struct pnr_frame_table {
+  const int32_t* ray_frame;     /* [R] frame of each ray                                                          */
+  const int32_t* frame_boxes;   /* [F,2] (begin, end) of each frame's dynamic block                               */
+  int32_t F, S;                 /* frames, static primitives                                                      */
+} pnr_frame_table;
+typedef struct pnr_intersect_frames_args {
+  const float* rays;            /* [R,6]                                                                          */
+  int64_t R;
+  const float* box_center;      /* [B,3] the sequence table                                                       */
+  const float* box_half;        /* [B,3]                                                                          */
+  const float* box_rot;         /* [B,3,3]                                                                        */
+  int32_t B, M;
+  const int32_t* mesh_tri_start;  /* [B+1] or NULL with T = 0, as pnr_intersect_meshes                            */
+  const float* mesh_tris;       /* [T,3,3]                                                                        */
+  int64_t T;
+  pnr_frame_table frames;
+  uint8_t* hit_mask;            /* [R]                                                                            */
+  int32_t* box_id;              /* [R,M]                                                                          */
+  float* t_in;                  /* [R,M]                                                                          */
+  float* t_out;                 /* [R,M]                                                                          */
+} pnr_intersect_frames_args;
+int pnr_intersect_frames(const pnr_intersect_frames_args* args, void* stream);
+
 /* a5 (AABB special case): per-ray near = max(tmin, near_min), far = tmax, or
  * (near_min, far_default) when the scene box is missed.  aabb_host = {lo.xyz, hi.xyz}. */
 int pnr_scene_near_far(const float* rays, int64_t R, const float* aabb_host, float near_min,
@@ -182,7 +215,7 @@ int pnr_generate_rays(int32_t H, int32_t W, int32_t row0, int32_t rows, int32_t 
  * 0 .. r1-r0-1, equal bit for bit to the matching rows of [0, R).
  * Outputs [r1 - r0, ...]: rays [., 6] (row v*W + u of pnr_generate_rays for that frame, bit for bit), rgb [., 3] =
  * byte / 255 (true division), u [., N], u_fine [., Ni] (needed when Ni > 0); nullable: depth_out [.] (0 without a depth
- * table), pseudo_label [.] i32 (-1 without a label table), pixel [.] i64 (the flat index p).
+ * table), pseudo_label [.] i32 (-1 without a label table), pixel [.] i64 (the flat index p), frame [.] i32 (f).
  * Refused before any launch (PNR_ERR_ARG, by name): F < 1 or >= 2^31 - 1, P < 1, r0 < 0, r1 < r0, r1 > 2^32, N outside
  * [1, 256], Ni < 0 or N + Ni > 256, num_cameras outside [1, PNR_RAY_BATCH_MAX_CAMERAS], a camera model other than 0 / 2
  * or H, W < 1, a null frame-set or required output pointer. */
@@ -212,6 +245,8 @@ typedef struct pnr_ray_batch_args {
   float* u;
   float* u_fine;
   int64_t* pixel;
+  int32_t* frame;               /* [.] i32 the frame f of the pixel, nullable (the index pnr_frame_table's
+                                   ray_frame takes when the frames map one to one onto frame_boxes)          */
 } pnr_ray_batch_args;
 int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream);
 
@@ -490,6 +525,12 @@ typedef struct pnr_render_args {
 /* ctx_fine: the network of the fine pass (NULL = ctx), with the same num_classes and num_instances as ctx
  * (PNR_ERR_ARG otherwise: the maps are [R,C] / [R,K] of ctx). */
 int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* args, void* stream);
+/* pnr_render_fused on a sequence table: `frames` (nullable; NULL or F = 0 is pnr_render_fused) gives each ray's frame
+ * (ray_frame [R], offset with the ray chunks) and the table's frame blocks, and the intersection is
+ * pnr_intersect_frames'.  Refused as there, and F >= 1 without primitives (B = 0).  pnr_render_args keeps its layout,
+ * so callers built against it are unchanged. */
+int pnr_render_fused_frames(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* args, const pnr_frame_table* frames,
+                            void* stream);
 
 /* Bytes of device scratch pnr_render_fused wants for R rays: enough for one chunk of min(R, rays_per_chunk) rays
  * with every optional output absent, where rays_per_chunk puts `raw` near 1.5 GB and never below ~64 tiles of the

@@ -76,6 +76,19 @@ class PnrRenderArgs(C.Structure):
                 ("mesh_tri_start", C.c_void_p), ("mesh_tris", C.c_void_p), ("T", C.c_int64)]
 
 
+class PnrFrameTable(C.Structure):
+    """pnr_frame_table of include/pnr.h: the frame fields of a sequence table (all zero: none)."""
+    _fields_ = [("ray_frame", C.c_void_p), ("frame_boxes", C.c_void_p), ("F", C.c_int32), ("S", C.c_int32)]
+
+
+class PnrIntersectFramesArgs(C.Structure):
+    """pnr_intersect_frames_args of include/pnr.h (same field order)."""
+    _fields_ = [("rays", C.c_void_p), ("R", C.c_int64), ("box_center", C.c_void_p), ("box_half", C.c_void_p),
+                ("box_rot", C.c_void_p), ("B", C.c_int32), ("M", C.c_int32), ("mesh_tri_start", C.c_void_p),
+                ("mesh_tris", C.c_void_p), ("T", C.c_int64), ("frames", PnrFrameTable), ("hit_mask", C.c_void_p),
+                ("box_id", C.c_void_p), ("t_in", C.c_void_p), ("t_out", C.c_void_p)]
+
+
 class PnrAdamArgs(C.Structure):
     """pnr_adam_args of include/pnr.h."""
     _fields_ = [("P", C.c_int64), ("ld_grad", C.c_int64), ("G", C.c_int32), ("beta1", C.c_double),
@@ -98,7 +111,7 @@ class PnrRayBatchArgs(C.Structure):
                 ("cams", PnrRayCamera * RAY_BATCH_MAX_CAMERAS), ("num_cameras", C.c_int32),
                 ("seed", C.c_uint64), ("step", C.c_uint64), ("r0", C.c_int64), ("r1", C.c_int64),
                 ("N", C.c_int32), ("Ni", C.c_int32)] + \
-               [(k, C.c_void_p) for k in ("rays", "rgb", "depth_out", "pseudo_label", "u", "u_fine", "pixel")]
+               [(k, C.c_void_p) for k in ("rays", "rgb", "depth_out", "pseudo_label", "u", "u_fine", "pixel", "frame")]
 
 
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
@@ -116,6 +129,7 @@ SIGNATURES = {
     "pnr_load_weights": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32]),
     "pnr_intersect": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "pnr_intersect_meshes": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "pnr_intersect_frames": (C.c_int, [C.POINTER(PnrIntersectFramesArgs), _vp]),
     "pnr_scene_near_far": (C.c_int, [_vp, _i64, C.POINTER(_f32), _f32, _f32, _vp, _vp, _vp]),
     "pnr_bound_by_primitives": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "pnr_sample_stratified": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _f32, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
@@ -148,6 +162,7 @@ SIGNATURES = {
                                    C.POINTER(C.c_size_t), _vp, C.c_size_t, C.POINTER(C.c_size_t), _vp, C.c_size_t,
                                    C.POINTER(C.c_size_t)]),
     "pnr_render_fused": (C.c_int, [_vp, _vp, C.POINTER(PnrRenderArgs), _vp]),
+    "pnr_render_fused_frames": (C.c_int, [_vp, _vp, C.POINTER(PnrRenderArgs), C.POINTER(PnrFrameTable), _vp]),
     "pnr_workspace_bytes": (C.c_size_t, [_vp, _i64, _i32, _i32]),
     "pnr_comm_available": (C.c_int, []),
     "pnr_comm_unique_id": (C.c_int, [C.POINTER(C.c_uint8)]),

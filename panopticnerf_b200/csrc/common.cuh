@@ -19,6 +19,9 @@ int launch_fixed_maps(const float* weights, const int32_t* sample_box, const int
 // pnr_sample_pdf with an explicit row stride for u (ray_kernels.cu; used by pnr_render_fused)
 int sample_pdf_strided(const float* z, const float* weights, int64_t R, int32_t N, int32_t Ni, const float* u,
                        int64_t u_stride, float* z_fine, int64_t* idx, float* z_all, void* stream);
+// the host checks of a sequence table's frame fields against B primitives (ray_kernels.cu; pnr_intersect_frames and
+// pnr_render_fused_frames name themselves with fn)
+int check_frame_table(const char* fn, const pnr_frame_table* fr, int32_t B);
 
 #define PNR_CHECK_ARG(cond, ...) \
   do { if (!(cond)) return ::pnr::set_error(PNR_ERR_ARG, __VA_ARGS__); } while (0)

@@ -15,7 +15,13 @@ constexpr int kBoxChunk = 512;  // boxes staged per shared-memory fill (15 float
 // [tri_start[b], tri_start[b+1]) is not empty is the cull volume of a closed mesh (ray_math.h: pnr_tri_cross,
 // PnrMeshCross); on a cull hit its triangles are read from global memory (the same rows for the whole warp, so
 // L1/L2-resident broadcasts).  Every range is clamped into [0, T], so a malformed start table cannot read outside tris.
-template <bool kMeshes>
+//
+// kFrames = true: a sequence table (DESIGN 3.2, pnr_intersect_frames).  B is then the static count S, staged as
+// above; after the static chunks each thread walks its own frame's block [begin, end) of the table's Bt primitives
+// with the same per-primitive step, reading the boxes from global memory (a block is a few dozen boxes, L2-resident,
+// and warp-uniform when the rays of a warp share a frame).  The static-only instantiations (kFrames = false) never
+// read the frame parameters, which follow all others, so their SASS is that of the kernel without them.
+template <bool kMeshes, bool kFrames>
 __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict__ rays, int64_t R,
                                                         const float* __restrict__ bc,
                                                         const float* __restrict__ bh,
@@ -25,7 +31,9 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
                                                         float* __restrict__ t_in,
                                                         float* __restrict__ t_out,
                                                         const int32_t* __restrict__ tri_start,
-                                                        const float* __restrict__ tris, int64_t T) {
+                                                        const float* __restrict__ tris, int64_t T,
+                                                        const int32_t* __restrict__ ray_frame,
+                                                        const int32_t* __restrict__ frame_boxes, int F, int Bt) {
   constexpr int kS = kMeshes ? 17 : 15;   // floats per staged box: center, half, rot (+ the triangle range)
   __shared__ float sb[kBoxChunk * kS];
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -78,6 +86,37 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
         } else if (hit) {
           pnr_hits_insert(&L, M, tmin, tmax, b0 + b);
         }
+      }
+    }
+  }
+  if (kFrames && r < R) {
+    int b0, b1;
+    pnr_frame_range(ray_frame[r], frame_boxes, F, B, Bt, &b0, &b1);
+    // the per-primitive step of the static chunks, on a box read from global memory
+    for (int b = b0; b < b1; ++b) {
+      float q[15];
+#pragma unroll
+      for (int e = 0; e < 3; ++e) { q[e] = __ldg(bc + (int64_t)b * 3 + e); q[3 + e] = __ldg(bh + (int64_t)b * 3 + e); }
+#pragma unroll
+      for (int e = 0; e < 9; ++e) q[6 + e] = __ldg(br + (int64_t)b * 9 + e);
+      float tmin, tmax;
+      const bool hit = pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax);
+      int k0 = 0, k1 = 0;
+      if (kMeshes) pnr_tri_range(tri_start, b, T, &k0, &k1);
+      if (k0 == k1) {
+        if (hit) pnr_hits_insert(&L, M, tmin, tmax, b);
+      } else if (hit) {
+        const PnrShear S = pnr_shear(dx, dy, dz);
+        PnrMeshCross X;
+        pnr_cross_init(&X);
+        for (int k = k0; k < k1; ++k) {
+          float v[9];
+#pragma unroll
+          for (int e = 0; e < 9; ++e) v[e] = __ldg(tris + (int64_t)k * 9 + e);
+          float t;
+          if (pnr_tri_cross(ox, oy, oz, S, v, &t)) pnr_cross_add(&X, M, t);
+        }
+        pnr_cross_emit(&X, &L, M, b);
       }
     }
   }
@@ -338,10 +377,26 @@ using namespace pnr;
 
 static inline unsigned blocks_for(int64_t n, int per) { return (unsigned)((n + per - 1) / per); }
 
-// fn: the entry point's name in the error messages
+int pnr::check_frame_table(const char* fn, const pnr_frame_table* fr, int32_t B) {
+  PNR_CHECK_ARG(fr->F >= 0, "%s: F=%d < 0", fn, fr->F);
+  if (fr->F == 0) {
+    PNR_CHECK_ARG(!fr->ray_frame && !fr->frame_boxes && fr->S == 0,
+                  "%s: F=0 (no frame table) needs ray_frame and frame_boxes null and S=0, got ray_frame (%s), "
+                  "frame_boxes (%s), S=%d", fn, fr->ray_frame ? "set" : "null", fr->frame_boxes ? "set" : "null", fr->S);
+    return PNR_OK;
+  }
+  PNR_CHECK_ARG(fr->ray_frame && fr->frame_boxes, "%s: F=%d needs ray_frame (%s) and frame_boxes (%s)", fn, fr->F,
+                fr->ray_frame ? "set" : "null", fr->frame_boxes ? "set" : "null");
+  PNR_CHECK_ARG(fr->S >= 0 && fr->S <= B, "%s: S=%d outside [0, B=%d]", fn, fr->S, B);
+  return PNR_OK;
+}
+
+// fn: the entry point's name in the error messages.  fr: the sequence table's frame fields, or null (every primitive
+// static).
 static int intersect_rays(const char* fn, const float* rays, int64_t R, const float* box_center, const float* box_half,
                      const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T, int32_t B,
-                     int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out, void* stream) {
+                     int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
+                     const pnr_frame_table* fr, void* stream) {
   if (R == 0) return PNR_OK;  // empty input: nothing to do (pointers of empty tensors may be null)
   PNR_CHECK_ARG(R >= 0 && B >= 0, "%s: R=%lld or B=%d < 0", fn, (long long)R, B);
   PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "%s: M=%d outside [1,%d]", fn, M, PNR_MAX_HITS);
@@ -351,12 +406,28 @@ static int intersect_rays(const char* fn, const float* rays, int64_t R, const fl
   PNR_CHECK_ARG(!meshes || (mesh_tri_start && mesh_tris && T >= 1 && T < (int64_t(1) << 31)),
                 "%s: mesh_tri_start (%s), mesh_tris (%s) and T=%lld: both pointers null with T == 0, or both set "
                 "with 1 <= T < 2^31", fn, mesh_tri_start ? "set" : "null", mesh_tris ? "set" : "null", (long long)T);
-  if (meshes && B > 0)
-    intersect_kernel<true><<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
-        rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id, t_in, t_out, mesh_tri_start, mesh_tris, T);
+  if (fr) {
+    const int rc = pnr::check_frame_table(fn, fr, B);
+    if (rc != PNR_OK) return rc;
+  }
+  const bool frames = fr && fr->F != 0;
+  const unsigned grid = blocks_for(R, 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (frames && meshes)
+    intersect_kernel<true, true><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, fr->S, M, hit_mask,
+                                                       box_id, t_in, t_out, mesh_tri_start, mesh_tris, T, fr->ray_frame,
+                                                       fr->frame_boxes, fr->F, B);
+  else if (frames)
+    intersect_kernel<false, true><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, fr->S, M, hit_mask,
+                                                        box_id, t_in, t_out, nullptr, nullptr, 0, fr->ray_frame,
+                                                        fr->frame_boxes, fr->F, B);
+  else if (meshes && B > 0)
+    intersect_kernel<true, false><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id,
+                                                        t_in, t_out, mesh_tri_start, mesh_tris, T, nullptr, nullptr, 0,
+                                                        B);
   else
-    intersect_kernel<false><<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
-        rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id, t_in, t_out, nullptr, nullptr, 0);
+    intersect_kernel<false, false><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id,
+                                                         t_in, t_out, nullptr, nullptr, 0, nullptr, nullptr, 0, B);
   PNR_LAUNCH_CHECK("intersect_kernel");
   return PNR_OK;
 }
@@ -366,7 +437,7 @@ extern "C" int pnr_intersect_meshes(const float* rays, int64_t R, const float* b
                                     int64_t T, int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in,
                                     float* t_out, void* stream) {
   return intersect_rays("pnr_intersect_meshes", rays, R, box_center, box_half, box_rot, mesh_tri_start, mesh_tris, T, B, M,
-                        hit_mask, box_id, t_in, t_out, stream);
+                        hit_mask, box_id, t_in, t_out, nullptr, stream);
 }
 
 extern "C" int pnr_intersect(const float* rays, int64_t R, const float* box_center,
@@ -374,7 +445,13 @@ extern "C" int pnr_intersect(const float* rays, int64_t R, const float* box_cent
                              uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
                              void* stream) {
   return intersect_rays("pnr_intersect", rays, R, box_center, box_half, box_rot, nullptr, nullptr, 0, B, M, hit_mask, box_id,
-                        t_in, t_out, stream);
+                        t_in, t_out, nullptr, stream);
+}
+
+extern "C" int pnr_intersect_frames(const pnr_intersect_frames_args* a, void* stream) {
+  PNR_CHECK_ARG(a, "pnr_intersect_frames: null args");
+  return intersect_rays("pnr_intersect_frames", a->rays, a->R, a->box_center, a->box_half, a->box_rot, a->mesh_tri_start,
+                        a->mesh_tris, a->T, a->B, a->M, a->hit_mask, a->box_id, a->t_in, a->t_out, &a->frames, stream);
 }
 
 extern "C" int pnr_scene_near_far(const float* rays, int64_t R, const float* aabb_host, float near_min,

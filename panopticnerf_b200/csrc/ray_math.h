@@ -266,6 +266,19 @@ PNR_HD void pnr_tri_range(const int32_t* tri_start, int b, int64_t T, int* k0, i
   *k0 = (int)lo;
   *k1 = (int)hi;
 }
+// Dynamic block [*b0, *b1) of frame f in a sequence table of S static and Bt primitives (DESIGN 3.2): the entry
+// frame_boxes[f] = (begin, end) clamped into [S, Bt], empty when end < begin; a frame outside [0, F) has no block, so
+// its rays meet the static primitives only.
+PNR_HD void pnr_frame_range(int f, const int32_t* frame_boxes, int F, int S, int Bt, int* b0, int* b1) {
+  int lo = S, hi = S;
+  if (f >= 0 && f < F) {
+    const int a = frame_boxes[2 * f], e = frame_boxes[2 * f + 1];
+    lo = a < S ? S : (a > Bt ? Bt : a);
+    hi = e < lo ? lo : (e > Bt ? Bt : e);
+  }
+  *b0 = lo;
+  *b1 = hi;
+}
 // Output slots of ray r: the M nearest hits, then padding (id -1, depths 0); t_in starts at the origin.
 PNR_HD void pnr_hits_store(const PnrHitList* L, int M, int64_t r, uint8_t* hit, int32_t* box_id, float* t_in,
                            float* t_out) {
@@ -545,6 +558,7 @@ PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, i
   if (a.depth_out) a.depth_out[row] = a.depth ? a.depth[p] : 0.f;
   if (a.pseudo_label) a.pseudo_label[row] = a.label ? (int32_t)a.label[p] : -1;
   if (a.pixel) a.pixel[row] = p;
+  if (a.frame) a.frame[row] = f;
   const int nw = a.N + a.Ni;
   for (int k = 0; k < nw; k += 4) {
     pnr_ray_draw(a.seed, a.step, r, 1u + (uint32_t)(k >> 2), w);

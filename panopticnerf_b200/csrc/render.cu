@@ -143,9 +143,16 @@ using namespace pnr;
     if (rc__ != PNR_OK) return rc__; \
   } while (0)
 
-extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* a, void* stream) {
+// fr: the sequence table's frame fields (pnr_render_fused_frames), or null
+static int render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* a, const pnr_frame_table* fr,
+                        void* stream) {
   PNR_CHECK_ARG(ctx && a, "pnr_render_fused: null pointer");
   if (a->R == 0) return PNR_OK;
+  if (fr) {   // checked first: these refusals need no context
+    PNR_TRY(check_frame_table("pnr_render_fused_frames", fr, a->B));
+    PNR_CHECK_ARG(fr->F == 0 || a->B > 0, "pnr_render_fused_frames: F=%d without primitives (B=%d)", fr->F, a->B);
+    if (fr->F == 0) fr = nullptr;
+  }
   if (!ctx_fine) ctx_fine = ctx;
   const int N = a->N, Ni = a->Ni, M = a->M;
   int C = 0, K = 0, Cf = 0, Kf = 0;
@@ -223,7 +230,12 @@ extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_rende
       bid = L.have_hits ? a->box_id + r0 * M : bid_s;
       tin = L.have_hits ? a->t_in + r0 * M : tin_s;
       tout = L.have_hits ? a->t_out + r0 * M : tout_s;
-      if (a->T > 0)
+      if (fr) {
+        pnr_intersect_frames_args x{rays, n, a->box_center, a->box_half, a->box_rot, a->B, M, a->mesh_tri_start,
+                                    a->mesh_tris, a->T, *fr, hit, bid, tin, tout};
+        x.frames.ray_frame += r0;
+        PNR_TRY(pnr_intersect_frames(&x, stream));
+      } else if (a->T > 0)
         PNR_TRY(pnr_intersect_meshes(rays, n, a->box_center, a->box_half, a->box_rot, a->mesh_tri_start, a->mesh_tris,
                                      a->T, a->B, M, hit, bid, tin, tout, stream));
       else
@@ -268,4 +280,13 @@ extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_rende
     }
   }
   return PNR_OK;
+}
+
+extern "C" int pnr_render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* a, void* stream) {
+  return render_fused(ctx, ctx_fine, a, nullptr, stream);
+}
+
+extern "C" int pnr_render_fused_frames(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* a,
+                                       const pnr_frame_table* frames, void* stream) {
+  return render_fused(ctx, ctx_fine, a, frames, stream);
 }

@@ -5,12 +5,12 @@ reference's dataset code is not in the mount; the formats follow the public KITT
 as recalled, every reader says what it expects and fails loudly on anything else."""
 from .calib import (load_cam0_to_world, load_cam_to_pose, load_fisheye_yaml, load_perspective, load_poses,
                     perspective_batch, fisheye_batch)
-from .bboxes import Box3D, boxes_to_primitives, parse_bboxes_xml, primitive_batch
+from .bboxes import Box3D, boxes_to_primitives, parse_bboxes_xml, primitive_batch, sequence_primitives
 from .intersection_cache import load_intersections, save_intersections
 from .groundtruth import load_panoptic_gt, load_semantic_gt
 from .frames import load_frames
 
 __all__ = ["load_cam0_to_world", "load_cam_to_pose", "load_fisheye_yaml", "load_perspective", "load_poses",
            "perspective_batch", "fisheye_batch", "Box3D", "boxes_to_primitives", "parse_bboxes_xml",
-           "primitive_batch", "load_intersections", "save_intersections", "load_panoptic_gt", "load_semantic_gt",
+           "primitive_batch", "sequence_primitives", "load_intersections", "save_intersections", "load_panoptic_gt", "load_semantic_gt",
            "load_frames"]

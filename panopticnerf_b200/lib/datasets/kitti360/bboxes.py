@@ -13,7 +13,7 @@ from __future__ import annotations
 
 import xml.etree.ElementTree as ET
 from dataclasses import dataclass
-from typing import Dict, Iterable, List, Optional
+from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 
@@ -164,12 +164,49 @@ def boxes_to_primitives(boxes: Iterable[Box3D], frame: Optional[int] = None, ort
     return out
 
 
+def sequence_primitives(boxes: Iterable[Box3D], frame_ids: Sequence[int], ortho_tol: float = 1e-3,
+                        meshes: bool = False) -> Dict[str, np.ndarray]:
+    """One primitive table for the rays of many frames (DESIGN 3.2): the static boxes (boxes_to_primitives(frame=None))
+    at ids [0, S), then one block of dynamic boxes per distinct timestamp among `frame_ids`, in order of first
+    appearance.  Adds static_boxes = S and frame_boxes [F,2] int32, row f = (begin, end) of frame_ids[f]'s block
+    (frames of one timestamp share it; a frame without dynamic boxes has an empty range).  A ray of frame f meets
+    [0, S) and its frame's block (include/pnr.h pnr_intersect_frames), which equals boxes_to_primitives(frame=
+    frame_ids[f]) up to the order of the boxes.  With a FrameSet: frame_ids = [fid for _, fid in frames.names]."""
+    boxes = list(boxes)
+    fids = [int(f) for f in frame_ids]
+    parts = [boxes_to_primitives(boxes, None, ortho_tol, meshes)]
+    begin, where = {}, parts[0]["box_center"].shape[0]
+    for t in fids:
+        if t in begin:
+            continue
+        part = boxes_to_primitives([b for b in boxes if b.timestamp == t != -1], t, ortho_tol, meshes)
+        begin[t] = (where, where + part["box_center"].shape[0])
+        where += part["box_center"].shape[0]
+        parts.append(part)
+    out = {k: np.concatenate([p[k] for p in parts], 0) for k in ("box_center", "box_half", "box_rot", "box_sem", "box_inst")}
+    out["names"] = [n for p in parts for n in p["names"]]
+    if any("mesh_tris" in p for p in parts):
+        start, tris = [0], []
+        for p in parts:
+            n = p["box_center"].shape[0]
+            own = np.diff(p["mesh_tri_start"]) if "mesh_tris" in p else np.zeros(n, dtype=np.int64)
+            start += (start[-1] + np.cumsum(own)).tolist()
+            if "mesh_tris" in p:
+                tris.append(p["mesh_tris"])
+        out["mesh_tri_start"] = np.asarray(start, dtype=np.int32)
+        out["mesh_tris"] = np.ascontiguousarray(np.concatenate(tris, 0), dtype=np.float32)
+    out["static_boxes"] = int(parts[0]["box_center"].shape[0])
+    out["frame_boxes"] = np.asarray([begin[t] for t in fids], dtype=np.int32).reshape(len(fids), 2)
+    return out
+
+
 def primitive_batch(prims: Dict[str, np.ndarray], sem_to_train: Optional[Dict[int, int]] = None,
                     inst_to_slot: Optional[Dict[int, int]] = None, device="cuda") -> Dict[str, "object"]:
     """The primitive block of a render batch (torch tensors on `device`).  `sem_to_train` maps KITTI-360 semanticIds
     to the network's class channels, `inst_to_slot` instanceIds to its instance channels; boxes whose id has no
     channel get -1 (they still bound samples, they just do not vote in the fixed maps).  The mesh table
-    (mesh_tri_start, mesh_tris) is carried along when the primitives have one."""
+    (mesh_tri_start, mesh_tris) and a sequence table's frame_boxes (int32 tensor) and static_boxes (int) are carried
+    along when the primitives have them."""
     import torch
     sem = np.array([(sem_to_train or {}).get(int(s), int(s) if sem_to_train is None else -1) for s in prims["box_sem"]], dtype=np.int32)
     inst = np.array([(inst_to_slot or {}).get(int(s), int(s) if inst_to_slot is None else -1) for s in prims["box_inst"]], dtype=np.int32)
@@ -177,4 +214,6 @@ def primitive_batch(prims: Dict[str, np.ndarray], sem_to_train: Optional[Dict[in
     return {"box_center": t(prims["box_center"], torch.float32), "box_half": t(prims["box_half"], torch.float32),
             "box_rot": t(prims["box_rot"], torch.float32), "box_sem": t(sem, torch.int32), "box_inst": t(inst, torch.int32),
             **({"mesh_tri_start": t(prims["mesh_tri_start"], torch.int32), "mesh_tris": t(prims["mesh_tris"], torch.float32)}
-               if "mesh_tris" in prims else {})}
+               if "mesh_tris" in prims else {}),
+            **({"frame_boxes": t(prims["frame_boxes"], torch.int32), "static_boxes": int(prims["static_boxes"])}
+               if "frame_boxes" in prims else {})}

@@ -138,10 +138,10 @@ def concat_frame_sets(*sets: FrameSet) -> FrameSet:
 
 
 def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N: int, Ni: int = 0,
-                     want_pixel: bool = False) -> Dict[str, torch.Tensor]:
+                     want_pixel: bool = False, want_frame: bool = False) -> Dict[str, torch.Tensor]:
     """Rays r0 .. r1-1 of the batch (seed, step): one pnr_sample_ray_batch launch on the frames' device.  Returns
     rays [n,6], rgb [n,3], u [n,N], u_fine [n,Ni] (Ni > 0), depth [n] / pseudo_label [n] i32 when the set has a depth /
-    label table, and pixel [n] i64 (the flat pixel index) when asked."""
+    label table, pixel [n] i64 (the flat pixel index) and frame [n] i32 (the frame of the pixel) when asked."""
     if not (0 <= int(seed) < 1 << 64 and 0 <= int(step) < 1 << 64):
         raise ValueError(f"sample_ray_batch: seed {seed} and step {step} must be in [0, 2^64)")
     dev = frames.rgb8.device
@@ -156,6 +156,8 @@ def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N
         out["pseudo_label"] = e(max(n, 0), dtype=torch.int32)
     if want_pixel:
         out["pixel"] = e(max(n, 0), dtype=torch.int64)
+    if want_frame:
+        out["frame"] = e(max(n, 0), dtype=torch.int32)
     a = _capi.PnrRayBatchArgs()
     a.c2w = _capi.ptr(frames.c2w, torch.float32, "c2w")
     a.frame_cam = _capi.ptr(frames.frame_cam, torch.int32, "frame_cam")
@@ -175,7 +177,7 @@ def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N
     a.rays, a.rgb, a.u = _capi.ptr(out["rays"]), _capi.ptr(out["rgb"]), _capi.ptr(out["u"])
     a.u_fine = _capi.ptr(out.get("u_fine"))
     a.depth_out, a.pseudo_label = _capi.ptr(out.get("depth")), _capi.ptr(out.get("pseudo_label"))
-    a.pixel = _capi.ptr(out.get("pixel"))
+    a.pixel, a.frame = _capi.ptr(out.get("pixel")), _capi.ptr(out.get("frame"))
     with torch.cuda.device(dev):
         _capi.check(_capi.lib().pnr_sample_ray_batch(C.byref(a), _capi.stream_ptr()), "pnr_sample_ray_batch")
     return out
@@ -183,20 +185,30 @@ def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N
 
 class RaySampler:
     """RaySampler(frames, seed, scene).batch(step, R, N, Ni) -> a training batch of R random pixels of the frame set.
-    `scene`: the replicated block every batch carries (the static primitive table of `kitti360.primitive_batch`, a
-    mesh table, scene_aabb, ...).  One table serves rays of every frame, so it holds the static annotations
-    (boxes_to_primitives(frame=None)); per-frame dynamic boxes are not part of a sampled batch."""
+    `scene`: the replicated block every batch carries (the primitive table of `kitti360.primitive_batch`, a mesh
+    table, scene_aabb, ...).  With a sequence table (`kitti360.sequence_primitives` with frame_ids = [fid for _, fid in
+    frames.names], so that frame_boxes has one row per frame of the set) each batch also carries ray_frame [R] i32,
+    the frame of each ray, and every ray meets the static primitives and its own frame's dynamic ones, as a render of
+    that frame does.  Without frame_boxes the table serves every frame as it is (e.g. the static annotations,
+    boxes_to_primitives(frame=None))."""
 
     def __init__(self, frames: FrameSet, seed: int, scene: Optional[Dict[str, torch.Tensor]] = None):
         self.frames, self.seed = frames, int(seed)
         self.scene = dict(scene or {})
-        clash = set(self.scene) & {"rays", "rgb", "u", "u_fine", "depth", "pseudo_label"}
+        clash = set(self.scene) & {"rays", "rgb", "u", "u_fine", "depth", "pseudo_label", "ray_frame"}
         if clash:
             raise ValueError(f"RaySampler: the scene block may not carry the per-ray keys {sorted(clash)}")
+        fb = self.scene.get("frame_boxes")
+        if fb is not None and tuple(fb.shape) != (frames.num_frames, 2):
+            raise ValueError(f"RaySampler: frame_boxes {tuple(fb.shape)} needs one (begin, end) row per frame of the "
+                             f"set, ({frames.num_frames}, 2)")
 
     def batch(self, step: int, R: int, N: int, Ni: int = 0) -> Dict[str, torch.Tensor]:
         """The global batch of `step`: rays 0 .. R-1, identical on every rank that uses the same seed."""
-        out = sample_ray_batch(self.frames, self.seed, step, 0, R, N, Ni)
+        seq = "frame_boxes" in self.scene
+        out = sample_ray_batch(self.frames, self.seed, step, 0, R, N, Ni, want_frame=seq)
+        if seq:
+            out["ray_frame"] = out.pop("frame")
         out.update(self.scene)
         return out
 

@@ -97,9 +97,12 @@ def _rays(rays_d: torch.Tensor) -> torch.Tensor:
 # stage wrappers (one libpnr call each)
 # ------------------------------------------------------------------------------------------------
 @_on_tensor_device
-def intersect(rays, box_center, box_half, box_rot, max_hits: int, mesh_tri_start=None, mesh_tris=None):
+def intersect(rays, box_center, box_half, box_rot, max_hits: int, mesh_tri_start=None, mesh_tris=None,
+              ray_frame=None, frame_boxes=None, static_boxes=None):
     """a5 -> hit_mask [R] bool, box_id [R,M] i32, t_in, t_out [R,M].  With a mesh table (mesh_tri_start [B+1] int32,
-    mesh_tris [T,3,3]) the primitives that own triangles are closed meshes culled by their box (DESIGN 3.2)."""
+    mesh_tris [T,3,3]) the primitives that own triangles are closed meshes culled by their box (DESIGN 3.2).  With a
+    sequence table (ray_frame [R] int, frame_boxes [F,2] int, static_boxes S: kitti360.sequence_primitives) ray r meets
+    the primitives [0, S) and its frame's block frame_boxes[ray_frame[r]] (include/pnr.h pnr_intersect_frames)."""
     rays = _f(rays, "rays")
     R, B, M = rays.shape[0], box_center.shape[0], int(max_hits)
     dev = rays.device
@@ -108,17 +111,46 @@ def intersect(rays, box_center, box_half, box_rot, max_hits: int, mesh_tri_start
     t_in = torch.empty(R, M, dtype=_F32, device=dev)
     t_out = torch.empty(R, M, dtype=_F32, device=dev)
     bc, bh, br = _f(box_center, "box_center"), _f(box_half, "box_half"), _f(box_rot, "box_rot")
-    if mesh_tri_start is None and mesh_tris is None:
+    mesh = mesh_tri_start is not None or mesh_tris is not None
+    starts, tris = _mesh_table(mesh_tri_start, mesh_tris, B, dev) if mesh else (None, None)
+    frames = _frame_table(ray_frame, frame_boxes, static_boxes, R, dev)
+    if frames is not None:
+        a = _capi.PnrIntersectFramesArgs(rays=_capi.ptr(rays), R=R, box_center=_capi.ptr(bc), box_half=_capi.ptr(bh),
+                                         box_rot=_capi.ptr(br), B=B, M=M, mesh_tri_start=_capi.ptr(starts),
+                                         mesh_tris=_capi.ptr(tris), T=tris.shape[0] if mesh else 0,
+                                         frames=frames[0], hit_mask=_capi.ptr(hit), box_id=_capi.ptr(box_id),
+                                         t_in=_capi.ptr(t_in), t_out=_capi.ptr(t_out))
+        _capi.check(_capi.lib().pnr_intersect_frames(C.byref(a), _capi.stream_ptr()), "pnr_intersect_frames")
+        return hit.bool(), box_id, t_in, t_out
+    if not mesh:
         _capi.check(_capi.lib().pnr_intersect(_capi.ptr(rays), R, _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br), B, M,
                                               _capi.ptr(hit), _capi.ptr(box_id), _capi.ptr(t_in), _capi.ptr(t_out),
                                               _capi.stream_ptr()), "pnr_intersect")
         return hit.bool(), box_id, t_in, t_out
-    starts, tris = _mesh_table(mesh_tri_start, mesh_tris, B, dev)
     _capi.check(_capi.lib().pnr_intersect_meshes(_capi.ptr(rays), R, _capi.ptr(bc), _capi.ptr(bh), _capi.ptr(br),
                                                  _capi.ptr(starts), _capi.ptr(tris), tris.shape[0], B, M,
                                                  _capi.ptr(hit), _capi.ptr(box_id), _capi.ptr(t_in), _capi.ptr(t_out),
                                                  _capi.stream_ptr()), "pnr_intersect_meshes")
     return hit.bool(), box_id, t_in, t_out
+
+
+def _frame_table(ray_frame, frame_boxes, static_boxes, R: int, device):
+    """(PnrFrameTable, tensors it points to) of a sequence table on `device`, or None without one; shapes checked (the
+    library checks S against B and clamps the ranges)."""
+    given = [x is not None for x in (ray_frame, frame_boxes, static_boxes)]
+    if not any(given):
+        return None
+    if not all(given):
+        raise ValueError("a sequence table needs ray_frame, frame_boxes and static_boxes together (ray_frame "
+                         f"{'set' if given[0] else 'missing'}, frame_boxes {'set' if given[1] else 'missing'}, "
+                         f"static_boxes {'set' if given[2] else 'missing'})")
+    rf = ray_frame.to(device=device, dtype=_I32).contiguous()
+    fb = frame_boxes.to(device=device, dtype=_I32).contiguous()
+    if tuple(rf.shape) != (R,) or fb.dim() != 2 or fb.shape[1] != 2 or fb.shape[0] < 1:
+        raise ValueError(f"sequence table: ray_frame {tuple(rf.shape)} (want ({R},)), frame_boxes {tuple(fb.shape)} "
+                         "(want (F, 2), F >= 1)")
+    t = _capi.PnrFrameTable(ray_frame=_capi.ptr(rf), frame_boxes=_capi.ptr(fb), F=fb.shape[0], S=int(static_boxes))
+    return t, (rf, fb)
 
 
 def _mesh_table(mesh_tri_start, mesh_tris, B: int, device):
@@ -363,6 +395,7 @@ class Renderer:
     """Renderer(cfg, net).render(batch) -> dict of per-ray maps (a3).  batch keys: rays [R,6] (o||d),
     optional near/far [R], scene_aabb [2,3], box_center/box_half [B,3], box_rot [B,3,3], box_sem/box_inst [B],
     mesh_tri_start [B+1] int32 / mesh_tris [T,3,3] (mesh primitives: include/pnr.h pnr_intersect_meshes),
+    ray_frame [R] / frame_boxes [F,2] / static_boxes (a sequence table: include/pnr.h pnr_intersect_frames),
     u [R,N] / u_fine [R,Ni] (externally supplied jitter), perturb."""
 
     def __init__(self, cfg, net, net_fine=None):
@@ -418,8 +451,10 @@ class Renderer:
         has_boxes = "box_center" in batch and batch["box_center"].shape[0] > 0
         box_id = t_in = t_out = None
         if has_boxes:
+            rf = batch["ray_frame"][sl] if batch.get("ray_frame") is not None else None
             hit, box_id, t_in, t_out = intersect(rays, batch["box_center"], batch["box_half"],
-                                                 batch["box_rot"], M, batch.get("mesh_tri_start"), batch.get("mesh_tris"))
+                                                 batch["box_rot"], M, batch.get("mesh_tri_start"), batch.get("mesh_tris"),
+                                                 rf, batch.get("frame_boxes"), batch.get("static_boxes"))
             out.update(hit_mask=hit, box_id=box_id, t_in=t_in, t_out=t_out)
             if bool(getattr(cfg, "bound_by_primitives", False)):
                 near, far = bound_by_primitives(hit, box_id, t_in, t_out, near, far)
@@ -581,6 +616,9 @@ class Renderer:
                 starts, tris = _mesh_table(batch.get("mesh_tri_start"), batch.get("mesh_tris"), bc.shape[0], dev)
                 keep += [starts, tris]
                 a.mesh_tri_start, a.mesh_tris, a.T = _capi.ptr(starts), _capi.ptr(tris), tris.shape[0]
+            frames = _frame_table(batch.get("ray_frame"), batch.get("frame_boxes"), batch.get("static_boxes"), R, dev)
+            if frames is not None:
+                keep.append(frames[1])
         a.N, a.Ni = N, Ni
         tv = self._tv(N, dev)
         a.t_vals = _capi.ptr(tv)
@@ -615,7 +653,11 @@ class Renderer:
         out["near"], out["far"] = near, far          # as given (bound_by_primitives works on a private copy)
         ws = self._workspace(ctx, R, N, Ni, dev)
         a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel()
-        _capi.check(_capi.lib().pnr_render_fused(ctx, ctx_fine, C.byref(a), _capi.stream_ptr()), "pnr_render_fused")
+        if has_boxes and frames is not None:
+            _capi.check(_capi.lib().pnr_render_fused_frames(ctx, ctx_fine, C.byref(a), C.byref(frames[0]),
+                                                            _capi.stream_ptr()), "pnr_render_fused_frames")
+        else:
+            _capi.check(_capi.lib().pnr_render_fused(ctx, ctx_fine, C.byref(a), _capi.stream_ptr()), "pnr_render_fused")
         del keep
         if has_boxes:
             out["hit_mask"] = hit8.bool()

@@ -7,10 +7,14 @@ the numbers as JSON, and also writes that JSON to --out when given.
   2. the same frame with the 64 cuboids plus the five meshes of synthetic.make_mesh_primitives (an ellipsoid and a
      nested one, a U extrusion, the ~2000-triangle road under the camera, a cuboid as 12 triangles), with the number of
      triangle tests (rays in each mesh's cull box x its triangles);
-  3. for scale, the fused render of that frame (cfg2 network) with cuboids only and with the meshes."""
+  3. for scale, the fused render of that frame (cfg2 network) with cuboids only and with the meshes;
+  4. a sequence table (pnr_intersect_frames: S static boxes, then 20 dynamic boxes for each of 300 frames) against the
+     static table alone (pnr_intersect on the S boxes), for S = 64 and 2000: a 2048-ray training batch whose rays belong
+     to random frames, and a cfg2 frame whose rays all belong to one frame."""
 from __future__ import annotations
 
 import argparse
+import ctypes as C
 import json
 import statistics
 import subprocess
@@ -51,6 +55,38 @@ def timed(fns, reps: int, warmup: int):
             b.synchronize()
             ms[k].append(a.elapsed_time(b))
     return {k: statistics.median(v) for k, v in ms.items()}, {k: (min(v), max(v)) for k, v in ms.items()}
+
+
+def sequence_tables(frame_rays, M: int, reps: int, warmup: int, F: int = 300, per_frame: int = 20):
+    """{case: median ms}: static-only against the sequence table, alternated, for a training batch and a frame."""
+    g = torch.Generator().manual_seed(0)
+    batch_rays = frame_rays[torch.randperm(frame_rays.shape[0], generator=g)[:2048].to(DEV)].contiguous()
+    L = _capi.lib()
+    fns, keep = {}, []
+    for S_ in (64, 2000):
+        prims = {k: v.to(DEV) for k, v in S.make_boxes(S_ + F * per_frame, seed=S_).items()}
+        fb = torch.stack([S_ + per_frame * torch.arange(F), S_ + per_frame * torch.arange(1, F + 1)], 1)
+        fb = fb.to(torch.int32).to(DEV)
+        for name, rays, rf in (("batch2048", batch_rays, torch.randint(0, F, (2048,), generator=g, dtype=torch.int32)),
+                               ("frame", frame_rays, torch.full((frame_rays.shape[0],), 7, dtype=torch.int32))):
+            R = rays.shape[0]
+            rf = rf.to(DEV)
+            out = [torch.empty(R, dtype=torch.uint8, device=DEV), torch.empty(R, M, dtype=torch.int32, device=DEV),
+                   torch.empty(R, M, device=DEV), torch.empty(R, M, device=DEV)]
+            keep += [prims, fb, rays, rf, out]
+            a = _capi.PnrIntersectFramesArgs(rays=rays.data_ptr(), R=R, box_center=prims["box_center"].data_ptr(),
+                                             box_half=prims["box_half"].data_ptr(), box_rot=prims["box_rot"].data_ptr(),
+                                             B=S_ + F * per_frame, M=M, hit_mask=out[0].data_ptr(),
+                                             box_id=out[1].data_ptr(), t_in=out[2].data_ptr(), t_out=out[3].data_ptr())
+            a.frames = _capi.PnrFrameTable(ray_frame=rf.data_ptr(), frame_boxes=fb.data_ptr(), F=F, S=S_)
+            static = lambda a=a, S_=S_: _capi.check(L.pnr_intersect(a.rays, a.R, a.box_center, a.box_half, a.box_rot,
+                                                                    S_, a.M, a.hit_mask, a.box_id, a.t_in, a.t_out,
+                                                                    _capi.stream_ptr()))
+            seq = lambda a=a: _capi.check(L.pnr_intersect_frames(C.byref(a), _capi.stream_ptr()))
+            keep.append(a)
+            fns[f"{name}_S{S_}_static"] = static
+            fns[f"{name}_S{S_}_sequence"] = seq
+    return timed(fns, reps, warmup)
 
 
 def main():
@@ -104,9 +140,11 @@ def main():
     b_cub, b_mesh = dict(base, **bx), dict(base, **mp)
     rmed, rrng = timed({"render_cuboids": lambda: ren.render(b_cub), "render_meshes": lambda: ren.render(b_mesh)},
                        max(20, args.reps // 5), 2)
+    smed, srng = sequence_tables(rays, M, args.reps, args.warmup)
     res = dict(card=card(), rays=R, M=M, cuboids=B, primitives_mixed=Bm, triangles=int(mp["mesh_tris"].shape[0]),
                triangle_tests=tests, triangle_tests_per_ray=tests / R, per_mesh=per_mesh, median_ms={**med, **rmed},
-               min_max_ms={**rng, **rrng})
+               min_max_ms={**rng, **rrng}, sequence_table=dict(frames=300, dynamic_per_frame=20, median_ms=smed,
+                                                               min_max_ms=srng))
     print(json.dumps(res, indent=1))
     if args.out is not None:
         args.out.parent.mkdir(parents=True, exist_ok=True)
