@@ -22,6 +22,13 @@ int sample_pdf_strided(const float* z, const float* weights, int64_t R, int32_t 
 // the host checks of a sequence table's frame fields against B primitives (ray_kernels.cu; pnr_intersect_frames and
 // pnr_render_fused_frames name themselves with fn)
 int check_frame_table(const char* fn, const pnr_frame_table* fr, int32_t B);
+// a5 on B primitives, with their meshes (mesh_tri_start / mesh_tris null and T = 0: cuboids only) and frame table
+// (fr null: every primitive static) (ray_kernels.cu; the pnr_intersect* entry points and pnr_render_fused*).  fn: the
+// entry point's name in the error messages.
+int intersect_rays(const char* fn, const float* rays, int64_t R, const float* box_center, const float* box_half,
+                   const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T, int32_t B,
+                   int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out, const pnr_frame_table* fr,
+                   void* stream);
 
 #define PNR_CHECK_ARG(cond, ...) \
   do { if (!(cond)) return ::pnr::set_error(PNR_ERR_ARG, __VA_ARGS__); } while (0)

@@ -11,6 +11,7 @@ namespace pnr {
 // ------------------------------------------------------------------------------------ a5 intersect
 constexpr int kBoxChunk = 512;  // boxes staged per shared-memory fill (15 floats each = 30 KB; 17 with meshes)
 
+// Each primitive goes through pnr_prim_step (ray_math.h), which the host build of the CPU tests calls too.
 // kMeshes = false: the slab test of every box (pnr_intersect).  kMeshes = true: a box whose triangle range
 // [tri_start[b], tri_start[b+1]) is not empty is the cull volume of a closed mesh (ray_math.h: pnr_tri_cross,
 // PnrMeshCross); on a cull hit its triangles are read from global memory (the same rows for the whole warp, so
@@ -60,64 +61,26 @@ __global__ void __launch_bounds__(256) intersect_kernel(const float* __restrict_
     }
     __syncthreads();
     if (r < R) {
-      // the per-primitive step; tests/host_emu.cpp writes it out again, because as a shared function it changes the
-      // mesh instantiation's SASS
       for (int b = 0; b < nb; ++b) {
         const float* q = sb + b * kS;
-        float tmin, tmax;
-        const bool hit = pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax);
-        if (kMeshes) {
-          const int k0 = __float_as_int(q[15]), k1 = __float_as_int(q[16]);
-          if (k0 == k1) {
-            if (hit) pnr_hits_insert(&L, M, tmin, tmax, b0 + b);
-          } else if (hit) {
-            const PnrShear S = pnr_shear(dx, dy, dz);
-            PnrMeshCross X;
-            pnr_cross_init(&X);
-            for (int k = k0; k < k1; ++k) {
-              float v[9];
-#pragma unroll
-              for (int e = 0; e < 9; ++e) v[e] = __ldg(tris + (int64_t)k * 9 + e);
-              float t;
-              if (pnr_tri_cross(ox, oy, oz, S, v, &t)) pnr_cross_add(&X, M, t);
-            }
-            pnr_cross_emit(&X, &L, M, b0 + b);
-          }
-        } else if (hit) {
-          pnr_hits_insert(&L, M, tmin, tmax, b0 + b);
-        }
+        const int k0 = kMeshes ? __float_as_int(q[15]) : 0, k1 = kMeshes ? __float_as_int(q[16]) : 0;
+        pnr_prim_step(ox, oy, oz, dx, dy, dz, q, k0, k1, tris, M, b0 + b, &L);
       }
     }
   }
   if (kFrames && r < R) {
     int b0, b1;
     pnr_frame_range(ray_frame[r], frame_boxes, F, B, Bt, &b0, &b1);
-    // the per-primitive step of the static chunks, on a box read from global memory
+    // the same step on a box read from global memory
     for (int b = b0; b < b1; ++b) {
       float q[15];
 #pragma unroll
       for (int e = 0; e < 3; ++e) { q[e] = __ldg(bc + (int64_t)b * 3 + e); q[3 + e] = __ldg(bh + (int64_t)b * 3 + e); }
 #pragma unroll
       for (int e = 0; e < 9; ++e) q[6 + e] = __ldg(br + (int64_t)b * 9 + e);
-      float tmin, tmax;
-      const bool hit = pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax);
       int k0 = 0, k1 = 0;
       if (kMeshes) pnr_tri_range(tri_start, b, T, &k0, &k1);
-      if (k0 == k1) {
-        if (hit) pnr_hits_insert(&L, M, tmin, tmax, b);
-      } else if (hit) {
-        const PnrShear S = pnr_shear(dx, dy, dz);
-        PnrMeshCross X;
-        pnr_cross_init(&X);
-        for (int k = k0; k < k1; ++k) {
-          float v[9];
-#pragma unroll
-          for (int e = 0; e < 9; ++e) v[e] = __ldg(tris + (int64_t)k * 9 + e);
-          float t;
-          if (pnr_tri_cross(ox, oy, oz, S, v, &t)) pnr_cross_add(&X, M, t);
-        }
-        pnr_cross_emit(&X, &L, M, b);
-      }
+      pnr_prim_step(ox, oy, oz, dx, dy, dz, q, k0, k1, tris, M, b, &L);
     }
   }
   if (r < R) pnr_hits_store(&L, M, r, hit_mask, box_id, t_in, t_out);
@@ -182,7 +145,8 @@ __global__ void __launch_bounds__(256) stratified_kernel(
     }
     if (sample_box != nullptr) {
       int32_t tag = -1;
-      // pnr_tag's rule, written out: sharing it changes the SASS of this kernel or of pnr_tag's callers
+      // pnr_tag's rule, written out: a predicate shared with pnr_tag takes the interval's bounds as values, so
+      // pnr_tag would load t_in / t_out before it tests the id, which changes tag_kernel's and interval_kernel's SASS
       for (int m = M - 1; m >= 0; --m) {   // first (nearest) containing interval wins
         const int32_t id = __shfl_sync(0xffffffffu, my_id, m);
         const float a = __shfl_sync(0xffffffffu, my_in, m), b = __shfl_sync(0xffffffffu, my_out, m);
@@ -391,12 +355,10 @@ int pnr::check_frame_table(const char* fn, const pnr_frame_table* fr, int32_t B)
   return PNR_OK;
 }
 
-// fn: the entry point's name in the error messages.  fr: the sequence table's frame fields, or null (every primitive
-// static).
-static int intersect_rays(const char* fn, const float* rays, int64_t R, const float* box_center, const float* box_half,
-                     const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T, int32_t B,
-                     int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
-                     const pnr_frame_table* fr, void* stream) {
+int pnr::intersect_rays(const char* fn, const float* rays, int64_t R, const float* box_center, const float* box_half,
+                        const float* box_rot, const int32_t* mesh_tri_start, const float* mesh_tris, int64_t T,
+                        int32_t B, int32_t M, uint8_t* hit_mask, int32_t* box_id, float* t_in, float* t_out,
+                        const pnr_frame_table* fr, void* stream) {
   if (R == 0) return PNR_OK;  // empty input: nothing to do (pointers of empty tensors may be null)
   PNR_CHECK_ARG(R >= 0 && B >= 0, "%s: R=%lld or B=%d < 0", fn, (long long)R, B);
   PNR_CHECK_ARG(M >= 1 && M <= PNR_MAX_HITS, "%s: M=%d outside [1,%d]", fn, M, PNR_MAX_HITS);
@@ -411,23 +373,12 @@ static int intersect_rays(const char* fn, const float* rays, int64_t R, const fl
     if (rc != PNR_OK) return rc;
   }
   const bool frames = fr && fr->F != 0;
-  const unsigned grid = blocks_for(R, 256);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (frames && meshes)
-    intersect_kernel<true, true><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, fr->S, M, hit_mask,
-                                                       box_id, t_in, t_out, mesh_tri_start, mesh_tris, T, fr->ray_frame,
-                                                       fr->frame_boxes, fr->F, B);
-  else if (frames)
-    intersect_kernel<false, true><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, fr->S, M, hit_mask,
-                                                        box_id, t_in, t_out, nullptr, nullptr, 0, fr->ray_frame,
-                                                        fr->frame_boxes, fr->F, B);
-  else if (meshes && B > 0)
-    intersect_kernel<true, false><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id,
-                                                        t_in, t_out, mesh_tri_start, mesh_tris, T, nullptr, nullptr, 0,
-                                                        B);
-  else
-    intersect_kernel<false, false><<<grid, 256, 0, st>>>(rays, R, box_center, box_half, box_rot, B, M, hit_mask, box_id,
-                                                         t_in, t_out, nullptr, nullptr, 0, nullptr, nullptr, 0, B);
+  // the cuboid instantiations never read the mesh table, nor the static-only ones the frame table
+  const auto kernel = frames ? (meshes ? intersect_kernel<true, true> : intersect_kernel<false, true>)
+                             : (meshes && B > 0 ? intersect_kernel<true, false> : intersect_kernel<false, false>);
+  kernel<<<blocks_for(R, 256), 256, 0, (cudaStream_t)stream>>>(
+      rays, R, box_center, box_half, box_rot, frames ? fr->S : B, M, hit_mask, box_id, t_in, t_out, mesh_tri_start,
+      mesh_tris, T, frames ? fr->ray_frame : nullptr, frames ? fr->frame_boxes : nullptr, frames ? fr->F : 0, B);
   PNR_LAUNCH_CHECK("intersect_kernel");
   return PNR_OK;
 }

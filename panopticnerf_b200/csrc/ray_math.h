@@ -1,11 +1,11 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
 // kernels (ray_kernels.cu, rays_kernel and ray_batch_kernel in stream_kernels.cu) and a host build used by the CPU tests
-// (tests/host_emu.cpp; tests/host_emu_ray_batch.cpp for the ray-batch routine) to prove the order matches the oracle
-// bit for bit without a GPU.  The kernels keep only layout here (staging, shuffles, sorts); the rules they apply per
-// ray - range clamps, sample depths, output slots, camera directions, batch draws - are the functions below, called by
-// both builds.  Two pieces stay written
-// out in the kernels and again in host_emu.cpp, because moving them into a function changes the SASS:
-// intersect_kernel's per-primitive step and stratified_kernel's interval test (pnr_tag's rule).
+// (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
+// here (staging, shuffles, sorts); the rules they apply per ray - the per-primitive intersection step, range clamps,
+// sample depths, output slots, camera directions, batch draws - are the functions below, called by both builds.  One
+// piece stays written out in stratified_kernel and again in host_emu.cpp: the interval test (pnr_tag's rule), because
+// a predicate shared with pnr_tag makes pnr_tag load t_in / t_out before it tests the id, which changes the SASS of
+// tag_kernel and interval_kernel.
 //
 // Rules (SURVEY.md 7.3 item 3): every multiply/add/subtract/divide is individually rounded (no FMA
 // contraction: __f*_rn intrinsics on device, -ffp-contract=off on host), true division, and min/max
@@ -30,6 +30,7 @@
 #define PNR_DSUB(a, b) __dsub_rn((a), (b))
 #define PNR_DMUL(a, b) __dmul_rn((a), (b))
 #define PNR_SQRT(a) __fsqrt_rn((a))
+#define PNR_LDG(p) __ldg((p))
 #else
 #define PNR_MUL(a, b) ((a) * (b))
 #define PNR_ADD(a, b) ((a) + (b))
@@ -39,6 +40,7 @@
 #define PNR_DSUB(a, b) ((a) - (b))
 #define PNR_DMUL(a, b) ((a) * (b))
 #define PNR_SQRT(a) sqrtf((a))
+#define PNR_LDG(p) (*(p))
 #endif
 
 #define PNR_MAX_HITS 8
@@ -252,6 +254,30 @@ PNR_HD void pnr_cross_emit(const PnrMeshCross* S, PnrHitList* L, int M, int32_t 
       if (c > a) pnr_hits_insert(L, M, a, c, b);
       kept += 1;
     }
+  }
+}
+
+// intersect_kernel's per-primitive step for primitive b: the slab test of its box q (center, half, rot: 15 floats),
+// then on a hit either the box's own interval (an empty triangle range: a cuboid) or the intervals of the mesh made of
+// triangles [k0, k1) of tris.
+PNR_HD void pnr_prim_step(float ox, float oy, float oz, float dx, float dy, float dz, const float* q, int k0, int k1,
+                          const float* tris, int M, int32_t b, PnrHitList* L) {
+  float tmin, tmax;
+  const bool hit = pnr_slab(ox, oy, oz, dx, dy, dz, q, q + 3, q + 6, &tmin, &tmax);
+  if (k0 == k1) {
+    if (hit) pnr_hits_insert(L, M, tmin, tmax, b);
+  } else if (hit) {
+    const PnrShear S = pnr_shear(dx, dy, dz);
+    PnrMeshCross X;
+    pnr_cross_init(&X);
+    for (int k = k0; k < k1; ++k) {
+      float v[9];
+#pragma unroll
+      for (int e = 0; e < 9; ++e) v[e] = PNR_LDG(tris + (int64_t)k * 9 + e);
+      float t;
+      if (pnr_tri_cross(ox, oy, oz, S, v, &t)) pnr_cross_add(&X, M, t);
+    }
+    pnr_cross_emit(&X, L, M, b);
   }
 }
 

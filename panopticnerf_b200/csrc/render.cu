@@ -230,16 +230,14 @@ static int render_fused(pnr_ctx* ctx, pnr_ctx* ctx_fine, const pnr_render_args* 
       bid = L.have_hits ? a->box_id + r0 * M : bid_s;
       tin = L.have_hits ? a->t_in + r0 * M : tin_s;
       tout = L.have_hits ? a->t_out + r0 * M : tout_s;
+      pnr_frame_table chunk_fr{};
       if (fr) {
-        pnr_intersect_frames_args x{rays, n, a->box_center, a->box_half, a->box_rot, a->B, M, a->mesh_tri_start,
-                                    a->mesh_tris, a->T, *fr, hit, bid, tin, tout};
-        x.frames.ray_frame += r0;
-        PNR_TRY(pnr_intersect_frames(&x, stream));
-      } else if (a->T > 0)
-        PNR_TRY(pnr_intersect_meshes(rays, n, a->box_center, a->box_half, a->box_rot, a->mesh_tri_start, a->mesh_tris,
-                                     a->T, a->B, M, hit, bid, tin, tout, stream));
-      else
-        PNR_TRY(pnr_intersect(rays, n, a->box_center, a->box_half, a->box_rot, a->B, M, hit, bid, tin, tout, stream));
+        chunk_fr = *fr;
+        chunk_fr.ray_frame += r0;
+      }
+      PNR_TRY(intersect_rays(fr ? "pnr_render_fused_frames" : "pnr_render_fused", rays, n, a->box_center, a->box_half,
+                             a->box_rot, a->mesh_tri_start, a->mesh_tris, a->T, a->B, M, hit, bid, tin, tout,
+                             fr ? &chunk_fr : nullptr, stream));
       if (a->bound_by_primitives) PNR_TRY(pnr_bound_by_primitives(hit, bid, tin, tout, n, M, near, far, stream));
     }
     // ---- a6: coarse depths + ids

@@ -1,43 +1,50 @@
 // host_emu.cpp — host build of csrc/ray_math.h, so CPU tests can prove that the ray kernels' fp32 operation order
 // equals the oracle's bit for bit without a GPU.  Each emu_* is a loop over rays or pixels around the ray_math.h
-// routines that intersect_kernel, stratified_kernel, interval_kernel, sample_pdf_kernel and rays_kernel call.  Two
-// pieces stay written out in both places, because sharing them changes the kernels' SASS: intersect_kernel's
-// per-primitive step (below) and stratified_kernel's interval test (pnr_tag here).
+// routines that intersect_kernel, stratified_kernel, interval_kernel, sample_pdf_kernel, rays_kernel and
+// ray_batch_kernel call.  One piece stays written out in both places: stratified_kernel's interval test (pnr_tag here),
+// because a predicate shared with pnr_tag changes the SASS of pnr_tag's callers.
 // Built by __graft_entry__.build() and tests/host_emu.py with: g++ -O2 -ffp-contract=off -shared -fPIC.
 #include <cstdint>
 #include "../panopticnerf_b200/csrc/ray_math.h"
 
+// primitive b of ray o, read as intersect_kernel reads it: the box as 15 floats and the clamped triangle range
+// (tri_start null: every primitive is a cuboid)
+static void prim_step(const float* o, const float* bc, const float* bh, const float* br, const int32_t* tri_start,
+                      const float* tris, int64_t T, int b, int M, PnrHitList* L) {
+  float q[15];
+  for (int e = 0; e < 3; ++e) { q[e] = bc[b * 3 + e]; q[3 + e] = bh[b * 3 + e]; }
+  for (int e = 0; e < 9; ++e) q[6 + e] = br[b * 9 + e];
+  int k0 = 0, k1 = 0;
+  if (tri_start) pnr_tri_range(tri_start, b, T, &k0, &k1);
+  pnr_prim_step(o[0], o[1], o[2], o[3], o[4], o[5], q, k0, k1, tris, M, b, L);
+}
+
 extern "C" {
 
-// tri_start / tris null (and T = 0): every primitive is a cuboid, as in pnr_intersect
+// intersect_kernel's loop on a sequence table of B primitives (DESIGN 3.2): the static primitives [0, S), then the
+// block of the ray's frame.  ray_frame null (and F = 0): every primitive is static.  No argument checks: the tests
+// pass valid tables.
+void emu_intersect_frames(const float* rays, int64_t R, const float* bc, const float* bh, const float* br,
+                          const int32_t* tri_start, const float* tris, int64_t T, int B, int S,
+                          const int32_t* frame_boxes, int F, const int32_t* ray_frame, int M, uint8_t* hit,
+                          int32_t* box_id, float* t_in, float* t_out) {
+  for (int64_t r = 0; r < R; ++r) {
+    PnrHitList L;
+    pnr_hits_init(&L);
+    for (int b = 0; b < S; ++b) prim_step(rays + r * 6, bc, bh, br, tri_start, tris, T, b, M, &L);
+    int b0, b1;
+    pnr_frame_range(ray_frame ? ray_frame[r] : -1, frame_boxes, F, S, B, &b0, &b1);
+    for (int b = b0; b < b1; ++b) prim_step(rays + r * 6, bc, bh, br, tri_start, tris, T, b, M, &L);
+    pnr_hits_store(&L, M, r, hit, box_id, t_in, t_out);
+  }
+}
+
+// a single table of B primitives, as pnr_intersect / pnr_intersect_meshes
 void emu_intersect(const float* rays, int64_t R, const float* bc, const float* bh, const float* br,
                    const int32_t* tri_start, const float* tris, int64_t T, int B, int M, uint8_t* hit,
                    int32_t* box_id, float* t_in, float* t_out) {
-  for (int64_t r = 0; r < R; ++r) {
-    const float* q = rays + r * 6;
-    PnrHitList L;
-    pnr_hits_init(&L);
-    for (int b = 0; b < B; ++b) {
-      int k0 = 0, k1 = 0;
-      if (tri_start) pnr_tri_range(tri_start, b, T, &k0, &k1);
-      // intersect_kernel's per-primitive step, restated: moved into a shared function, it changes the kernel's SASS
-      float tmin, tmax;
-      if (!pnr_slab(q[0], q[1], q[2], q[3], q[4], q[5], bc + b * 3, bh + b * 3, br + b * 9, &tmin, &tmax)) continue;
-      if (k0 == k1) {
-        pnr_hits_insert(&L, M, tmin, tmax, b);
-        continue;
-      }
-      const PnrShear S = pnr_shear(q[3], q[4], q[5]);
-      PnrMeshCross X;
-      pnr_cross_init(&X);
-      for (int k = k0; k < k1; ++k) {
-        float t;
-        if (pnr_tri_cross(q[0], q[1], q[2], S, tris + (int64_t)k * 9, &t)) pnr_cross_add(&X, M, t);
-      }
-      pnr_cross_emit(&X, &L, M, b);
-    }
-    pnr_hits_store(&L, M, r, hit, box_id, t_in, t_out);
-  }
+  emu_intersect_frames(rays, R, bc, bh, br, tri_start, tris, T, B, B, nullptr, 0, nullptr, M, hit, box_id, t_in,
+                       t_out);
 }
 
 void emu_stratified(const float* near, const float* far, const float* t_vals, const float* u, int64_t R, int N,
@@ -106,4 +113,17 @@ int emu_generate_rays(int H, int W, int row0, int rows, int camera, const float*
   }
   return 0;
 }
+
+// ray_batch_kernel's loop over pnr_ray_batch_row: rows r0 .. r1-1 with host pointers (no argument checks: the tests
+// pass valid sets)
+void emu_sample_ray_batch(const pnr_ray_batch_args* a) {
+  for (int64_t r = a->r0; r < a->r1; ++r) pnr_ray_batch_row(*a, a->pix_offset, r);
+}
+
+// one Philox4x32-10 block
+void emu_philox4x32_10(const uint32_t* ctr, const uint32_t* key, uint32_t* out) {
+  pnr_philox4x32_10(ctr[0], ctr[1], ctr[2], ctr[3], key[0], key[1], out);
+}
+
+uint64_t emu_mulhi64(uint64_t a, uint64_t b) { return pnr_mulhi64(a, b); }
 }

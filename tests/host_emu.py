@@ -14,4 +14,7 @@ def emu():
     out.parent.mkdir(exist_ok=True)
     subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
                            str(ROOT / "tests" / "host_emu.cpp")])
-    return C.CDLL(str(out))
+    lib = C.CDLL(str(out))
+    lib.emu_mulhi64.argtypes = [C.c_uint64, C.c_uint64]
+    lib.emu_mulhi64.restype = C.c_uint64
+    return lib

@@ -1,31 +1,12 @@
 """numpy restatement of pnr_sample_ray_batch's draws (include/pnr.h): Philox4x32-10, the 64-bit multiply-high pixel
 pick, the frame search and the jitter words; plus helpers that build frame sets and call the host build of
-pnr_ray_batch_row (tests/host_emu_ray_batch.cpp, fixture `emu_rb`).  Shared by the CPU and GPU ray-batch tests."""
+pnr_ray_batch_row (tests/host_emu.cpp, fixture `emu` of tests/host_emu.py).  Shared by the CPU and GPU ray-batch
+tests."""
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
-import pytest
 
 from panopticnerf_b200 import _capi
-
-ROOT = Path(__file__).resolve().parent.parent
-
-
-@pytest.fixture(scope="session")
-def emu_rb():
-    """The host build of the ray-batch routine (tests/host_emu_ray_batch.cpp)."""
-    out = ROOT / "build" / "host_emu_ray_batch.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu_ray_batch.cpp")])
-    lib = C.CDLL(str(out))
-    lib.emu_sample_ray_batch.argtypes = [C.POINTER(_capi.PnrRayBatchArgs)]
-    lib.emu_sample_ray_batch.restype = None
-    lib.emu_mulhi64.argtypes = [C.c_uint64, C.c_uint64]
-    lib.emu_mulhi64.restype = C.c_uint64
-    return lib
 
 MASK = np.uint64(0xFFFFFFFF)
 
@@ -117,7 +98,7 @@ def fill_args(a, fs, seed, step, r0, r1, N, Ni, ptr):
     return a
 
 
-def host_batch(emu_rb, fs, seed, step, r0, r1, N, Ni):
+def host_batch(emu, fs, seed, step, r0, r1, N, Ni):
     """The host build's rows r0 .. r1-1 (numpy outputs; depth / pseudo_label / pixel always written)."""
     n = r1 - r0
     out = dict(rays=np.zeros((n, 6), np.float32), rgb=np.zeros((n, 3), np.float32), u=np.zeros((n, N), np.float32),
@@ -135,7 +116,7 @@ def host_batch(emu_rb, fs, seed, step, r0, r1, N, Ni):
     a.rays, a.rgb, a.u = out["rays"].ctypes.data, out["rgb"].ctypes.data, out["u"].ctypes.data
     a.u_fine = out["u_fine"].ctypes.data if Ni else None
     a.depth_out, a.pseudo_label, a.pixel = out["depth"].ctypes.data, out["pseudo_label"].ctypes.data, out["pixel"].ctypes.data
-    emu_rb.emu_sample_ray_batch(C.byref(a))
+    emu.emu_sample_ray_batch(C.byref(a))
     return out
 
 

@@ -1,30 +1,12 @@
 """Oracle of a5 on a sequence table (DESIGN 3.2, include/pnr.h pnr_intersect_frames): the rays of each frame are
 intersected with that frame's own table cat(static, block) by any single-table intersection (the torch oracle, the host
 build, the device kernel), and the dynamic ids are mapped back to the sequence table (seq_id = id + begin - S).  Also a
-random sequence table, the per-frame tables the renderer tests compare against, and the host build of
-pnr_intersect_frames (tests/host_emu_sequence.cpp, fixture `emu_seq`)."""
+random sequence table and the per-frame tables the renderer tests compare against."""
 from __future__ import annotations
 
-import ctypes as C
-import subprocess
-from pathlib import Path
-
-import pytest
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-
 PRIM_KEYS = ("box_center", "box_half", "box_rot", "box_sem", "box_inst")
-
-
-@pytest.fixture(scope="session")
-def emu_seq():
-    """The host build of pnr_intersect_frames (tests/host_emu_sequence.cpp)."""
-    out = ROOT / "build" / "host_emu_sequence.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu_sequence.cpp")])
-    return C.CDLL(str(out))
 
 
 def frame_range(f: int, frame_boxes, F: int, S: int, B: int):

@@ -1,5 +1,5 @@
 """CPU tier of training ray batches: the numpy Philox4x32-10 against Random123's known answers; the host build of
-pnr_ray_batch_row (tests/host_emu_ray_batch.cpp) against the numpy oracle bit for bit (pixels, frames, colours,
+pnr_ray_batch_row (tests/host_emu.cpp) against the numpy oracle bit for bit (pixels, frames, colours,
 targets, u, u_fine, and rays against the host build of pnr_generate_rays); the 64-bit multiply-high; the KITTI-360
 frame reader on fixtures written here in the documented layouts, and each refusal by name; the argument refusals of
 pnr_sample_ray_batch before any device call; and pnr_ray_batch_args' layout against a C compile of include/pnr.h."""
@@ -12,8 +12,7 @@ import pytest
 import torch
 
 import oracle_ray_batch as O
-from host_emu import emu  # noqa: F401  (session fixture: the host build of pnr_generate_rays)
-from oracle_ray_batch import emu_rb  # noqa: F401  (session fixture: the host build of the ray-batch routine)
+from host_emu import emu  # noqa: F401  (session fixture: the host build of ray_math.h)
 from panopticnerf_b200 import _capi
 
 ROOT = Path(__file__).resolve().parent.parent
@@ -27,28 +26,28 @@ KAT = [((0, 0, 0, 0), (0, 0), (0x6627e8d5, 0xe169c58d, 0xbc57ac4c, 0x9b00dbd8)),
 
 
 @pytest.mark.parametrize("ctr,key,want", KAT)
-def test_philox_known_answers(ctr, key, want, emu_rb):
+def test_philox_known_answers(ctr, key, want, emu):
     got = [int(x) for x in O.philox4x32_10(*ctr, *key)]
     assert got == list(want)
     c, k, out = (C.c_uint32 * 4)(*ctr), (C.c_uint32 * 2)(*key), (C.c_uint32 * 4)()
-    emu_rb.emu_philox4x32_10(c, k, out)
+    emu.emu_philox4x32_10(c, k, out)
     assert list(out) == list(want)
 
 
 @pytest.mark.parametrize("P", [1, 2, (1 << 32) - 1, 1 << 32, (1 << 32) + 1, 1 << 40, (1 << 31) + 3, (1 << 62) + 7])
-def test_mulhi64(P, emu_rb):
+def test_mulhi64(P, emu):
     rng = np.random.default_rng(P % 1000)
     xs = [0, 1, (1 << 32) - 1, 1 << 32, (1 << 63), (1 << 64) - 1] + [int(v) for v in rng.integers(0, 1 << 63, 64)]
     for x in xs:
         want = (x * P) >> 64
-        assert emu_rb.emu_mulhi64(x, P) == want
+        assert emu.emu_mulhi64(x, P) == want
         assert 0 <= want < P
-    assert emu_rb.emu_mulhi64((1 << 64) - 1, P) == P - 1
+    assert emu.emu_mulhi64((1 << 64) - 1, P) == P - 1
 
 
 # ------------------------------------------------------------------------------------------------ host build vs oracle
-def _check_rows(emu, emu_rb, fs, seed, step, r0, r1, N, Ni):
-    got = O.host_batch(emu_rb, fs, seed, step, r0, r1, N, Ni)
+def _check_rows(emu, fs, seed, step, r0, r1, N, Ni):
+    got = O.host_batch(emu, fs, seed, step, r0, r1, N, Ni)
     r = np.arange(r0, r1, dtype=np.int64)
     off, P = fs["pix_offset"], int(fs["pix_offset"][-1])
     p = O.pixels(seed, step, r, P)
@@ -75,15 +74,15 @@ def _check_rows(emu, emu_rb, fs, seed, step, r0, r1, N, Ni):
 @pytest.mark.parametrize("F,ncam,N,Ni,label,depth", [
     (1, 1, 1, 0, False, False), (3, 2, 64, 128, True, True), (17, 4, 7, 5, True, False), (60, 3, 32, 0, False, True),
     (200, 4, 3, 253, True, True)])
-def test_host_build_equals_the_oracle(F, ncam, N, Ni, label, depth, emu, emu_rb):
+def test_host_build_equals_the_oracle(F, ncam, N, Ni, label, depth, emu):
     rng = np.random.default_rng(F * 7 + ncam)
     fs = O.random_frame_set(rng, F, O.random_cameras(rng, ncam, tiny=ncam == 4), label, depth)
     seed, step = int(rng.integers(0, 1 << 63)) * 2 + 1, (1 << 33) + F
-    _check_rows(emu, emu_rb, fs, seed, step, 0, 700, N, Ni)
-    _check_rows(emu, emu_rb, fs, seed, step, 1 << 31, (1 << 31) + 100, N, Ni)   # ray indices past int32: 32-bit words
+    _check_rows(emu, fs, seed, step, 0, 700, N, Ni)
+    _check_rows(emu, fs, seed, step, 1 << 31, (1 << 31) + 100, N, Ni)   # ray indices past int32: 32-bit words
 
 
-def test_frame_boundaries_and_one_pixel_frames(emu, emu_rb):
+def test_frame_boundaries_and_one_pixel_frames(emu):
     """A set of one-pixel frames between larger ones: every frame, its first and its last pixel are drawn, and each
     sits in the frame that owns it."""
     rng = np.random.default_rng(5)
@@ -96,20 +95,20 @@ def test_frame_boundaries_and_one_pixel_frames(emu, emu_rb):
     fs["pix_offset"] = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
     P = int(fs["pix_offset"][-1])
     fs["rgb8"], fs["label"], fs["depth"] = fs["rgb8"][:P], fs["label"][:P], fs["depth"][:P]
-    got, f = _check_rows(emu, emu_rb, fs, 11, 3, 0, 4000, 4, 4)
+    got, f = _check_rows(emu, fs, 11, 3, 0, 4000, 4, 4)
     assert set(f.tolist()) == set(range(24))
     assert {int(x) for x in fs["pix_offset"][:-1]} <= set(got["pixel"].tolist())
     assert {int(x) - 1 for x in fs["pix_offset"][1:]} <= set(got["pixel"].tolist())
 
 
-def test_a_range_is_the_rows_of_the_whole_batch(emu_rb):
+def test_a_range_is_the_rows_of_the_whole_batch(emu):
     rng = np.random.default_rng(9)
     fs = O.random_frame_set(rng, 12, O.random_cameras(rng, 2))
-    whole = O.host_batch(emu_rb, fs, 3, 4, 0, 600, 10, 6)
-    part = O.host_batch(emu_rb, fs, 3, 4, 255, 513, 10, 6)
+    whole = O.host_batch(emu, fs, 3, 4, 0, 600, 10, 6)
+    part = O.host_batch(emu, fs, 3, 4, 255, 513, 10, 6)
     for k in whole:
         assert np.array_equal(part[k], whole[k][255:513]), k
-    other = O.host_batch(emu_rb, fs, 3, 5, 0, 600, 10, 6)                  # another step draws other pixels
+    other = O.host_batch(emu, fs, 3, 5, 0, 600, 10, 6)                  # another step draws other pixels
     assert not np.array_equal(other["pixel"], whole["pixel"])
 
 

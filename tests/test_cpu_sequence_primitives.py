@@ -1,5 +1,5 @@
 """CPU tier of sequence tables (DESIGN 3.2): kitti360.sequence_primitives on a synthetic annotation file; the host build of
-pnr_intersect_frames (tests/host_emu_sequence.cpp) against the per-frame oracle (tests/oracle_sequence.py
+pnr_intersect_frames (tests/host_emu.cpp) against the per-frame oracle (tests/oracle_sequence.py
 over tests/oracle_mesh.py) bit for bit, with empty, shared, clamped and out-of-range frames, ties, overflowing lists
 and meshes in the dynamic blocks; the argument refusals of pnr_intersect_frames and pnr_render_fused_frames (before
 any CUDA call: the pointers are placeholders that are never dereferenced); the ctypes layouts against the header; and
@@ -15,7 +15,7 @@ import torch
 
 import oracle_mesh as OM
 import oracle_sequence as OS
-from oracle_sequence import emu_seq  # noqa: F401  (fixture)
+from host_emu import emu  # noqa: F401  (fixture)
 from panopticnerf_b200 import _capi, make_cfg, parallel, synthetic as S
 from panopticnerf_b200.lib.datasets import kitti360 as K
 
@@ -104,17 +104,17 @@ def test_sequence_table_with_meshes_keeps_each_primitives_triangles(tmp_path):
 
 
 # ------------------------------------------------------------------------------------------ host build vs oracle
-def emu_frames(emu_seq, rays, prims, S, fb, rf, M):
+def emu_frames(emu, rays, prims, S, fb, rf, M):
     R, B = rays.shape[0], prims["box_center"].shape[0]
     hit = torch.zeros(R, dtype=torch.uint8)
     bid = torch.zeros(R, M, dtype=torch.int32)
     tin, tout = torch.zeros(R, M), torch.zeros(R, M)
     mesh = prims.get("mesh_tri_start")
     tris = prims["mesh_tris"].contiguous() if mesh is not None else None
-    emu_seq.emu_intersect_frames(_p(rays), C.c_int64(R), _p(prims["box_center"]), _p(prims["box_half"]),
-                                 _p(prims["box_rot"]), _p(mesh), _p(tris),
-                                 C.c_int64(tris.shape[0] if mesh is not None else 0), B, S, _p(fb), fb.shape[0], _p(rf),
-                                 M, _p(hit), _p(bid), _p(tin), _p(tout))
+    emu.emu_intersect_frames(_p(rays), C.c_int64(R), _p(prims["box_center"]), _p(prims["box_half"]),
+                             _p(prims["box_rot"]), _p(mesh), _p(tris),
+                             C.c_int64(tris.shape[0] if mesh is not None else 0), B, S, _p(fb), fb.shape[0], _p(rf),
+                             M, _p(hit), _p(bid), _p(tin), _p(tout))
     return hit.bool(), bid, tin, tout
 
 
@@ -135,7 +135,7 @@ def _rays(n, seed):
 
 
 @pytest.mark.parametrize("S_,M", [(0, 4), (20, 1), (40, 4), (64, 8)])
-def test_random_frames_match_the_per_frame_oracle(emu_seq, S_, M):
+def test_random_frames_match_the_per_frame_oracle(emu, S_, M):
     prims = S.make_boxes(160, seed=S_)
     F = 12
     fb = OS.random_sequence(prims, S_, F, 40, seed=S_, shared=3)
@@ -147,7 +147,7 @@ def test_random_frames_match_the_per_frame_oracle(emu_seq, S_, M):
     rf = torch.randint(-1, F + 1, (rays.shape[0],), generator=torch.Generator().manual_seed(7), dtype=torch.int32)
     assert bool((rf == -1).any()) and bool((rf == F).any())            # out of range: static only
     ref = OS.per_frame(oracle_one, rays, prims, S_, fb, rf, M)
-    got = emu_frames(emu_seq, rays, prims, S_, fb, rf, M)
+    got = emu_frames(emu, rays, prims, S_, fb, rf, M)
     assert_same(got, ref)
     assert bool((got[1] >= S_).any()), "no ray reached a dynamic box"
     if M < 8:
@@ -156,13 +156,13 @@ def test_random_frames_match_the_per_frame_oracle(emu_seq, S_, M):
     assert bool((got[1][out] < S_).all())
 
 
-def test_a_static_and_a_dynamic_box_tied_at_t_in_keep_the_static_first(emu_seq):
+def test_a_static_and_a_dynamic_box_tied_at_t_in_keep_the_static_first(emu):
     bx = S.make_boxes(8, seed=2)
     prims = {k: torch.cat([v, v[:3]]).contiguous() for k, v in bx.items()}   # dynamic 8..10 copy static 0..2
     fb = torch.tensor([[8, 11]], dtype=torch.int32)
     rays = _rays(4000, 2)
     rf = torch.zeros(rays.shape[0], dtype=torch.int32)
-    got = emu_frames(emu_seq, rays, prims, 8, fb, rf, 8)
+    got = emu_frames(emu, rays, prims, 8, fb, rf, 8)
     assert_same(got, OS.per_frame(oracle_one, rays, prims, 8, fb, rf, 8))
     ids, tin = got[1], got[2]
     tied = 0
@@ -176,7 +176,7 @@ def test_a_static_and_a_dynamic_box_tied_at_t_in_keep_the_static_first(emu_seq):
     assert tied > 20
 
 
-def test_meshes_in_a_dynamic_block(emu_seq):
+def test_meshes_in_a_dynamic_block(emu):
     prims = S.make_mesh_primitives(seed=1)          # 64 cuboids, then the meshes 64..68
     B = prims["box_center"].shape[0]
     fb = torch.tensor([[40, B], [60, 66], [64, 64], [66, B]], dtype=torch.int32)
@@ -184,17 +184,17 @@ def test_meshes_in_a_dynamic_block(emu_seq):
     rf = torch.arange(rays.shape[0], dtype=torch.int32) % 5 - 1           # -1 .. 3
     for M in (2, 8):
         ref = OS.per_frame(oracle_one, rays, prims, 40, fb, rf, M)
-        got = emu_frames(emu_seq, rays, prims, 40, fb, rf, M)
+        got = emu_frames(emu, rays, prims, 40, fb, rf, M)
         assert_same(got, ref)
         assert bool((got[1] >= 64).any()), "no ray reached a mesh"
 
 
-def test_without_frames_it_is_the_static_kernel(emu_seq):
+def test_without_frames_it_is_the_static_kernel(emu):
     prims = S.make_mesh_primitives(seed=3)
     B = prims["box_center"].shape[0]
     rays = _rays(1500, 3)
     rf = torch.zeros(rays.shape[0], dtype=torch.int32)
-    got = emu_frames(emu_seq, rays, prims, B, torch.tensor([[B, B]], dtype=torch.int32), rf, 4)
+    got = emu_frames(emu, rays, prims, B, torch.tensor([[B, B]], dtype=torch.int32), rf, 4)
     assert_same(got, oracle_one(rays, prims, 4))
 
 

@@ -12,7 +12,7 @@ import pytest
 import torch
 
 import oracle_ray_batch as O
-from oracle_ray_batch import emu_rb  # noqa: F401  (session fixture: the host build of the ray-batch routine)
+from host_emu import emu  # noqa: F401  (session fixture: the host build of ray_math.h)
 import panopticnerf_b200 as PN
 from panopticnerf_b200 import parallel, synthetic as S
 from panopticnerf_b200.lib.datasets.ray_batch import Camera, FrameSet, RaySampler, sample_ray_batch
@@ -41,13 +41,13 @@ CASES = [(1, 1, False, False, 1), (1, 2, True, True, 255), (7, 3, True, False, 2
 
 
 @pytest.mark.parametrize("F,ncam,label,depth,R", CASES)
-def test_kernel_equals_the_host_build(F, ncam, label, depth, R, emu_rb):
+def test_kernel_equals_the_host_build(F, ncam, label, depth, R, emu):
     rng = np.random.default_rng(F + R)
     fs = O.random_frame_set(rng, F, O.random_cameras(rng, ncam, tiny=ncam >= 3), label, depth)
     N, Ni = (64, 128) if R == 1 << 20 else (int(rng.integers(1, 40)), int(rng.integers(0, 30)))
     seed, step = int(rng.integers(0, 1 << 62)), int(rng.integers(0, 1 << 40))
     got = sample_ray_batch(device_set(fs), seed, step, 0, R, N, Ni, want_pixel=True)
-    want = O.host_batch(emu_rb, fs, seed, step, 0, R, N, Ni)
+    want = O.host_batch(emu, fs, seed, step, 0, R, N, Ni)
     assert set(got) == {"rays", "rgb", "u", "pixel"} | ({"u_fine"} if Ni else set()) | \
         ({"depth"} if depth else set()) | ({"pseudo_label"} if label else set())
     for k, v in got.items():

@@ -11,7 +11,7 @@ import torch
 
 import oracle_ray_batch as ORB
 import oracle_sequence as OS
-from oracle_sequence import emu_seq  # noqa: F401  (fixture)
+from host_emu import emu  # noqa: F401  (fixture)
 from panopticnerf_b200 import _capi, make_cfg, make_network, make_renderer, synthetic as S
 from panopticnerf_b200.lib.datasets import kitti360 as K
 from panopticnerf_b200.lib.datasets.kitti360.bboxes import Box3D
@@ -44,7 +44,7 @@ def _gpu_one(rays, table, M):
 # ------------------------------------------------------------------------------------------------ kernel
 @pytest.mark.parametrize("meshes", [False, True])
 @pytest.mark.parametrize("S_,M", [(511, 1), (512, 4), (513, 8), (2000, 8)])
-def test_kernel_equals_the_per_frame_tables_and_the_host_build(S_, M, meshes, emu_seq):
+def test_kernel_equals_the_per_frame_tables_and_the_host_build(S_, M, meshes, emu):
     F, pool = 300, 1500
     prims = S.make_mesh_primitives(num_boxes=S_ + pool - 5, seed=S_) if meshes else S.make_boxes(S_ + pool, seed=S_)
     B = prims["box_center"].shape[0]
@@ -65,7 +65,7 @@ def test_kernel_equals_the_per_frame_tables_and_the_host_build(S_, M, meshes, em
     if meshes and M > 1 and S_ < 1000:   # with one slot, or 2000 static boxes in front, the nearest hits are cuboids
         assert bool((got[1] >= B - 5).any()), "no ray reached a mesh in a dynamic block"
     sub = torch.randperm(R, generator=torch.Generator().manual_seed(1))[:8192].to(DEV)
-    host = emu_frames(emu_seq, rays[sub].cpu().contiguous(), prims, S_, fb, rf[sub].cpu().contiguous(), M)
+    host = emu_frames(emu, rays[sub].cpu().contiguous(), prims, S_, fb, rf[sub].cpu().contiguous(), M)
     for a, b, k in zip(got, host, ("hit_mask", "box_id", "t_in", "t_out")):
         _bits(a[sub].cpu(), b, f"S={S_} host {k}")
 
