@@ -352,6 +352,34 @@ int pnr_hashgrid_encode(const float* x, int64_t n, const float* aabb, const floa
 int pnr_hashgrid_backward(const float* x, int64_t n, const float* aabb, const float* grad_out, int32_t L, int32_t F,
                           int32_t T_log2, float base_resolution, float per_level_scale, float* grad_table, void* stream);
 
+/* The same gradient, reproducible bit for bit: a fixed-point sum that does not depend on the order of the points, the
+ * launch or the GPU.  Same arguments as pnr_hashgrid_backward, plus a workspace; ACCUMULATES into grad_table.  For a
+ * call over n > 0 points, level l, entry e of that level and feature f:
+ *   1. Scale.  m_l = the largest finite |grad_out[p, l*F + f]| over all p and f; m_l = frac * 2^e_l with frac in
+ *      [0.5, 1) (frexp); s_l = 61 - ceil(log2 n) - e_l.  A level with m_l = 0 adds nothing.
+ *   2. Contribution of corner k of point p (w_k and the row idx from the forward's corner arithmetic):
+ *      c = fp32(w_k * g), g = grad_out[p, l*F + f] (the product the atomic path makes);
+ *      q = round-to-nearest-even((double)c * 2^s_l) as an int64 (the product is exact in double).
+ *   3. Sum.  acc[l, e, f] = sum of q over the contributions to (l, e, f), in int64: exact, in any order.
+ *   4. Result.  grad_table[l, e, f] += fp32((double)acc * 2^-s_l): int64 -> double (round to nearest), the exact
+ *      product with the power of two, double -> float (round to nearest), then one fp32 add.
+ *   5. Non-finite gradients.  A non-finite g at (p, l, f) is left out of m_l and of the sums; it sets the (l, idx_k, f)
+ *      entries of all 8 of p's corners to NaN.  Every other entry is the rule applied to the finite contributions.
+ * Overflow cannot happen: a point's 8 corner weights sum to at most 1 + 2^-20, |c| * 2^s_l <= |w_k| m_l (1 + 2^-24)
+ * 2^s_l and m_l 2^s_l < 2^(61 - ceil(log2 n)) <= 2^61 / n, so the absolute sum of every quantized contribution of a
+ * level - a fortiori of one entry - stays below 2^61 (1 + 2^-20) + 4n < 2^63 (each rounding adds at most 1/2).
+ * Error against float64: 2^-24 |w_k g| + 2^-(s_l + 1) per contribution (at n = 2^19 the quantum 2^-s_l is at most
+ * 2^-42 m_l), then the final two roundings of each entry.
+ * workspace: pnr_hashgrid_fixed_workspace_bytes(L, F, T_log2) bytes of device scratch, 16-byte aligned, zeroed by the
+ * call: int64 acc [L, 2^T_log2, F], one poison bit per entry (in 16-byte units), u32 max_bits [L], i32 scale [L],
+ * u32 flags [2], rounded up to 16 bytes.  A short or misaligned workspace is refused before any launch.  The host
+ * reads nothing back: the call can be captured in a CUDA graph.  pnr_hashgrid_fixed_workspace_bytes returns 0 for an
+ * L, F or T_log2 the call refuses. */
+size_t pnr_hashgrid_fixed_workspace_bytes(int32_t L, int32_t F, int32_t T_log2);
+int pnr_hashgrid_backward_fixed(const float* x, int64_t n, const float* aabb, const float* grad_out, int32_t L,
+                                int32_t F, int32_t T_log2, float base_resolution, float per_level_scale,
+                                float* grad_table, void* workspace, size_t workspace_bytes, void* stream);
+
 /* a8 + a9 in ONE kernel: Network.forward with the compositing done in the MLP's epilogue - per-sample alpha /
  * transmittance / weight right after the sigma-producing layer, colours and logits reduced on chip per ray - so the
  * network outputs `raw` [R,N,4+C+K] (456 B per sample with both heads) are never written to memory; only

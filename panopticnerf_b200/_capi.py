@@ -149,6 +149,9 @@ SIGNATURES = {
     "pnr_panoptic_fuse": (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "pnr_hashgrid_encode": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, C.c_float, C.c_float, _vp, _vp]),
     "pnr_hashgrid_backward": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, C.c_float, C.c_float, _vp, _vp]),
+    "pnr_hashgrid_fixed_workspace_bytes": (C.c_size_t, [_i32, _i32, _i32]),
+    "pnr_hashgrid_backward_fixed": (C.c_int, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, C.c_float, C.c_float, _vp, _vp,
+                                              C.c_size_t, _vp]),
     "pnr_label_tiles": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "pnr_composite_backward": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
                                          _i32, C.POINTER(PnrCompositeGrads), _vp, _vp]),

@@ -21,6 +21,9 @@ _DEFAULTS = dict(
     # 360 architecture is not in the mount).  hash_aabb [lo.xyz, hi.xyz] is required with "hashgrid".
     xyz_encoding="frequency", hash_levels=16, hash_features=2, hash_log2_size=19,
     hash_base_resolution=16.0, hash_per_level_scale=1.3819, hash_aabb=None,
+    # the hash table's gradient: "atomic" = pnr_hashgrid_backward (fp32 atomics, the last bits vary between runs) |
+    # "fixed" = pnr_hashgrid_backward_fixed (a fixed-point sum: every run gives the same bits)
+    hash_grad="atomic",
     # sampling / rendering (a5, a6, a9, a10)
     N_samples=64, N_importance=0, perturb=0.0, white_bkgd=False, raw_noise_std=0.0,
     near=0.05, far=80.0, max_hits=4, bound_by_primitives=False, mask_outside=False,

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
+#include <algorithm>
 #include "../../include/pnr.h"
 #include "common.cuh"
 #include "hashgrid_math.cuh"
@@ -168,6 +169,193 @@ __global__ void __launch_bounds__(256) hashgrid_backward_kernel(HashArgs a, cons
   }
 }
 
+// ---------------------------------------------------------------------------- hash grid, fixed-point table gradient
+// pnr_hashgrid_backward_fixed (rule: include/pnr.h).  Every contribution w_k * g is rounded once to an int64 at the
+// level's power-of-two scale 2^s_l and summed with integer atomics, which are associative: the result does not depend
+// on the order of the points, the launch or the GPU.  Three kernels: the level maxima (and s_l), the scatter, and the
+// finalize that turns the integer sums into fp32 and adds them to grad_table.
+//
+// Warp combining in the scatter: the lanes of a warp whose corner falls in the same row sum their integers first
+// (one atomic per distinct row and feature).  Integer sums, so the result is the same bit for bit either way;
+// PNR_HASH_FIXED_COMBINE=0 builds the plain scatter (tools/time_hashgrid_backward.py times both).
+#ifndef PNR_HASH_FIXED_COMBINE
+#define PNR_HASH_FIXED_COMBINE 1
+#endif
+
+constexpr int32_t kNoScale = INT32_MIN;   // scale of a level whose finite gradients are all zero: it adds nothing
+constexpr int kFixedMaxBlocks = 2048;
+
+// The workspace, in this order: int64 acc [L, T, F]; u32 poison bits, one per (l, e, f) entry, in 16-byte units;
+// u32 max_bits [L] (|g| of the largest finite gradient of the level, as fp32 bits); i32 scale [L]; u32 flags [2]
+// (any non-finite gradient, blocks done); the whole rounded up to 16 bytes.
+struct FixedLayout {
+  size_t acc, poison, max_bits, scale, flags, total;
+  FixedLayout(int L, int F, int T_log2) {
+    const size_t entries = (size_t)L * F << T_log2;
+    acc = 0;
+    poison = entries * sizeof(int64_t);
+    max_bits = poison + ((entries + 31) / 32 * 4 + 15) / 16 * 16;
+    scale = max_bits + (size_t)L * 4;
+    flags = scale + (size_t)L * 4;
+    total = (flags + 8 + 15) / 16 * 16;
+  }
+};
+
+struct FixedWs {
+  int64_t* acc; uint32_t* poison; uint32_t* max_bits; int32_t* scale; uint32_t* flags;
+};
+
+__device__ __forceinline__ double pow2d(int e) {            // 2^e, exact, for |e| <= 1022
+  return __longlong_as_double((long long)(e + 1023) << 52);
+}
+
+// e of frexp(m) = frac * 2^e, frac in [0.5, 1), for a positive finite fp32 m given by its bits (subnormals included)
+__device__ __forceinline__ int frexp_exponent(uint32_t bits) {
+  const uint32_t E = bits >> 23;
+  return E ? (int)E - 126 : 32 - __clz(bits) - 149;
+}
+
+// m_l = max |grad_out[p, l*F + f]| over the finite values, as fp32 bits (for non-negative floats the bit patterns order
+// like the values, so atomicMax on them is the max in any order); flags[0] = 1 when any value is non-finite.  The
+// grid stride is a multiple of the row width W = L*F, so each thread stays on one column.  The last block to finish
+// derives s_l = 61 - ceil(log2 n) - e_l from the maxima.
+__global__ void __launch_bounds__(256) hashgrid_fixed_maxima_kernel(const float* __restrict__ g, int64_t total, int W,
+                                                                    int F, int L, int clog2n, FixedWs w) {
+  __shared__ uint32_t smax[kHashMaxLevels];
+  __shared__ int sbad;
+  __shared__ bool last;
+  if (threadIdx.x < kHashMaxLevels) smax[threadIdx.x] = 0;
+  if (threadIdx.x == 0) sbad = 0;
+  __syncthreads();
+  const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x / W * W;
+  if (tid < stride) {
+    uint32_t m = 0;
+    bool bad = false;
+#pragma unroll 4
+    for (int64_t i = tid; i < total; i += stride) {
+      const uint32_t b = __float_as_uint(g[i]) & 0x7fffffffu;
+      if (b >= 0x7f800000u) bad = true;
+      else m = max(m, b);
+    }
+    if (m) atomicMax(&smax[(int)(tid % W) / F], m);
+    if (bad) sbad = 1;
+  }
+  __syncthreads();
+  if (threadIdx.x < L && smax[threadIdx.x]) atomicMax(&w.max_bits[threadIdx.x], smax[threadIdx.x]);
+  if (threadIdx.x == 0 && sbad) atomicOr(&w.flags[0], 1u);
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(&w.flags[1], 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (last && threadIdx.x < L) {
+    __threadfence();
+    const uint32_t mb = atomicOr(&w.max_bits[threadIdx.x], 0u);
+    w.scale[threadIdx.x] = mb ? 61 - clog2n - frexp_exponent(mb) : kNoScale;
+  }
+}
+
+// Sends one corner's F integers (and the F poison bits of its non-finite gradients) to row idx of the level.
+template <int F>
+__device__ __forceinline__ void fixed_emit(int64_t* __restrict__ acc, uint32_t* __restrict__ poison, size_t row,
+                                           const long long (&q)[F], uint32_t bad, bool live) {
+  const size_t b0 = row * F;                                  // first poison bit of the row: its F bits share a word
+#if PNR_HASH_FIXED_COMBINE
+  const unsigned lane = threadIdx.x & 31u;
+  const unsigned grp = __match_any_sync(0xffffffffu, live ? (unsigned)row : 0xffffffffu);
+  if (grp == (1u << lane)) {
+    if (!live) return;
+#pragma unroll
+    for (int f = 0; f < F; ++f)
+      if (q[f]) atomicAdd(reinterpret_cast<unsigned long long*>(acc) + b0 + f, (unsigned long long)q[f]);
+    if (bad) atomicOr(poison + (b0 >> 5), bad << (b0 & 31));
+    return;
+  }
+  // the group's sum mod 2^64 from three 22-bit limbs (each limb's sum over <= 32 lanes stays below 2^27)
+  const bool leader = (unsigned)(__ffs(grp) - 1) == lane;
+#pragma unroll
+  for (int f = 0; f < F; ++f) {
+    const unsigned long long u = (unsigned long long)q[f];
+    const unsigned s0 = __reduce_add_sync(grp, (unsigned)(u & 0x3fffffu));
+    const unsigned s1 = __reduce_add_sync(grp, (unsigned)((u >> 22) & 0x3fffffu));
+    const unsigned s2 = __reduce_add_sync(grp, (unsigned)(u >> 44));
+    const unsigned long long t = (unsigned long long)s0 + ((unsigned long long)s1 << 22) + ((unsigned long long)s2 << 44);
+    if (leader && live && t) atomicAdd(reinterpret_cast<unsigned long long*>(acc) + b0 + f, t);
+  }
+  const uint32_t bm = __reduce_or_sync(grp, bad);
+  if (leader && live && bm) atomicOr(poison + (b0 >> 5), bm << (b0 & 31));
+#else
+  if (!live) return;
+#pragma unroll
+  for (int f = 0; f < F; ++f)
+    if (q[f]) atomicAdd(reinterpret_cast<unsigned long long*>(acc) + b0 + f, (unsigned long long)q[f]);
+  if (bad) atomicOr(poison + (b0 >> 5), bad << (b0 & 31));
+#endif
+}
+
+// The scatter: hashgrid_backward_kernel's thread layout (one point x 8/F levels) and corner arithmetic; contribution
+// c = fp32(w_k * g), q = round-to-nearest-even(c * 2^s_l) as an int64, acc[l, idx, f] += q.  A non-finite g sets the
+// poison bits of its (l, idx_k, f) at all 8 corners instead.  Lanes past n stay in the loop (as dead lanes) so that a
+// warp's combining sees all 32 lanes.
+template <int F>
+__global__ void __launch_bounds__(256) hashgrid_fixed_scatter_kernel(HashArgs a, const float* __restrict__ gout, FixedWs w) {
+  constexpr int LPT = 8 / F;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int l0 = blockIdx.y * LPT;
+  const bool live = i < a.n;
+#if !PNR_HASH_FIXED_COMBINE
+  if (!live) return;
+#endif
+  const uint32_t T = 1u << a.T_log2, mask = T - 1u;
+  float v[3] = {0.f, 0.f, 0.f};
+  if (live) {
+    const float x[3] = {a.x[i * 3], a.x[i * 3 + 1], a.x[i * 3 + 2]};
+    hash_normalize(x, a.aabb, v);
+  }
+  const float* go = gout + (live ? i : 0) * (int64_t)(a.L * F);
+#pragma unroll
+  for (int ll = 0; ll < LPT; ++ll) {
+    const int l = l0 + ll;
+    if (l >= a.L) break;
+    const int32_t s = w.scale[l];
+    const double up = s == kNoScale ? 0.0 : pow2d(s);      // kNoScale: every finite g of the level is 0
+    const uint32_t res = a.res[l], res1 = res + 1u;
+    const bool dense = (uint64_t)res1 * res1 * res1 <= (uint64_t)T;
+    float wv[3], g[F];
+    uint32_t c[3], bad = 0;
+#pragma unroll
+    for (int f = 0; f < F; ++f) {
+      g[f] = live ? go[l * F + f] : 0.f;
+      if (!isfinite(g[f])) { bad |= 1u << f; g[f] = 0.f; }
+    }
+    hash_cell(v, res, c, wv);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      uint32_t idx;
+      const float wk = hash_corner(c, wv, k, res1, dense, mask, idx);
+      long long q[F];
+#pragma unroll
+      for (int f = 0; f < F; ++f) q[f] = __double2ll_rn(__dmul_rn((double)__fmul_rn(wk, g[f]), up));
+      fixed_emit<F>(w.acc, w.poison, (size_t)l * T + idx, q, bad, live);
+    }
+  }
+}
+
+// grad_table[i] += fp32((double)acc[i] * 2^-s_l): int64 -> double (RN), the exact power-of-two product, double -> float
+// (RN), one fp32 add.  NaN where a poison bit is set; a level without a scale is left as it is.
+__global__ void __launch_bounds__(256) hashgrid_fixed_finalize_kernel(FixedWs w, int64_t total, int TF_log2, float* gtab) {
+  const bool any_bad = w.flags[0] != 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    if (any_bad && ((w.poison[i >> 5] >> (i & 31)) & 1u)) {
+      gtab[i] = __int_as_float(0x7fffffff);
+      continue;
+    }
+    const int32_t s = w.scale[i >> TF_log2];
+    if (s == kNoScale) continue;
+    gtab[i] = __fadd_rn(gtab[i], __double2float_rn(__dmul_rn(__ll2double_rn(w.acc[i]), pow2d(-s))));
+  }
+}
+
 }  // namespace
 }  // namespace pnr
 
@@ -233,6 +421,63 @@ extern "C" int pnr_hashgrid_backward(const float* x, int64_t n, const float* aab
     default: hashgrid_backward_kernel<8><<<grid, 256, 0, (cudaStream_t)stream>>>(a, grad_out, grad_table); break;
   }
   PNR_LAUNCH_CHECK("hashgrid_backward_kernel");
+  return PNR_OK;
+}
+
+static bool hash_fixed_shape_ok(int32_t L, int32_t F, int32_t T_log2) {
+  return L >= 1 && L <= 32 && (F == 1 || F == 2 || F == 4 || F == 8) && T_log2 >= 4 && T_log2 <= 28;
+}
+
+extern "C" size_t pnr_hashgrid_fixed_workspace_bytes(int32_t L, int32_t F, int32_t T_log2) {
+  return hash_fixed_shape_ok(L, F, T_log2) ? FixedLayout(L, F, T_log2).total : 0;
+}
+
+extern "C" int pnr_hashgrid_backward_fixed(const float* x, int64_t n, const float* aabb, const float* grad_out, int32_t L,
+                                           int32_t F, int32_t T_log2, float base_resolution, float per_level_scale,
+                                           float* grad_table, void* workspace, size_t workspace_bytes, void* stream) {
+  static const char* fn = "pnr_hashgrid_backward_fixed";
+  if (n == 0) return PNR_OK;
+  PNR_CHECK_ARG(n > 0, "%s: n=%lld", fn, (long long)n);
+  PNR_CHECK_ARG(x, "%s: x is null", fn);
+  PNR_CHECK_ARG(grad_out, "%s: grad_out is null", fn);
+  PNR_CHECK_ARG(grad_table, "%s: grad_table is null", fn);
+  PNR_CHECK_ARG(L >= 1 && L <= 32 && (F == 1 || F == 2 || F == 4 || F == 8), "%s: L=%d F=%d (L in [1,32], F in {1,2,4,8})", fn, L, F);
+  PNR_CHECK_ARG(T_log2 >= 4 && T_log2 <= 28, "%s: T_log2=%d outside [4,28]", fn, T_log2);
+  PNR_CHECK_ARG(base_resolution >= 1.0f && per_level_scale >= 1.0f, "%s: base_resolution / per_level_scale < 1", fn);
+  const double finest = (double)base_resolution * pow((double)per_level_scale, (double)(L - 1));
+  PNR_CHECK_ARG(finest < 1048576.0, "%s: finest resolution %.0f >= 2^20", fn, finest);
+  const FixedLayout lay(L, F, T_log2);
+  PNR_CHECK_ARG(workspace != nullptr && workspace_bytes >= lay.total,
+                "%s: workspace of %zu bytes, %zu needed (pnr_hashgrid_fixed_workspace_bytes)", fn, workspace_bytes, lay.total);
+  PNR_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 15) == 0, "%s: workspace must be 16-byte aligned", fn);
+  char* ws = static_cast<char*>(workspace);
+  const FixedWs w{reinterpret_cast<int64_t*>(ws + lay.acc), reinterpret_cast<uint32_t*>(ws + lay.poison),
+                  reinterpret_cast<uint32_t*>(ws + lay.max_bits), reinterpret_cast<int32_t*>(ws + lay.scale),
+                  reinterpret_cast<uint32_t*>(ws + lay.flags)};
+  cudaStream_t st = (cudaStream_t)stream;
+  PNR_CUDA(cudaMemsetAsync(workspace, 0, lay.total, st));
+  int clog2n = 0;
+  while (clog2n < 63 && ((int64_t)1 << clog2n) < n) ++clog2n;
+  const int W = L * F;
+  const int64_t total_g = n * W;
+  const unsigned mblocks = (unsigned)std::min<int64_t>((total_g + 1023) / 1024, kFixedMaxBlocks);
+  hashgrid_fixed_maxima_kernel<<<mblocks, 256, 0, st>>>(grad_out, total_g, W, F, L, clog2n, w);
+  PNR_LAUNCH_CHECK("hashgrid_fixed_maxima_kernel");
+  HashArgs a{x, n, nullptr, nullptr, aabb, L, F, T_log2, {}};
+  hash_level_resolutions(L, base_resolution, per_level_scale, a.res);
+  const int lpt = 8 / F;
+  const dim3 grid((unsigned)((n + 255) / 256), (unsigned)((L + lpt - 1) / lpt));
+  switch (F) {
+    case 1: hashgrid_fixed_scatter_kernel<1><<<grid, 256, 0, st>>>(a, grad_out, w); break;
+    case 2: hashgrid_fixed_scatter_kernel<2><<<grid, 256, 0, st>>>(a, grad_out, w); break;
+    case 4: hashgrid_fixed_scatter_kernel<4><<<grid, 256, 0, st>>>(a, grad_out, w); break;
+    default: hashgrid_fixed_scatter_kernel<8><<<grid, 256, 0, st>>>(a, grad_out, w); break;
+  }
+  PNR_LAUNCH_CHECK("hashgrid_fixed_scatter_kernel");
+  const int64_t entries = (int64_t)W << T_log2;
+  const unsigned fblocks = (unsigned)std::min<int64_t>((entries + 255) / 256, 8 * kFixedMaxBlocks);
+  hashgrid_fixed_finalize_kernel<<<fblocks, 256, 0, st>>>(w, entries, T_log2 + __builtin_ctz((unsigned)F), grad_table);
+  PNR_LAUNCH_CHECK("hashgrid_fixed_finalize_kernel");
   return PNR_OK;
 }
 

@@ -49,8 +49,12 @@ def make_xyz_encoder(cfg) -> Optional[HashGrid]:
     aabb = getattr(cfg, "hash_aabb", None)
     if aabb is None:
         raise ValueError("cfg.xyz_encoding='hashgrid' needs cfg.hash_aabb = [lo.xyz, hi.xyz]")
+    grad = str(getattr(cfg, "hash_grad", "atomic"))
+    if grad not in ("atomic", "fixed"):
+        raise ValueError(f"cfg.hash_grad={grad!r}: 'atomic' or 'fixed'")
     return HashGrid(L, F_, int(getattr(cfg, "hash_log2_size", 19)), float(getattr(cfg, "hash_base_resolution", 16.0)),
-                    float(getattr(cfg, "hash_per_level_scale", 1.3819)), aabb=torch.as_tensor(aabb, dtype=torch.float32))
+                    float(getattr(cfg, "hash_per_level_scale", 1.3819)), aabb=torch.as_tensor(aabb, dtype=torch.float32),
+                    grad=grad)
 
 
 class Network(nn.Module):
