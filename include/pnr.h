@@ -250,6 +250,69 @@ typedef struct pnr_ray_batch_args {
 } pnr_ray_batch_args;
 int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream);
 
+/* Depth targets from LiDAR scans (DESIGN 3.4): the points of scan s, projected into frame f of a frame set, leave per
+ * pixel the nearest depth, written into that set's depth table.  Rules (chosen here: the reference's preprocessing
+ * is not public):
+ *   1. Transform.  pair_M[k] is the row-major 3x4 [R|t] from the scan's Velodyne frame to the camera of frame
+ *      pair_frame[k], composed by the caller in float64 and rounded once (kitti360/lidar.py:
+ *      inv(cam_to_world_f) @ poses[s] @ cam_to_pose[image_00] @ inv(cam_to_velo)).  p_c = R p + t in fp32 without
+ *      FMA: ((R0 x + R1 y) + R2 z) + t0, each operation rounded, as the rotation of pnr_generate_rays.
+ *   2. Projection, the inverse of the rays of pnr_generate_rays.  Pinhole (model 0): u = (fx x) / z + cx,
+ *      v = (fy y) / z + cy.  Fisheye (model 2, MEI): n = sqrt((x x + y y) + z z), x_s = p_c / n (three divisions),
+ *      m = (x_s.x, x_s.y) / (x_s.z + xi), r2 = m.x m.x + m.y m.y, d = (1 + k1 r2) + k2 (r2 r2),
+ *      u = ((gamma1 m.x) d) + u0, v likewise; no p1 / p2 terms (the rays have none); a point with
+ *      x_s.z + xi <= 0 (or NaN) is not projected.  The equirect model (1) is refused.
+ *   3. Pixel: u = floor(fp32(uf + 0.5)), v likewise, kept when 0 <= u < W and 0 <= v < H (a pixel's ray goes through
+ *      its integer coordinates).
+ *   4. Depth: the ray parameter t of the camera's ray direction, t = z for the pinhole (direction (x, y, 1)) and t = n
+ *      for the fisheye (unit directions); a point counts when min_depth < t <= max_depth (NaN never counts).
+ *   5. Nearest wins: per pixel the smallest t, by an integer atomicMin on the bits of the positive floats over a buffer
+ *      set to +Inf, then +Inf -> 0 (no depth).  The result does not depend on the order of the points, the pairs or
+ *      the launches.
+ *   6. Occlusion filter (occlusion_radius r > 0): a pixel's depth d is kept iff d <= fp32(m * fp32(1 + margin)), m the
+ *      smallest non-zero depth in the (2r+1)^2 window around it inside the same frame (clipped at its borders), else
+ *      0.  It reads the whole z-buffer of the frame and writes depth, so it does not depend on thread order.
+ * Inputs: points [Npts, 4] f32 device (x, y, z, reflectance; reflectance unread; 16-byte aligned); scan_offset [S+1]
+ * i64 HOST: scan s is points [scan_offset[s], scan_offset[s+1]).  Pairs, HOST: pair_frame [Q] i32, pair_scan [Q] i32,
+ * pair_M [Q, 12] f32.  Frame set (device, as pnr_ray_batch_args: frame_cam [F], pix_offset [F+1], P pixels; a malformed
+ * device table is clamped, never read or written outside) and cams[0 .. num_cameras) by value.  Output depth [P] f32
+ * device: only the pixels of the frames named by some pair are rewritten (every pixel of such a frame: 0 where no point
+ * lands), every other byte is left as it is.  The host tables are read during the call; the device work is a fixed
+ * sequence of launches on `stream`, with the tables in the kernels' parameters, so the call can be captured in a CUDA
+ * graph.
+ * workspace: pnr_project_depth_workspace_bytes(P, occlusion_radius) bytes of device scratch, 16-byte aligned (the
+ * filter's z-buffer, P u32; 0 bytes and NULL without the filter).
+ * Refused before any launch (PNR_ERR_ARG, by name): F < 1 or >= 2^31 - 1, P < 1, Q < 0, S < 0, Npts < 0, a pair_frame
+ * outside [0, F) or pair_scan outside [0, S), a scan_offset that is negative, decreasing or past Npts, num_cameras
+ * outside [1, PNR_RAY_BATCH_MAX_CAMERAS], a camera model other than 0 / 2 or H, W outside [1, 2^24), min_depth not
+ * finite and > 0, max_depth not finite or <= min_depth, occlusion_radius outside [0, 8], occlusion_margin outside
+ * (0, 1) when the filter is on, a null required pointer, a misaligned points pointer, a short or misaligned
+ * workspace. */
+typedef struct pnr_project_depth_args {
+  const float* points;          /* [Npts, 4] device                                                             */
+  int64_t Npts;
+  const int64_t* scan_offset;   /* [S+1] host                                                                   */
+  int32_t S;
+  const int32_t* pair_frame;    /* [Q] host                                                                     */
+  const int32_t* pair_scan;     /* [Q] host                                                                     */
+  const float* pair_M;          /* [Q, 12] host                                                                 */
+  int32_t Q;
+  const int32_t* frame_cam;     /* [F] device                                                                   */
+  const int64_t* pix_offset;    /* [F+1] device                                                                 */
+  int32_t F;
+  int64_t P;
+  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
+  int32_t num_cameras;
+  float min_depth, max_depth;
+  int32_t occlusion_radius;     /* 0 = no filter                                                                */
+  float occlusion_margin;
+  float* depth;                 /* [P] device                                                                   */
+  void* workspace;
+  size_t workspace_bytes;
+} pnr_project_depth_args;
+size_t pnr_project_depth_workspace_bytes(int64_t P, int32_t occlusion_radius);
+int pnr_project_depth(const pnr_project_depth_args* args, void* stream);
+
 /* a7: standalone positional encoding, out [n, 3+6L]. */
 int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void* stream);
 

@@ -114,6 +114,17 @@ class PnrRayBatchArgs(C.Structure):
                [(k, C.c_void_p) for k in ("rays", "rgb", "depth_out", "pseudo_label", "u", "u_fine", "pixel", "frame")]
 
 
+class PnrProjectDepthArgs(C.Structure):
+    """pnr_project_depth_args of include/pnr.h (same field order); scan_offset and the pair tables are host pointers."""
+    _fields_ = [("points", C.c_void_p), ("Npts", C.c_int64), ("scan_offset", C.c_void_p), ("S", C.c_int32),
+                ("pair_frame", C.c_void_p), ("pair_scan", C.c_void_p), ("pair_M", C.c_void_p), ("Q", C.c_int32),
+                ("frame_cam", C.c_void_p), ("pix_offset", C.c_void_p), ("F", C.c_int32), ("P", C.c_int64),
+                ("cams", PnrRayCamera * RAY_BATCH_MAX_CAMERAS), ("num_cameras", C.c_int32),
+                ("min_depth", C.c_float), ("max_depth", C.c_float), ("occlusion_radius", C.c_int32),
+                ("occlusion_margin", C.c_float), ("depth", C.c_void_p), ("workspace", C.c_void_p),
+                ("workspace_bytes", C.c_size_t)]
+
+
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
 COMM_ID_BYTES = 128
 
@@ -137,6 +148,8 @@ SIGNATURES = {
     "pnr_tag_samples": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
     "pnr_generate_rays": (C.c_int, [_i32, _i32, _i32, _i32, _i32, C.POINTER(_f32), C.POINTER(_f32), _vp, _vp]),
     "pnr_sample_ray_batch": (C.c_int, [C.POINTER(PnrRayBatchArgs), _vp]),
+    "pnr_project_depth_workspace_bytes": (C.c_size_t, [_i64, _i32]),
+    "pnr_project_depth": (C.c_int, [C.POINTER(PnrProjectDepthArgs), _vp]),
     "pnr_encode": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_forward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_composite": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i32,

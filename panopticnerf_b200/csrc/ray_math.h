@@ -1,6 +1,6 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
-// kernels (ray_kernels.cu, rays_kernel and ray_batch_kernel in stream_kernels.cu) and a host build used by the CPU tests
-// (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
+// kernels (ray_kernels.cu, rays_kernel, ray_batch_kernel and the depth kernels in stream_kernels.cu) and host builds used
+// by the CPU tests (tests/host_emu.cpp, tests/host_emu_lidar.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
 // here (staging, shuffles, sorts); the rules they apply per ray - the per-primitive intersection step, range clamps,
 // sample depths, output slots, camera directions, batch draws - are the functions below, called by both builds.  One
 // piece stays written out in stratified_kernel and again in host_emu.cpp: the interval test (pnr_tag's rule), because
@@ -13,6 +13,7 @@
 #pragma once
 #include <stdint.h>
 #include <math.h>
+#include <string.h>
 #include "../../include/pnr.h"   // pnr_ray_batch_args: the ray-batch routine reads the entry point's own arguments
 
 #if defined(__CUDACC__)
@@ -595,4 +596,113 @@ PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, i
       else if (i < nw) a.u_fine[row * a.Ni + (i - a.N)] = pnr_u01(w[j]);
     }
   }
+}
+
+// ---------------------------------------------------------------------------------------------- LiDAR depth targets
+// pnr_project_depth (include/pnr.h; DESIGN 3.4): a scan's points projected into a frame, the nearest per pixel.  The
+// projections are the inverses of pnr_pinhole_dir / pnr_fisheye_dir; depth_kernels in stream_kernels.cu and the host
+// build (tests/host_emu_lidar.cpp) call the routines below.
+
+PNR_HD uint32_t pnr_float_bits(float x) {
+#if defined(__CUDA_ARCH__)
+  return __float_as_uint(x);
+#else
+  uint32_t b;
+  memcpy(&b, &x, 4);
+  return b;
+#endif
+}
+PNR_HD float pnr_bits_float(uint32_t b) {
+#if defined(__CUDA_ARCH__)
+  return __uint_as_float(b);
+#else
+  float x;
+  memcpy(&x, &b, 4);
+  return x;
+#endif
+}
+#define PNR_DEPTH_NONE 0x7f800000u   // +Inf: a z-buffer entry no point reached
+
+// Pinhole: camera point (x, y, z) -> (uf, vf), u = (fx x) / z + cx.
+PNR_HD void pnr_pinhole_project(float x, float y, float z, float fx, float fy, float cx, float cy, float* u, float* v) {
+  *u = PNR_ADD(PNR_DIV(PNR_MUL(fx, x), z), cx);
+  *v = PNR_ADD(PNR_DIV(PNR_MUL(fy, y), z), cy);
+}
+// Fisheye (MEI): camera point -> (uf, vf) and its distance n = |p|; false when x_s.z + xi <= 0 (or NaN).
+PNR_HD bool pnr_fisheye_project(float x, float y, float z, float g1, float g2, float u0, float v0, float xi, float k1,
+                                float k2, float* u, float* v, float* n_out) {
+  const float n = PNR_SQRT(PNR_ADD(PNR_ADD(PNR_MUL(x, x), PNR_MUL(y, y)), PNR_MUL(z, z)));
+  *n_out = n;
+  const float xs = PNR_DIV(x, n), ys = PNR_DIV(y, n), zs = PNR_DIV(z, n);
+  const float den = PNR_ADD(zs, xi);
+  if (!(den > 0.f)) return false;
+  const float mx = PNR_DIV(xs, den), my = PNR_DIV(ys, den);
+  const float r2 = PNR_ADD(PNR_MUL(mx, mx), PNR_MUL(my, my));
+  const float d = PNR_ADD(PNR_ADD(1.0f, PNR_MUL(k1, r2)), PNR_MUL(k2, PNR_MUL(r2, r2)));
+  *u = PNR_ADD(PNR_MUL(PNR_MUL(g1, mx), d), u0);
+  *v = PNR_ADD(PNR_MUL(PNR_MUL(g2, my), d), v0);
+  return true;
+}
+// One point (x, y, z) of a scan through M (row-major 3x4 [R|t], scan -> camera) into camera c: whether it lands, the
+// pixel v * W + u within the frame (*pix) and its depth (*t).
+PNR_HD bool pnr_project_point(const pnr_ray_camera& c, const float* M, float x, float y, float z, float min_depth,
+                              float max_depth, int64_t* pix, float* t_out) {
+  float xc, yc, zc;
+  pnr_cam_to_world(M, x, y, z, &xc, &yc, &zc);
+  xc = PNR_ADD(xc, M[3]);
+  yc = PNR_ADD(yc, M[7]);
+  zc = PNR_ADD(zc, M[11]);
+  float uf, vf, t;
+  if (c.model == 0) {
+    t = zc;
+    if (!(t > min_depth && t <= max_depth)) return false;
+    pnr_pinhole_project(xc, yc, zc, c.intr[0], c.intr[1], c.intr[2], c.intr[3], &uf, &vf);
+  } else {
+    if (!pnr_fisheye_project(xc, yc, zc, c.intr[0], c.intr[1], c.intr[2], c.intr[3], c.intr[4], c.intr[5], c.intr[6],
+                             &uf, &vf, &t))
+      return false;
+    if (!(t > min_depth && t <= max_depth)) return false;
+  }
+  const float fu = floorf(PNR_ADD(uf, 0.5f)), fv = floorf(PNR_ADD(vf, 0.5f));
+  if (!(fu >= 0.f && fu < (float)c.W && fv >= 0.f && fv < (float)c.H)) return false;   // NaN fails too
+  *pix = (int64_t)fv * c.W + (int64_t)fu;
+  *t_out = t;
+  return true;
+}
+// Frame f of a depth call: its camera (frame_cam clamped into the table) and pixel range [*lo, *hi) (pix_offset
+// clamped into [0, P]), so a malformed device table is never read or written outside.
+PNR_HD int pnr_depth_frame(const int32_t* frame_cam, const int64_t* off, int num_cameras, int64_t P, int f,
+                           int64_t* lo, int64_t* hi) {
+  int cam = frame_cam[f];
+  cam = cam < 0 ? 0 : (cam >= num_cameras ? num_cameras - 1 : cam);
+  int64_t a = off[f], b = off[f + 1];
+  a = a < 0 ? 0 : (a > P ? P : a);
+  b = b < a ? a : (b > P ? P : b);
+  *lo = a;
+  *hi = b;
+  return cam;
+}
+// The final depth of pixel q (= v * W + u, q < n) of a frame whose z-buffer (bits, PNR_DEPTH_NONE = none) holds its n
+// pixels at z: r = 0 -> the nearest depth or 0; r > 0 -> the occlusion filter: 0 unless d <= fp32(m * fp32(1 + margin))
+// with m the smallest depth in the (2r+1)^2 window around (u, v) inside the frame.
+PNR_HD float pnr_depth_pixel(const uint32_t* z, int64_t n, int W, int H, int64_t q, int r, float margin) {
+  const uint32_t bd = z[q];
+  if (bd == PNR_DEPTH_NONE) return 0.f;
+  const float d = pnr_bits_float(bd);
+  if (r == 0) return d;
+  const int v = (int)(q / W), u = (int)(q % W);
+  float m = d;
+  for (int dv = -r; dv <= r; ++dv) {
+    const int vv = v + dv;
+    if (vv < 0 || vv >= H) continue;
+    for (int du = -r; du <= r; ++du) {
+      const int uu = u + du;
+      if (uu < 0 || uu >= W) continue;
+      const int64_t k = (int64_t)vv * W + uu;
+      if (k >= n) continue;
+      const float x = pnr_bits_float(z[k]);   // +Inf (none) never wins
+      m = x < m ? x : m;
+    }
+  }
+  return d <= PNR_MUL(m, PNR_ADD(1.0f, margin)) ? d : 0.f;
 }

@@ -7,9 +7,15 @@
 //               striding the (contiguous) channel axis so every raw row is read once, coalesced.
 //   ray batch : one thread per training ray: a seeded random pixel of a device frame set, its camera ray, targets
 //               and jitter (pnr_ray_batch_row of ray_math.h).
+//   depth     : LiDAR depth targets: grid-strided over (pair, point), a z-buffer by integer atomicMin, then per pixel
+//               the final depth or the occlusion filter (pnr_project_point / pnr_depth_pixel of ray_math.h).
 #include "common.cuh"
 #include "composite_math.cuh"
 #include "ray_math.h"
+
+#include <algorithm>
+#include <memory>
+#include <vector>
 
 namespace pnr {
 
@@ -92,6 +98,81 @@ __global__ void __launch_bounds__(kRayBatchThreads) ray_batch_kernel(const pnr_r
   for (int64_t i = (int64_t)blockIdx.x * kRayBatchThreads + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * kRayBatchThreads)
     pnr_ray_batch_row(a, off, a.r0 + i);
+}
+
+// ------------------------------------------------------------------------------------ LiDAR depth targets
+// pnr_project_depth: fill the named frames' z-buffer with +Inf, scatter every (pair, point), then finalise (+Inf -> 0)
+// or filter into depth.  The pair and frame tables travel in the kernels' parameters (__grid_constant__, read through
+// the constant cache), in chunks, so a call is a fixed sequence of launches with no host copy and can be captured.
+//
+// The scatter is the hot path: per point one 16-byte load (__ldg; a scan is re-read by each frame of its window, and
+// those pairs sit next to each other in the table, so the re-reads mostly hit L2), about 60 fp32 operations in
+// registers, and for a point that lands one 32-bit atomicMin resolved in L2.  KITTI-360 scans put a few tens of per
+// cent of their points into a perspective frame, scattered over a frame of 2 MB of z-buffer that stays in L2, so the
+// kernel is bound by the point reads from HBM on a cold scan and by the L2 atomics' throughput otherwise.
+constexpr int kDepthThreads = 256;
+constexpr int kDepthPairsPerLaunch = 256;    // 72 B each: 18 KB of parameters
+constexpr int kDepthFramesPerLaunch = 2048;  // 4 B each: 8 KB
+
+struct DepthPair {
+  float M[12];
+  int64_t p0, n;   // the scan's points [p0, p0 + n)
+  int32_t frame;
+};
+struct DepthScatterParams {
+  const float4* points;
+  const int32_t* frame_cam;
+  const int64_t* pix_offset;
+  int64_t P;
+  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
+  int32_t num_cameras;
+  float min_depth, max_depth;
+  uint32_t* zbuf;
+  DepthPair pairs[kDepthPairsPerLaunch];
+};
+// blockIdx.y = pair of the chunk; x grid-strides over its scan's points
+__global__ void __launch_bounds__(kDepthThreads) depth_scatter_kernel(const __grid_constant__ DepthScatterParams p) {
+  const DepthPair& q = p.pairs[blockIdx.y];
+  int64_t lo, hi;
+  const int cam = pnr_depth_frame(p.frame_cam, p.pix_offset, p.num_cameras, p.P, q.frame, &lo, &hi);
+  const pnr_ray_camera& c = p.cams[cam];
+  const float4* pts = p.points + q.p0;
+  for (int64_t i = (int64_t)blockIdx.x * kDepthThreads + threadIdx.x; i < q.n;
+       i += (int64_t)gridDim.x * kDepthThreads) {
+    const float4 x = __ldg(pts + i);
+    int64_t pix;
+    float t;
+    if (pnr_project_point(c, q.M, x.x, x.y, x.z, p.min_depth, p.max_depth, &pix, &t) && lo + pix < hi)
+      atomicMin(p.zbuf + lo + pix, pnr_float_bits(t));
+  }
+}
+
+// kFill: zbuf = +Inf over the frames' pixels; otherwise depth = pnr_depth_pixel of the z-buffer (r = 0: finalise, in
+// place when zbuf aliases depth; r > 0: the filter, from the workspace's z-buffer)
+struct DepthFrameParams {
+  const int32_t* frame_cam;
+  const int64_t* pix_offset;
+  int64_t P;
+  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
+  int32_t num_cameras;
+  uint32_t* zbuf;
+  float* depth;
+  int32_t radius;
+  float margin;
+  int32_t frames[kDepthFramesPerLaunch];
+};
+template <bool kFill>
+__global__ void __launch_bounds__(kDepthThreads) depth_frames_kernel(const __grid_constant__ DepthFrameParams p) {
+  int64_t lo, hi;
+  const int cam = pnr_depth_frame(p.frame_cam, p.pix_offset, p.num_cameras, p.P, p.frames[blockIdx.y], &lo, &hi);
+  const pnr_ray_camera& c = p.cams[cam];
+  const int64_t n = hi - lo;
+  for (int64_t q = (int64_t)blockIdx.x * kDepthThreads + threadIdx.x; q < n; q += (int64_t)gridDim.x * kDepthThreads) {
+    if (kFill)
+      p.zbuf[lo + q] = PNR_DEPTH_NONE;
+    else
+      p.depth[lo + q] = pnr_depth_pixel(p.zbuf + lo, n, c.W, c.H, q, p.radius, p.margin);
+  }
 }
 
 // ------------------------------------------------------------------------------------ a9 composite
@@ -598,6 +679,134 @@ extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream
   }
   PNR_LAUNCH_CHECK("ray_batch_kernel");
   return PNR_OK;
+}
+
+extern "C" size_t pnr_project_depth_workspace_bytes(int64_t P, int32_t occlusion_radius) {
+  if (P < 1 || occlusion_radius < 0 || occlusion_radius > 8) return 0;
+  return occlusion_radius == 0 ? 0 : (((size_t)P * sizeof(uint32_t) + 15) & ~(size_t)15);
+}
+
+extern "C" int pnr_project_depth(const pnr_project_depth_args* args, void* stream) {
+  PNR_CHECK_ARG(args, "pnr_project_depth: null args");
+  const pnr_project_depth_args& a = *args;
+  PNR_CHECK_ARG(a.F >= 1 && a.F < INT32_MAX, "pnr_project_depth: F=%d outside [1, 2^31 - 1)", a.F);
+  PNR_CHECK_ARG(a.P >= 1, "pnr_project_depth: P=%lld < 1", (long long)a.P);
+  PNR_CHECK_ARG(a.Q >= 0, "pnr_project_depth: Q=%d < 0", a.Q);
+  PNR_CHECK_ARG(a.S >= 0, "pnr_project_depth: S=%d < 0", a.S);
+  PNR_CHECK_ARG(a.Npts >= 0, "pnr_project_depth: Npts=%lld < 0", (long long)a.Npts);
+  PNR_CHECK_ARG(a.num_cameras >= 1 && a.num_cameras <= PNR_RAY_BATCH_MAX_CAMERAS,
+                "pnr_project_depth: num_cameras=%d outside [1,%d]", a.num_cameras, PNR_RAY_BATCH_MAX_CAMERAS);
+  for (int k = 0; k < a.num_cameras; ++k) {
+    const pnr_ray_camera& c = a.cams[k];
+    if (c.model == 1)
+      return set_error(PNR_ERR_ARG, "pnr_project_depth: camera %d is equirect (model 1); depth targets take pinhole "
+                       "(0) and fisheye (2) cameras, as training batches do", k);
+    PNR_CHECK_ARG(c.model == 0 || c.model == 2, "pnr_project_depth: camera %d model %d (0 pinhole, 2 fisheye)", k,
+                  c.model);
+    PNR_CHECK_ARG(c.H >= 1 && c.W >= 1 && c.H < (1 << 24) && c.W < (1 << 24),
+                  "pnr_project_depth: camera %d size H=%d W=%d outside [1, 2^24)", k, c.H, c.W);
+  }
+  PNR_CHECK_ARG(isfinite(a.min_depth) && a.min_depth > 0.f, "pnr_project_depth: min_depth=%g is not finite and > 0",
+                (double)a.min_depth);
+  PNR_CHECK_ARG(isfinite(a.max_depth) && a.max_depth > a.min_depth,
+                "pnr_project_depth: max_depth=%g is not finite and > min_depth=%g", (double)a.max_depth,
+                (double)a.min_depth);
+  PNR_CHECK_ARG(a.occlusion_radius >= 0 && a.occlusion_radius <= 8,
+                "pnr_project_depth: occlusion_radius=%d outside [0, 8]", a.occlusion_radius);
+  const bool filter = a.occlusion_radius > 0;
+  PNR_CHECK_ARG(!filter || (a.occlusion_margin > 0.f && a.occlusion_margin < 1.f),
+                "pnr_project_depth: occlusion_margin=%g outside (0, 1)", (double)a.occlusion_margin);
+  PNR_CHECK_ARG(a.frame_cam && a.pix_offset && a.depth,
+                "pnr_project_depth: null frame-set pointer (frame_cam, pix_offset and depth are required)");
+  PNR_CHECK_ARG(a.scan_offset, "pnr_project_depth: null scan_offset (host [S+1])");
+  PNR_CHECK_ARG(a.Q == 0 || (a.pair_frame && a.pair_scan && a.pair_M),
+                "pnr_project_depth: null pair table (pair_frame, pair_scan and pair_M are required with Q=%d)", a.Q);
+  PNR_CHECK_ARG(a.Npts == 0 || a.points, "pnr_project_depth: null points with Npts=%lld", (long long)a.Npts);
+  PNR_CHECK_ARG(((uintptr_t)a.points & 15) == 0, "pnr_project_depth: points is not 16-byte aligned");
+  for (int s = 0; s <= a.S; ++s) {
+    const int64_t o = a.scan_offset[s];
+    PNR_CHECK_ARG(o >= 0 && o <= a.Npts, "pnr_project_depth: scan_offset[%d]=%lld outside [0, Npts=%lld]", s,
+                  (long long)o, (long long)a.Npts);
+    PNR_CHECK_ARG(s == 0 || o >= a.scan_offset[s - 1], "pnr_project_depth: scan_offset decreases at %d (%lld < %lld)",
+                  s, (long long)o, (long long)a.scan_offset[s - 1]);
+  }
+  for (int k = 0; k < a.Q; ++k) {
+    PNR_CHECK_ARG(a.pair_frame[k] >= 0 && a.pair_frame[k] < a.F, "pnr_project_depth: pair_frame[%d]=%d outside [0, F=%d)",
+                  k, a.pair_frame[k], a.F);
+    PNR_CHECK_ARG(a.pair_scan[k] >= 0 && a.pair_scan[k] < a.S, "pnr_project_depth: pair_scan[%d]=%d outside [0, S=%d)",
+                  k, a.pair_scan[k], a.S);
+  }
+  const size_t need = pnr_project_depth_workspace_bytes(a.P, a.occlusion_radius);
+  PNR_CHECK_ARG(!filter || (a.workspace && a.workspace_bytes >= need && ((uintptr_t)a.workspace & 15) == 0),
+                "pnr_project_depth: workspace of %zu bytes at %p; the filter needs %zu bytes, 16-byte aligned",
+                a.workspace_bytes, a.workspace, need);
+  if (a.Q == 0) return PNR_OK;
+  int dev = 0;
+  int rc = current_device("pnr_project_depth", &dev);
+  if (rc != PNR_OK) return rc;
+  const int sms = num_sms(dev);
+  const cudaStream_t st = (cudaStream_t)stream;
+
+  std::vector<int32_t> frames(a.pair_frame, a.pair_frame + a.Q);
+  std::sort(frames.begin(), frames.end());
+  frames.erase(std::unique(frames.begin(), frames.end()), frames.end());
+  int64_t max_hw = 1;
+  for (int k = 0; k < a.num_cameras; ++k) max_hw = std::max(max_hw, (int64_t)a.cams[k].H * a.cams[k].W);
+  uint32_t* zbuf = filter ? (uint32_t*)a.workspace : (uint32_t*)a.depth;
+
+  // the frame passes: kFill over zbuf, then (after the scatter) the final depth
+  auto frame_pass = [&](bool fill) -> int {
+    std::unique_ptr<DepthFrameParams> hold(new DepthFrameParams());   // 8 KB, copied by each launch
+    DepthFrameParams& fp = *hold;
+    fp.frame_cam = a.frame_cam; fp.pix_offset = a.pix_offset; fp.P = a.P;
+    for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k) fp.cams[k] = a.cams[k < a.num_cameras ? k : 0];
+    fp.num_cameras = a.num_cameras; fp.zbuf = zbuf; fp.depth = a.depth;
+    fp.radius = a.occlusion_radius; fp.margin = a.occlusion_margin;
+    for (size_t f0 = 0; f0 < frames.size(); f0 += kDepthFramesPerLaunch) {
+      const int nf = (int)std::min<size_t>(kDepthFramesPerLaunch, frames.size() - f0);
+      for (int i = 0; i < nf; ++i) fp.frames[i] = frames[f0 + i];
+      const int64_t want = (max_hw + kDepthThreads - 1) / kDepthThreads;
+      const int64_t cap = std::max<int64_t>(1, (int64_t)sms * 16 / nf);
+      const dim3 grid((unsigned)std::min(want, cap), (unsigned)nf);
+      if (fill) depth_frames_kernel<true><<<grid, kDepthThreads, 0, st>>>(fp);
+      else depth_frames_kernel<false><<<grid, kDepthThreads, 0, st>>>(fp);
+      PNR_LAUNCH_CHECK("depth_frames_kernel");
+    }
+    return PNR_OK;
+  };
+  rc = frame_pass(true);
+  if (rc != PNR_OK) return rc;
+
+  std::unique_ptr<DepthScatterParams> hold(new DepthScatterParams());   // 18 KB, copied by each launch
+  DepthScatterParams& sp = *hold;
+  sp.points = (const float4*)a.points; sp.frame_cam = a.frame_cam; sp.pix_offset = a.pix_offset; sp.P = a.P;
+  for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k) sp.cams[k] = a.cams[k < a.num_cameras ? k : 0];
+  sp.num_cameras = a.num_cameras; sp.min_depth = a.min_depth; sp.max_depth = a.max_depth; sp.zbuf = zbuf;
+  int np = 0;
+  int64_t max_n = 0;
+  auto flush = [&]() -> int {
+    if (np == 0) return PNR_OK;
+    const int64_t want = (max_n + kDepthThreads - 1) / kDepthThreads;
+    const int64_t cap = std::max<int64_t>(1, (int64_t)sms * 8 / np);
+    depth_scatter_kernel<<<dim3((unsigned)std::max<int64_t>(1, std::min(want, cap)), (unsigned)np), kDepthThreads, 0,
+                           st>>>(sp);
+    PNR_LAUNCH_CHECK("depth_scatter_kernel");
+    np = 0;
+    max_n = 0;
+    return PNR_OK;
+  };
+  for (int k = 0; k < a.Q; ++k) {
+    const int s = a.pair_scan[k];
+    const int64_t p0 = a.scan_offset[s], n = a.scan_offset[s + 1] - p0;
+    if (n == 0) continue;
+    DepthPair& q = sp.pairs[np++];
+    for (int i = 0; i < 12; ++i) q.M[i] = a.pair_M[(int64_t)k * 12 + i];
+    q.p0 = p0; q.n = n; q.frame = a.pair_frame[k];
+    max_n = std::max(max_n, n);
+    if (np == kDepthPairsPerLaunch && (rc = flush()) != PNR_OK) return rc;
+  }
+  if ((rc = flush()) != PNR_OK) return rc;
+  return frame_pass(false);
 }
 
 extern "C" int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void* stream) {

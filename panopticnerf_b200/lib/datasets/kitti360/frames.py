@@ -67,28 +67,41 @@ def camera_of(root, camera: str) -> Camera:
                   tuple(fe[k] for k in ("gamma1", "gamma2", "u0", "v0", "xi", "k1", "k2")))
 
 
+def camera_poses(root, seq: str, camera: str):
+    """(pose_of, src): pose_of(frame) -> the float64 4x4 camera -> world of `camera` at `frame` (KeyError without a
+    pose), src the pose file it reads.  image_00: cam0_to_world; image_02 / 03: poses.txt @ calib_cam_to_pose."""
+    root = Path(root)
+    poses = root / "data_poses" / seq
+    if camera == "image_00":
+        table = load_cam0_to_world(poses / "cam0_to_world.txt")
+        return (lambda f: table[f]), poses / "cam0_to_world.txt"
+    imu = load_poses(poses / "poses.txt")
+    c2p = load_cam_to_pose(root / "calibration" / "calib_cam_to_pose.txt")
+    if camera not in c2p:
+        raise ValueError(f"{root / 'calibration' / 'calib_cam_to_pose.txt'}: no {camera}")
+    return (lambda f: fisheye_to_world(c2p[camera], imu[f])), poses / "poses.txt"
+
+
 def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00", pseudo_dir=None, depth_dir=None,
-                sem_to_train: Optional[Dict[int, int]] = None, device="cuda") -> FrameSet:
-    """The frames `frames` of sequence `seq` seen by `camera`, on `device` (module docstring: layout and formats)."""
+                sem_to_train: Optional[Dict[int, int]] = None, device="cuda", lidar=False) -> FrameSet:
+    """The frames `frames` of sequence `seq` seen by `camera`, on `device` (module docstring: layout and formats).
+    lidar: False, True or a dict of `lidar.lidar_depth` options - the depth table from the sequence's Velodyne scans
+    instead of depth_dir's PNGs (the two are refused together)."""
     if camera not in CAMERAS:
         raise ValueError(f"load_frames: camera {camera!r}; one of {CAMERAS}")
+    want_lidar = lidar is not False and lidar is not None   # {} is on, with the defaults
+    if want_lidar:
+        from .lidar import LIDAR_OPTIONS
+        if depth_dir is not None:
+            raise ValueError("load_frames: lidar and depth_dir both give the depth table; pass one of them")
+        if lidar is not True and (not isinstance(lidar, dict) or set(lidar) - set(LIDAR_OPTIONS)):
+            raise ValueError(f"load_frames: lidar={lidar!r}; False, True or a dict with keys from {LIDAR_OPTIONS}")
     root = Path(root)
     frames = [int(f) for f in frames]
     if not frames:
         raise ValueError("load_frames: no frames")
     cam = camera_of(root, camera)
-    poses = root / "data_poses" / seq
-    if camera == "image_00":
-        table = load_cam0_to_world(poses / "cam0_to_world.txt")
-        pose_of = lambda f: table[f]
-        src = poses / "cam0_to_world.txt"
-    else:
-        imu = load_poses(poses / "poses.txt")
-        c2p = load_cam_to_pose(root / "calibration" / "calib_cam_to_pose.txt")
-        if camera not in c2p:
-            raise ValueError(f"{root / 'calibration' / 'calib_cam_to_pose.txt'}: no {camera}")
-        pose_of = lambda f: fisheye_to_world(c2p[camera], imu[f])
-        src = poses / "poses.txt"
+    pose_of, src = camera_poses(root, seq, camera)
     images = root / "data_2d_raw" / seq / camera / ("data_rect" if camera == "image_00" else "data_rgb")
     lut = None
     if sem_to_train is not None:
@@ -113,9 +126,13 @@ def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00",
             p = Path(depth_dir) / name
             d = _sized(_read(p, "a depth image", np.uint16, 1), cam, p, "the depth image")
             dep.append(torch.from_numpy(d.astype(np.float32) / np.float32(256.0)))
-    return FrameSet.from_images([cam], [0] * len(frames), np.stack(c2w).astype(np.float32), rgb,
-                                lab if pseudo_dir is not None else None, dep if depth_dir is not None else None,
-                                [(camera, f) for f in frames], device)
+    fs = FrameSet.from_images([cam], [0] * len(frames), np.stack(c2w).astype(np.float32), rgb,
+                              lab if pseudo_dir is not None else None, dep if depth_dir is not None else None,
+                              [(camera, f) for f in frames], device)
+    if want_lidar:
+        from .lidar import lidar_depth
+        lidar_depth(fs, root, seq, **({} if lidar is True else lidar))
+    return fs
 
 
-__all__ = ["CAMERAS", "camera_of", "load_frames"]
+__all__ = ["CAMERAS", "camera_of", "camera_poses", "load_frames"]
