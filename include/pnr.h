@@ -89,6 +89,18 @@ int pnr_status(pnr_ctx* ctx, uint32_t* status_host, int32_t reset, void* stream)
  * (PNR_ERR_ARG), here and by pnr_hashgrid_encode. */
 int pnr_bind_hashgrid_table(pnr_ctx* ctx, const float* table);
 
+/* Tile of the fused MLP kernel for this context's raw-row launches (pnr_mlp_forward, and pnr_render_fused on a network
+ * without heads): 0 (default) = 128 samples on two consumer warpgroups when the network's program allows it (a
+ * 256-wide network without heads, pnr_program_tile_rows), else 64; 64 = always the 64-sample kernel; 128 = the
+ * 128-sample kernel, and a launch whose program does not allow it returns PNR_ERR_UNSUPPORTED.  Both kernels give the
+ * same bits.  The compositing and backward launches run 64-sample tiles whatever the setting.  PNR_ERR_ARG for any
+ * other value. */
+int pnr_set_mlp_rows(pnr_ctx* ctx, int32_t rows);
+
+/* Host only: the tile (64 or 128 samples) a raw-row launch of `program` (the MlpProgram struct pnr_program_host
+ * returns, program_bytes = its size) runs on when pnr_set_mlp_rows is 0. */
+int pnr_program_tile_rows(const void* program, size_t program_bytes, int32_t* rows);
+
 /* a2: load a Network state_dict.  `tensors_host[i]` are HOST fp32 pointers in this fixed order:
  *   pts_linears.{0..D-1}.weight/.bias (interleaved w,b), alpha_linear.w/.b, feature_linear.w/.b,
  *   views_linears.0.w/.b, rgb_linear.w/.b, [semantic_linears.0.w/.b, semantic_linears.1.w/.b],

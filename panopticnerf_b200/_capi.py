@@ -137,6 +137,8 @@ SIGNATURES = {
     "pnr_destroy": (C.c_int, [_vp]),
     "pnr_status": (C.c_int, [_vp, C.POINTER(C.c_uint32), _i32, _vp]),
     "pnr_bind_hashgrid_table": (C.c_int, [_vp, _vp]),
+    "pnr_set_mlp_rows": (C.c_int, [_vp, _i32]),
+    "pnr_program_tile_rows": (C.c_int, [_vp, C.c_size_t, C.POINTER(_i32)]),
     "pnr_load_weights": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32]),
     "pnr_intersect": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "pnr_intersect_meshes": (C.c_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
@@ -214,6 +216,11 @@ def check(rc: int, what: str = "") -> None:
     if rc != 0:
         msg = lib().pnr_last_error()
         raise PnrError(f"{what or 'libpnr'} failed (rc={rc}): {msg.decode() if msg else '?'}")
+
+
+def set_mlp_rows(ctx: int, rows: int) -> None:
+    """Tile of the context's raw-row MLP launches (pnr_set_mlp_rows): 0 = the one its program allows, 64 or 128."""
+    check(lib().pnr_set_mlp_rows(ctx, rows), "pnr_set_mlp_rows")
 
 
 def stream_ptr() -> int:

@@ -204,6 +204,9 @@ struct MlpParams {
   float* raw;
   int32_t num_tiles;
   uint32_t* status;       // sticky device word: bit 0 = a non-finite / out-of-range activation was seen (may be null)
+  int32_t head_blocks;    // 1: the sigma / rgb heads are summed in 8-column blocks (head_dot_*, mlp_wgmma.cu), the order
+                          // of the 128-row kernel, for every launch of a program mlp_rows128_ok accepts; 0: one running
+                          // sum per column share (the order of every other program); set by launch_mlp
   // ---- compositing epilogue (COMPOSITE kernels only: rays mode, N % 32 == 0; `raw` is not written)
   int64_t rays_per_cta;   // every CTA owns a contiguous range of whole rays (carries stay on chip)
   const int32_t* sample_box;   // [S] primitive id per sample, or null (only read when mask_outside)
@@ -266,5 +269,61 @@ constexpr int kSmemCompS = kSmemCompQ + 64;                     // float qsum[2]
 constexpr int kSmemCompR = kSmemCompS + 2 * kQuarters * kCompChPad * 4; // float racc[kCompChPad]: running sums of the open ray
 constexpr int kSmemTotalComp = kSmemCompR + kCompChPad * 4;
 static_assert(kSmemTotalComp <= 232448, "shared-memory map exceeds the 227 KB per-CTA limit");
+
+// Shared-memory map of the 128-row kernel (mlp_rows128_kernel: forward programs without heads, see
+// mlp_rows128_ok).  Two consumer warpgroups, rows [64g, 64g + 64) of a 128-sample tile each; warpgroup g owns block g:
+// its trunk activations (operand columns [256, 512), hi and lo), its xyz embedding and its view-dir embedding, in the
+// layouts of the 64-row kernel.  Both read every slot of one 3-slot weight ring.  No staging tile: every epilogue runs
+// from the accumulator registers.
+constexpr int kRows128 = 2 * kRows;
+constexpr int kMlp128Threads = 3 * kConsumerThreads;     // two consumer warpgroups + the weight-stream warpgroup
+constexpr int kSlots128 = 3;
+constexpr int kSlot128Bytes = kStageBytes / 2;            // half a stage, as in the 64-row kernel's ring
+constexpr int kSmem128Ring = 0;
+constexpr int kSmem128Blk = kSmem128Ring + kSlots128 * kSlot128Bytes;           // block of warpgroup 0
+constexpr int kBlk128Op = 0;                                                     // columns [256, 512): 64 K-cores
+constexpr int kBlk128Emb = kBlk128Op + (512 - kColAHi) / 4 * kOpKCoreBytes;      // xyz embedding: hi 8K, lo 8K
+constexpr int kBlk128Dir = kBlk128Emb + 2 * kEmbPartBytes;                       // view-dir embedding: hi 4K, lo 4K
+constexpr int kBlk128Bytes = kBlk128Dir + 2 * kDirPartBytes;
+constexpr int kSmem128Sig = kSmem128Blk + 2 * kBlk128Bytes;   // float [kRows128]: each row's sigma dot, bias not added
+constexpr int kSmem128Bars = kSmem128Sig + kRows128 * 4;      // full [kSlots128], empty [kSlots128]
+constexpr int kSmem128Total = kSmem128Bars + 2 * kSlots128 * 8;
+static_assert(kBlk128Bytes == 65536 + 16384 + 8192, "block: activations, embedding, view-dir embedding");
+static_assert(kSmem128Blk % 1024 == 0 && kBlk128Bytes % 1024 == 0, "operand blocks 1024-aligned");
+static_assert(kSmem128Total <= 232448, "128-row shared-memory map exceeds the 227 KB per-CTA limit");
+static_assert(kConsumerThreads / 32 * 24 + 2 * kConsumerThreads / 32 * 240 <= 65536 / 32,
+              "register split: 24 per weight-stream thread and 240 per consumer thread fit the register file");
+
+// Can the 128-row kernel run forward program `pg`?  Its epilogues are the register ones (mlp_wgmma.cu): every step
+// but the last is a ReLU hand-over of N = 256 as two N = 128 halves into the trunk activation columns, the one before
+// the last also forming the sigma head; the last is the view step, N = 128 as one half.  Every A operand is the xyz
+// embedding (K <= 64), the view-dir embedding (K <= 32) or the trunk activations, so no step reads or writes the head
+// columns [128, 256), which the 128-row map does not have.  A 256-wide network without heads: cfg2, in every precision
+// and with either trunk input.
+inline bool mlp_rows128_ok(const MlpProgram& pg) {
+  const int S = pg.n_steps;
+  if (S < 2 || S > kMaxSteps || pg.n_stages < 1 || pg.n_stages > kMaxStages) return false;
+  for (int s = 0; s < S; ++s) {
+    const EpiDesc& e = pg.ep[s];
+    if (e.acc_col != kColAcc || e.sigma != (s == S - 2 ? 1 : 0)) return false;
+    if (s < S - 1 && !(e.kind == EPI_RELU_TO_A && e.n == 256 && e.n0 == 128 && e.dst_col == kColAHi &&
+                       e.dst_lo_col == kColALo))
+      return false;
+    if (s == S - 1 && !(e.kind == EPI_VIEW_RGB && e.n == 128 && e.n0 == 128)) return false;
+  }
+  for (int i = 0; i < pg.n_stages; ++i) {
+    const StageDesc& sd = pg.st[i];
+    const int k = sd.ksteps * 16;   // K of the stage
+    if (sd.a_kind == A_EMB) {
+      if (k > 64) return false;
+    } else if (sd.a_kind == A_DIR) {
+      if (k > 32) return false;
+    } else if (sd.a_kind != A_TMEM || sd.a_off < kColAHi || sd.a_lo_off < kColAHi || sd.a_off + k / 2 > 512 ||
+               sd.a_lo_off + k / 2 > 512) {
+      return false;
+    }
+  }
+  return true;
+}
 
 }  // namespace pnr

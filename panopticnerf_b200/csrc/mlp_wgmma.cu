@@ -146,19 +146,50 @@ __device__ __forceinline__ float4 relu_bias4(const uint32_t (&r)[16], int q, flo
                      relu_nan(__uint_as_float(r[4 * q + 2]) + b.z), relu_nan(__uint_as_float(r[4 * q + 3]) + b.w));
 }
 
-// activation -> next layer's A operand: v = act(acc + bias); [sigma += v . wsig]; split into hi / lo parts.
-// `vmax` collects the largest hi-part bit patterns seen (two 16-bit lanes; range check of the operand format).
+// The sigma and rgb heads' dot products, in ONE summation order for both kernels (the 64-row kernel's staged epilogue
+// and the 128-row kernel's register epilogue give the same bits).  A head's K columns fall into two SHARES - in every
+// 128-column window, the first ceil(groups / 2) 16-column groups and the rest (the staged epilogue's column shares;
+// for K = 256 or 128, columns c with c % 128 < 64 and the others) - and into 8-column BLOCKS (one core row; a quad of
+// lanes holds one in a wgmma accumulator fragment, lane t the pair 2t, 2t + 1).  Pair t of a block: v[2t] w[2t], then
+// a fused multiply-add of v[2t+1] w[2t+1]; a block: (pair 0 + pair 1) + (pair 2 + pair 3); a share: the sum of its
+// blocks in increasing column order, from 0; the dot product: (share 0 + share 1) + bias.  Explicit round-to-nearest
+// operations: no call site can contract them differently.
+__device__ __forceinline__ float head_dot_pair(float v0, float w0, float v1, float w1) {
+  return __fmaf_rn(v1, w1, __fmul_rn(v0, w0));
+}
+__device__ __forceinline__ float head_dot_block(float p0, float p1, float p2, float p3) {
+  return __fadd_rn(__fadd_rn(p0, p1), __fadd_rn(p2, p3));
+}
+// head_dot_block when lane t of each quad holds pair t: every lane of the quad returns it (addition commutes)
+__device__ __forceinline__ float head_dot_block_quad(float p) {
+  const float x = __fadd_rn(p, __shfl_xor_sync(0xffffffffu, p, 1));
+  return __fadd_rn(x, __shfl_xor_sync(0xffffffffu, x, 2));
+}
+__device__ __forceinline__ float head_dot_add_block(float share, float block) { return __fadd_rn(share, block); }
+__device__ __forceinline__ float head_dot_total(float share0, float share1, float bias) {
+  return __fadd_rn(__fadd_rn(share0, share1), bias);
+}
+
+// activation -> next layer's A operand: v = act(acc + bias); [sigma share += v . wsig, head_dot_*]; split into hi / lo
+// parts.  `vmax` collects the largest hi-part bit patterns seen (two 16-bit lanes; range check of the operand format).
 template <int PASSES, int FMT>
 __device__ __forceinline__ void epi_group_act(const uint32_t (&r)[16], int g, const EpiDesc& ed,
-                                              const float* bias, const float* wsig, float& sig, uint32_t& vmax,
-                                              uint32_t (&hi)[8], uint32_t (&lo)[8]) {
+                                              const float* bias, const float* wsig, bool blocks, float& sig,
+                                              uint32_t& vmax, uint32_t (&hi)[8], uint32_t (&lo)[8]) {
   const float4* b4 = reinterpret_cast<const float4*>(bias + g * 16);
+  float p0 = 0.f, p1 = 0.f;   // the first two pairs of the current block
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const float4 v = relu_bias4(r, q, b4[q]);
-    if (ed.sigma) {
+    if (ed.sigma) {   // columns 16g + 4q .. + 3: pairs 0, 1 (q even) or 2, 3 (q odd) of block 2g + q / 2
       const float4 w = reinterpret_cast<const float4*>(wsig + g * 16)[q];
-      sig += v.x * w.x + v.y * w.y + v.z * w.z + v.w * w.w;
+      if (blocks) {
+        const float pa = head_dot_pair(v.x, w.x, v.y, w.y), pb = head_dot_pair(v.z, w.z, v.w, w.w);
+        if ((q & 1) == 0) { p0 = pa; p1 = pb; }
+        else sig = head_dot_add_block(sig, head_dot_block(p0, p1, pa, pb));
+      } else {
+        sig += v.x * w.x + v.y * w.y + v.z * w.z + v.w * w.w;
+      }
     }
     split_x2<FMT>(v.x, v.y, hi[2 * q], lo[2 * q]);
     split_x2<FMT>(v.z, v.w, hi[2 * q + 1], lo[2 * q + 1]);
@@ -186,21 +217,37 @@ __device__ __forceinline__ void epi_group_store(int g, const EpiDesc& ed, uint8_
   }
 }
 
+// the rgb head on this group's columns, added to this share's sums c0, c1, c2: in blocks (head_dot_*) or one running
+// sum per channel (MlpParams::head_blocks)
 __device__ __forceinline__ void epi_group_rgb(const uint32_t (&r)[16], int g, const EpiDesc& ed, const float* bias,
-                                              const float* wr, float& c0, float& c1, float& c2) {
+                                              const float* wr, bool blocks, float& c0, float& c1, float& c2) {
   // bias and the three weight rows come as 16-byte shared-memory loads (every offset is a multiple of 4 floats)
   const float4* b4 = reinterpret_cast<const float4*>(bias + g * 16);
   const float4* w0 = reinterpret_cast<const float4*>(wr + g * 16);
   const float4* w1 = reinterpret_cast<const float4*>(wr + ed.n + g * 16);
   const float4* w2 = reinterpret_cast<const float4*>(wr + 2 * ed.n + g * 16);
+  float p[3][2];   // the first two pairs of the current block, per channel
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     const float4 b = b4[q], a0 = w0[q], a1 = w1[q], a2 = w2[q];
     const float4 v = relu_bias4(r, q, b);
-    c0 += v.x * a0.x; c1 += v.x * a1.x; c2 += v.x * a2.x;
-    c0 += v.y * a0.y; c1 += v.y * a1.y; c2 += v.y * a2.y;
-    c0 += v.z * a0.z; c1 += v.z * a1.z; c2 += v.z * a2.z;
-    c0 += v.w * a0.w; c1 += v.w * a1.w; c2 += v.w * a2.w;
+    if (!blocks) {
+      c0 += v.x * a0.x; c1 += v.x * a1.x; c2 += v.x * a2.x;
+      c0 += v.y * a0.y; c1 += v.y * a1.y; c2 += v.y * a2.y;
+      c0 += v.z * a0.z; c1 += v.z * a1.z; c2 += v.z * a2.z;
+      c0 += v.w * a0.w; c1 += v.w * a1.w; c2 += v.w * a2.w;
+      continue;
+    }
+    const float q0a = head_dot_pair(v.x, a0.x, v.y, a0.y), q0b = head_dot_pair(v.z, a0.z, v.w, a0.w);
+    const float q1a = head_dot_pair(v.x, a1.x, v.y, a1.y), q1b = head_dot_pair(v.z, a1.z, v.w, a1.w);
+    const float q2a = head_dot_pair(v.x, a2.x, v.y, a2.y), q2b = head_dot_pair(v.z, a2.z, v.w, a2.w);
+    if ((q & 1) == 0) {   // pairs 0, 1 of a block
+      p[0][0] = q0a; p[0][1] = q0b; p[1][0] = q1a; p[1][1] = q1b; p[2][0] = q2a; p[2][1] = q2b;
+    } else {              // pairs 2, 3: the block is complete
+      c0 = head_dot_add_block(c0, head_dot_block(p[0][0], p[0][1], q0a, q0b));
+      c1 = head_dot_add_block(c1, head_dot_block(p[1][0], p[1][1], q1a, q1b));
+      c2 = head_dot_add_block(c2, head_dot_block(p[2][0], p[2][1], q2a, q2b));
+    }
   }
 }
 
@@ -357,9 +404,13 @@ __device__ __forceinline__ constexpr uint32_t inf_bits16() {
 constexpr int kSlots = 4;
 constexpr int kSlotBytes = kRing * kStageBytes / kSlots;
 static_assert(2 * kSlotBytes == kStageBytes, "a program stage is two ring slots");
-// ring slot and barrier phase of the gs-th slot taken (the weight stream and the consumers count alike)
-__device__ __forceinline__ uint32_t ring_slot(uint32_t gs) { return gs % kSlots; }
-__device__ __forceinline__ uint32_t ring_phase(uint32_t gs) { return (gs / kSlots) & 1; }
+static_assert(kSlot128Bytes == kSlotBytes, "both kernels' rings have slots of half a stage");
+// ring slot and barrier phase of the gs-th slot taken (the weight stream and the consumers count alike) in a ring of
+// NS slots (kSlots in the 64-row kernel, kSlots128 in the 128-row kernel)
+template <int NS>
+__device__ __forceinline__ uint32_t ring_slot(uint32_t gs) { return gs % NS; }
+template <int NS>
+__device__ __forceinline__ uint32_t ring_phase(uint32_t gs) { return (gs / NS) & 1; }
 
 __device__ __forceinline__ int stage_slots(const StageDesc& sd) { return sd.ksteps > 1 ? 2 : 1; }
 // the K16 steps [k0, k0 + kn) of slot j of the stage (the first K-half is the larger one)
@@ -370,8 +421,39 @@ __device__ __forceinline__ void slot_ksteps(const StageDesc& sd, int j, int& k0,
 }
 
 // The slot's MMAs have retired: one arrival per consumer warp (lane 0) on its empty barrier; slot < 0: none.
+template <int NS>
 __device__ __forceinline__ void release_slot(uint32_t bar_empty, int slot, bool leader) {
-  mbar_arrive_if(bar_empty + 8u * (uint32_t)(slot & (kSlots - 1)), leader && slot >= 0);
+  const uint32_t s = (NS & (NS - 1)) == 0 ? (uint32_t)(slot & (NS - 1)) : (uint32_t)(slot < 0 ? 0 : slot);
+  mbar_arrive_if(bar_empty + 8u * s, leader && slot >= 0);
+}
+
+// The weight stream (one thread): every stage of the program, n_iter times, one slot per K-half of a stage, each slot
+// refilled once every consumer warp has released it.
+template <int PASSES, int NS>
+__device__ __forceinline__ void stream_weights(const MlpParams& p, const MlpProgram& prog, int n_iter, uint32_t ring_s,
+                                               uint32_t bar_full, uint32_t bar_empty) {
+  const int n_stages = prog.n_stages;
+  uint32_t gs = 0;  // global slot counter
+  for (int it = 0; it < n_iter; ++it) {
+    for (int si = 0; si < n_stages; ++si) {
+      const StageDesc& sd = prog.st[si];
+      const uint32_t step_bytes = (uint32_t)sd.n * 32u;   // one K16 step of one image
+      const int nslots = stage_slots(sd);
+      for (int j = 0; j < nslots; ++j, ++gs) {
+        int k0, kn;
+        slot_ksteps(sd, j, k0, kn);
+        const uint32_t slot = ring_slot<NS>(gs), ph = ring_phase<NS>(gs);
+        const uint32_t part = (uint32_t)kn * step_bytes;   // bytes of one image in this slot
+        const uint32_t dst = ring_s + slot * (uint32_t)kSlotBytes, bar = bar_full + 8 * slot;
+        const uint8_t* hi = p.wpacked + sd.gofs + (uint32_t)k0 * step_bytes;
+        const uint8_t* lo = p.wpacked + sd.gofs + (uint32_t)sd.lo_off16 * 16u + (uint32_t)k0 * step_bytes;
+        mbar_wait_backoff(bar_empty + 8 * slot, ph ^ 1);
+        mbar_arrive_expect_tx(bar, PASSES == 3 ? 2 * part : part);
+        bulk_g2s(dst, hi, part, bar);
+        if (PASSES == 3) bulk_g2s(dst + part, lo, part, bar);
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -407,7 +489,7 @@ __device__ __forceinline__ void mma_issue(float (&d)[64], uint64_t a_hi, uint64_
 
 // Slot j of stage sd into the accumulator d: wait for it to land, issue its kn (<= KMAX) K16 steps and release the
 // previous slot once they are issued (wait_group 1: the previous slot's MMAs are done).
-template <int N, int PASSES, int FMT>
+template <int N, int PASSES, int FMT, int NS>
 __device__ __forceinline__ void mma_slot(float (&d)[64], const StageDesc& sd, int j, uint32_t acc, uint32_t ring_s,
                                          uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
                                          uint32_t op_s, RingPos& rp, bool leader) {
@@ -424,7 +506,7 @@ __device__ __forceinline__ void mma_slot(float (&d)[64], const StageDesc& sd, in
   }
   int k0, kn;
   slot_ksteps(sd, j, k0, kn);
-  const uint32_t slot = ring_slot(rp.gs), ph = ring_phase(rp.gs);
+  const uint32_t slot = ring_slot<NS>(rp.gs), ph = ring_phase<NS>(rp.gs);
   const uint32_t b = ring_s + slot * (uint32_t)kSlotBytes;
   const uint64_t ad_hi = make_smem_desc_noswz(a_hi, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
   const uint64_t ad_lo = make_smem_desc_noswz(a_lo, kOpKCoreBytes, 128) + (uint64_t)(k0 * a_inc16);
@@ -437,13 +519,13 @@ __device__ __forceinline__ void mma_slot(float (&d)[64], const StageDesc& sd, in
   else if (kn == 3) mma_issue<N, PASSES, FMT, (KMAX < 3 ? KMAX : 3)>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
   else mma_issue<N, PASSES, FMT, KMAX>(d, ad_hi, ad_lo, b_hi, b_lo, acc);
   wgmma_wait<1>();
-  release_slot(bar_empty, rp.prev, leader);
+  release_slot<NS>(bar_empty, rp.prev, leader);
   rp.prev = (int)slot;
   ++rp.gs;
 }
 
 // The stages [si, si_end) of one half of a step (all of width N) into d.
-template <int N, int PASSES, int FMT>
+template <int N, int PASSES, int FMT, int NS>
 __device__ __forceinline__ void mma_half(float (&d)[64], const MlpProgram& prog, int si, int si_end, uint32_t ring_s,
                                          uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
                                          uint32_t op_s, RingPos& rp, bool leader) {
@@ -453,20 +535,20 @@ __device__ __forceinline__ void mma_half(float (&d)[64], const MlpProgram& prog,
     const uint32_t acc = (sd.flags & F_FIRST) ? 0u : 1u;
 #pragma unroll 1
     for (int j = 0; j < stage_slots(sd); ++j)
-      mma_slot<N, PASSES, FMT>(d, sd, j, j == 0 ? acc : 1u, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+      mma_slot<N, PASSES, FMT, NS>(d, sd, j, j == 0 ? acc : 1u, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
   }
   // retire the half here: no wgmma may be in flight where the N-dispatch merges (the compiler may move accumulators)
   wgmma_wait<0>();
-  release_slot(bar_empty, rp.prev, leader);
+  release_slot<NS>(bar_empty, rp.prev, leader);
   rp.prev = -1;
 }
 
-template <int PASSES, int FMT>
+template <int PASSES, int FMT, int NS>
 __device__ __forceinline__ void mma_half_n(float (&d)[64], int n, const MlpProgram& prog, int si, int si_end, uint32_t ring_s,
                                            uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s, uint32_t dir_s,
                                            uint32_t op_s, RingPos& rp, bool leader) {
 #define PNR_MMA_N(NN) \
-  case NN / 8: mma_half<NN, PASSES, FMT>(d, prog, si, si_end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader); break;
+  case NN / 8: mma_half<NN, PASSES, FMT, NS>(d, prog, si, si_end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader); break;
   switch (n >> 3) {
     PNR_MMA_N(8) PNR_MMA_N(16) PNR_MMA_N(24) PNR_MMA_N(32) PNR_MMA_N(40) PNR_MMA_N(48) PNR_MMA_N(56) PNR_MMA_N(64)
     PNR_MMA_N(72) PNR_MMA_N(80) PNR_MMA_N(88) PNR_MMA_N(96) PNR_MMA_N(104) PNR_MMA_N(112) PNR_MMA_N(120) PNR_MMA_N(128)
@@ -487,16 +569,29 @@ __device__ __forceinline__ void mma_half_n(float (&d)[64], int n, const MlpProgr
 // one packed 32-bit word per row and part, and a quad of lanes covers one 16-byte core-matrix row (conflict-free: a
 // warp stores 8 consecutive 16-byte rows).  `bias` = the step's bias + 2(t%4), `op_t` = the operand region + this
 // thread's byte offset r0 * 16 + (t%4) * 4.
-template <int PASSES, int FMT, int HALF>
-__device__ __forceinline__ void epi_regs_act(const float (&d)[64], const float* bias, uint8_t* op_t, uint32_t& vmax) {
+// SIGMA: the sigma step (128-row kernel), which also forms the sigma head on the same activations (head_dot_*): every
+// 8-column block j of rows r0 and r0 + 8 is summed over the quad, and lane t%4 = i + 2 sh adds the blocks of row r0 + 8i
+// in column share sh (j < 8 of a half: share 0) to `sig`; `wsig` = the sigma weights + 2(t%4) like `bias`.
+template <int PASSES, int FMT, int HALF, bool SIGMA>
+__device__ __forceinline__ void epi_regs_act_sig(const float (&d)[64], const float* bias, const float* wsig, uint8_t* op_t,
+                                                 uint32_t& vmax, float& sig) {
   constexpr int kHi = ((kColAHi - kColOpBase) / 4 + 16 * HALF) * kOpKCoreBytes;
   constexpr int kLo = ((kColALo - kColOpBase) / 4 + 16 * HALF) * kOpKCoreBytes;
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const float2 b = *reinterpret_cast<const float2*>(bias + 128 * HALF + 8 * j);
     uint32_t h0, l0, h1, l1;
-    split_x2<FMT>(relu_nan(d[4 * j + 0] + b.x), relu_nan(d[4 * j + 1] + b.y), h0, l0);
-    split_x2<FMT>(relu_nan(d[4 * j + 2] + b.x), relu_nan(d[4 * j + 3] + b.y), h1, l1);
+    const float v00 = relu_nan(d[4 * j + 0] + b.x), v01 = relu_nan(d[4 * j + 1] + b.y);
+    const float v10 = relu_nan(d[4 * j + 2] + b.x), v11 = relu_nan(d[4 * j + 3] + b.y);
+    if (SIGMA) {
+      const float2 w = *reinterpret_cast<const float2*>(wsig + 128 * HALF + 8 * j);
+      const float b0 = head_dot_block_quad(head_dot_pair(v00, w.x, v01, w.y));
+      const float b1 = head_dot_block_quad(head_dot_pair(v10, w.x, v11, w.y));
+      const int lt = (int)(threadIdx.x & 3);
+      if ((lt >> 1) == (j < 8 ? 0 : 1)) sig = head_dot_add_block(sig, (lt & 1) ? b1 : b0);
+    }
+    split_x2<FMT>(v00, v01, h0, l0);
+    split_x2<FMT>(v10, v11, h1, l1);
 #ifndef PNR_ABL_NOVMAX
     vmax = __vimax3_u16x2(vmax, h0, h1);   // range check, as in epi_group_act
 #endif
@@ -507,6 +602,11 @@ __device__ __forceinline__ void epi_regs_act(const float (&d)[64], const float* 
       *reinterpret_cast<uint32_t*>(op_t + kLo + j * kOpKCoreBytes + 8 * 16) = l1;
     }
   }
+}
+template <int PASSES, int FMT, int HALF>
+__device__ __forceinline__ void epi_regs_act(const float (&d)[64], const float* bias, uint8_t* op_t, uint32_t& vmax) {
+  float unused = 0.f;
+  epi_regs_act_sig<PASSES, FMT, HALF, false>(d, bias, nullptr, op_t, vmax, unused);
 }
 
 // Can step `ed` run its epilogue in registers?  (Its halves are N = 128 whenever ed.n = 256 and ed.n0 = 128.)
@@ -549,15 +649,16 @@ constexpr bool kAblNoTrunkEpi = true;
 constexpr bool kAblNoTrunkEpi = false;
 #endif
 
-// Embeddings of the tile from s_base: threads 0-63 gamma(x) of row t, threads 64-127 gamma(d) of row t - 64.  A
-// hash-grid trunk input (p.hash_table set) replaces gamma(x) by h(x): both threads of a row form its point, the xyz
-// thread gathers the first half of the feature core rows, the dir thread (after gamma(d), if any) the second half.
+// Embeddings of the warpgroup's 64 rows from s_base into its regions `emb` and `dir`: threads (tid, in the
+// warpgroup) 0-63 gamma(x) of row tid, threads 64-127 gamma(d) of row tid - 64.  A hash-grid trunk input (p.hash_table
+// set) replaces gamma(x) by h(x): both threads of a row form its point, the xyz thread gathers the first half of the
+// feature core rows, the dir thread (after gamma(d), if any) the second half.  `bar`: the warpgroup's named barrier.
 template <int PASSES, int FMT, bool BWD>
-__device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgram& prog, uint8_t* smem, int64_t s_base,
-                                              uint32_t& vmax) {
-  named_bar_sync(1, kConsumerThreads);    // the previous tile's end-of-tile reads are done
-  const int erow = threadIdx.x & (kRows - 1);
-  const bool dir_thread = threadIdx.x >= kRows;
+__device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgram& prog, uint8_t* emb, uint8_t* dir,
+                                              int tid, int bar, int64_t s_base, uint32_t& vmax) {
+  named_bar_sync(bar, kConsumerThreads);  // the previous tile's end-of-tile reads are done
+  const int erow = tid & (kRows - 1);
+  const bool dir_thread = tid >= kRows;
   const bool hashgrid = p.hash_table != nullptr;
   if (!kAblNoPrologue && (!(BWD && dir_thread) || hashgrid)) {
     int64_t se = s_base + erow;
@@ -583,9 +684,9 @@ __device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgr
       for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(d[c], nrm);
     }
     if (dir_thread) {
-      if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, smem + kSmemDir, smem + kSmemDir + kDirPartBytes, erow, vmax);
+      if (!BWD) encode_row<PASSES, FMT, 4, 32>(d, prog.Ld, dir, dir + kDirPartBytes, erow, vmax);
     } else if (!hashgrid) {
-      encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, smem + kSmemEmb, smem + kSmemEmb + kEmbPartBytes, erow, vmax);
+      encode_row<PASSES, FMT, 10, 64>(x, prog.Lx, emb, emb + kEmbPartBytes, erow, vmax);
     }
     if (hashgrid) {
       // a non-finite point is flagged here: the clamp below sends a NaN to the corner (0,0,0), whose features are
@@ -594,18 +695,18 @@ __device__ __forceinline__ void tile_prologue(const MlpParams& p, const MlpProgr
       float v[3];
       hash_normalize(x, p.hash_aabb, v);
       const int nc = ((p.hash_L * p.hash_F + 15) & ~15) / 8, half = (nc + 1) / 2;   // core rows the MMAs read
-      hash_rows_f<PASSES, FMT>(p, v, dir_thread ? half : 0, dir_thread ? nc : half, smem + kSmemEmb,
-                               smem + kSmemEmb + kEmbPartBytes, erow, vmax);
+      hash_rows_f<PASSES, FMT>(p, v, dir_thread ? half : 0, dir_thread ? nc : half, emb, emb + kEmbPartBytes, erow,
+                               vmax);
     }
   }
   fence_proxy_async_smem();   // generic-proxy stores -> visible to the MMAs' async proxy
-  named_bar_sync(1, kConsumerThreads);
+  named_bar_sync(bar, kConsumerThreads);
 }
 
 // The MMAs of step `ed` from stage si on: its stages up to the one that closes it, those of the first half (accumulator
 // column ed.acc_col) into acc0, the rest into acc1; a ring slot is released when the MMAs that read it have retired.
 // Returns the next step's first stage.
-template <int PASSES, int FMT>
+template <int PASSES, int FMT, int NS>
 __device__ __forceinline__ int step_mmas(float (&acc0)[64], float (&acc1)[64], const MlpProgram& prog, const EpiDesc& ed,
                                          int si, uint32_t ring_s, uint32_t bar_full, uint32_t bar_empty, uint32_t emb_s,
                                          uint32_t dir_s, uint32_t op_s, RingPos& rp, bool leader) {
@@ -621,21 +722,22 @@ __device__ __forceinline__ int step_mmas(float (&acc0)[64], float (&acc1)[64], c
   // live accumulators - a move in a divergent path would serialize every wgmma
 #pragma unroll
   for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
-  mma_half_n<PASSES, FMT>(acc0, prog.st[si].n, prog, si, h1, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+  mma_half_n<PASSES, FMT, NS>(acc0, prog.st[si].n, prog, si, h1, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
   if (h1 < end)
-    mma_half_n<PASSES, FMT>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
+    mma_half_n<PASSES, FMT, NS>(acc1, prog.st[h1].n, prog, h1, end, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, leader);
   return end;
 }
 
-// A trunk step's epilogue in registers: both halves through epi_regs_act (bias_t, op_t as there) between two barriers.
+// A trunk step's epilogue in registers: both halves through epi_regs_act (bias_t, op_t as there) between two barriers
+// of the warpgroup (named barrier `bar`).
 template <int PASSES, int FMT>
 __device__ __forceinline__ void trunk_epilogue(const float (&acc0)[64], const float (&acc1)[64], const float* bias_t,
-                                               uint8_t* op_t, uint32_t& vmax) {
-  named_bar_sync(1, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
+                                               uint8_t* op_t, uint32_t& vmax, int bar) {
+  named_bar_sync(bar, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
   epi_regs_act<PASSES, FMT, 0>(acc0, bias_t, op_t, vmax);
   epi_regs_act<PASSES, FMT, 1>(acc1, bias_t, op_t, vmax);
-  fence_proxy_async_smem();              // the next step's MMAs read what was just stored
-  named_bar_sync(1, kConsumerThreads);
+  fence_proxy_async_smem();                // the next step's MMAs read what was just stored
+  named_bar_sync(bar, kConsumerThreads);
 }
 
 // End of a COMP tile (one warp, lanes stride channels): fold its per-quarter sums (qsum half `par`) into the open ray's
@@ -722,29 +824,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
 
   if (warp == kConsumerThreads / 32) {
     // =============================================================== weight stream (one elected thread)
-    if (elect_one()) {
-      uint32_t gs = 0;  // global slot counter
-      for (int it = 0; it < n_iter; ++it) {
-        for (int si = 0; si < n_stages; ++si) {
-          const StageDesc& sd = prog.st[si];
-          const uint32_t step_bytes = (uint32_t)sd.n * 32u;   // one K16 step of one image
-          const int nslots = stage_slots(sd);
-          for (int j = 0; j < nslots; ++j, ++gs) {
-            int k0, kn;
-            slot_ksteps(sd, j, k0, kn);
-            const uint32_t slot = ring_slot(gs), ph = ring_phase(gs);
-            const uint32_t part = (uint32_t)kn * step_bytes;   // bytes of one image in this slot
-            const uint32_t dst = ring_s + slot * (uint32_t)kSlotBytes, bar = bar_full + 8 * slot;
-            const uint8_t* hi = p.wpacked + sd.gofs + (uint32_t)k0 * step_bytes;
-            const uint8_t* lo = p.wpacked + sd.gofs + (uint32_t)sd.lo_off16 * 16u + (uint32_t)k0 * step_bytes;
-            mbar_wait_backoff(bar_empty + 8 * slot, ph ^ 1);
-            mbar_arrive_expect_tx(bar, PASSES == 3 ? 2 * part : part);
-            bulk_g2s(dst, hi, part, bar);
-            if (PASSES == 3) bulk_g2s(dst + part, lo, part, bar);
-          }
-        }
-      }
-    }
+    if (elect_one()) stream_weights<PASSES, kSlots>(p, prog, n_iter, ring_s, bar_full, bar_empty);
   } else {
     // =============================================================== consumer warpgroup
     const int q = warp & 1, ch = warp >> 1;     // 32-row group (a "quarter" of the compositing code) ; column share
@@ -778,8 +858,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
         for (int si = 0; si < n_stages; ++si) {
 #pragma unroll 1
           for (int j = 0; j < stage_slots(prog.st[si]); ++j, ++rp.gs) {
-            mbar_wait(bar_full + 8 * ring_slot(rp.gs), ring_phase(rp.gs));
-            release_slot(bar_empty, (int)ring_slot(rp.gs), lane == 0);
+            mbar_wait(bar_full + 8 * ring_slot<kSlots>(rp.gs), ring_phase<kSlots>(rp.gs));
+            release_slot<kSlots>(bar_empty, (int)ring_slot<kSlots>(rp.gs), lane == 0);
           }
         }
         continue;
@@ -787,15 +867,15 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
       const int par = it & 1;
       float* qsum_q = qsum + (par * kQuarters + q) * kCompChPad;     // this quarter's partial sums of this tile
       float w_mine = 0.f;                                            // this row's compositing weight (COMP)
-      float sig = 0.f;
+      float sig = 0.f;                                               // this share's sigma sum (head_dot_*)
 
-      tile_prologue<PASSES, FMT, BWD>(p, prog, smem, s_base, vmax);
+      tile_prologue<PASSES, FMT, BWD>(p, prog, smem + kSmemEmb, smem + kSmemDir, threadIdx.x, 1, s_base, vmax);
       int si = 0;
       for (int st = 0; st < n_steps; ++st) {
         const EpiDesc ed = prog.ep[st];
-        si = step_mmas<PASSES, FMT>(acc0, acc1, prog, ed, si, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
+        si = step_mmas<PASSES, FMT, kSlots>(acc0, acc1, prog, ed, si, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s, rp, lane == 0);
         if (!BWD && !kAblNoTrunkEpi && trunk_in_regs(ed)) {
-          trunk_epilogue<PASSES, FMT>(acc0, acc1, consts + ed.bias_off + 2 * (lane & 3), op_t, vmax);
+          trunk_epilogue<PASSES, FMT>(acc0, acc1, consts + ed.bias_off + 2 * (lane & 3), op_t, vmax, 1);
           continue;
         }
 
@@ -804,7 +884,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
         const float* aux = consts + ed.aux_off;
         const bool to_a = BWD ? epi_writes_a(ed.kind) : ed.kind == EPI_RELU_TO_A;
         const int ng = ed.n >> 4;
-        float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+        float c0 = 0.f, c1 = 0.f, c2 = 0.f;   // this share's rgb sums (head_dot_*)
         uint32_t smax = 0;   // backward programs: largest hi-part magnitudes of the A operand this step produces (16x2)
         // backward programs: this row's sign patterns and its row of the incoming gradient (tail rows read row S-1)
         uint16_t* mask_row = reinterpret_cast<uint16_t*>(smem + kSmemMask) + row;
@@ -840,7 +920,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
             if (to_a) {
               uint32_t hi[8], lo[8];
               if (BWD) epi_group_bwd<PASSES, FMT>(r, g, ed, bias, mask_row, gin, stash_row, p.grad_scale, p.grad_unscale, smax, hi, lo);
-              else epi_group_act<PASSES, FMT>(r, g, ed, bias, aux, sig, vmax, hi, lo);
+              else epi_group_act<PASSES, FMT>(r, g, ed, bias, aux, p.head_blocks != 0, sig, vmax, hi, lo);
               epi_group_store<PASSES>(g, ed, op, row, hi, lo);
             } else {
               // EPI_LOGITS: where this group's columns go (the columns from n0 on may be a logit layer of its own)
@@ -854,7 +934,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
                 if (valid && ed.kind == EPI_ACT_OUT) epi_group_actout(r, g, bias, out_row);
                 else if (valid) epi_group_gradout(r, g, ed.n_valid, ed.n_valid1 != 0, out_vec, p.grad_unscale, out_row);
               } else if (ed.kind == EPI_VIEW_RGB) {
-                epi_group_rgb(r, g, ed, bias, aux, c0, c1, c2);
+                epi_group_rgb(r, g, ed, bias, aux, p.head_blocks != 0, c0, c1, c2);
               } else if (COMP) {
                 epi_group_logits_comp(r, g, out_c0, out_valid, out_ch, bias, w_mine, lane, qsum_q);
               } else if (valid) {
@@ -876,9 +956,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
             named_bar_sync(1, kConsumerThreads);
             if (ch == 0 && (COMP || valid)) {
               const float* b3 = consts + prog.rgb_bias_off;
-              const float* other = part + (kRows + row) * 4;   // fixed order: deterministic sums
-              float o0 = c0 + other[0], o1 = c1 + other[1], o2 = c2 + other[2], o3 = mine[3] + other[3];
-              o0 += b3[0]; o1 += b3[1]; o2 += b3[2]; o3 += consts[prog.sigma_bias_off];
+              const float* other = part + (kRows + row) * 4;   // share 0 (this thread's) + share 1: head_dot_total
+              const float o0 = head_dot_total(c0, other[0], b3[0]), o1 = head_dot_total(c1, other[1], b3[1]);
+              const float o2 = head_dot_total(c2, other[2], b3[2]);
+              const float o3 = head_dot_total(mine[3], other[3], consts[prog.sigma_bias_off]);
               if (COMP) {   // colours weighted and summed over this aligned group of 32 samples (w = 0 on dummy rows)
                 const float r0 = warp_sum32(w_mine * comp_sigmoid(o0));
                 const float r1 = warp_sum32(w_mine * comp_sigmoid(o1));
@@ -921,9 +1002,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
               const float z_next = has_next ? p.z[sq + lane + 1] : 0.f;
               const float* rr = p.rays + r * 6;
               const float dist = comp_dist(zi, z_next, has_next, comp_dnorm(rr[3], rr[4], rr[5]));
-              float sraw = part[row * 4 + 3];
-              sraw += part[(kRows + row) * 4 + 3];
-              sraw += consts[prog.sigma_bias_off];
+              const float sraw = head_dot_total(part[row * 4 + 3], part[(kRows + row) * 4 + 3], consts[prog.sigma_bias_off]);
               const bool masked = p.mask_outside && p.sample_box != nullptr && p.sample_box[sq + lane] < 0;
               alpha = comp_alpha(sraw, dist, masked);
               t = 1.0f - alpha + 1e-10f;
@@ -972,6 +1051,156 @@ __global__ void __launch_bounds__(kMlpThreads, 1) mlp_fused_kernel(const __grid_
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// 128-row kernel: forward programs without heads (mlp_rows128_ok).  384 threads: consumer warpgroups 0 and 1 own rows
+// [0, 64) and [64, 128) of a 128-sample tile, each with its own operand block (mlp_program.h) and named barrier
+// (kBar128 + g); warpgroup 2 streams the weights (one elected thread) into a 3-slot ring that both consumers read, so
+// a slot feeds the MMAs of 128 rows and the stream per sample is halved.  The weight-stream warpgroup lowers its
+// registers to 24 and the consumers raise theirs to 240 (384 x 168 = 128 x 24 + 256 x 240).  Two consumer warps per
+// SM sub-partition: one warpgroup's prologue and epilogues run while the other's MMAs keep the tensor pipe busy.  The
+// two warpgroups meet only at the ring's barriers.  Every epilogue runs from the accumulator registers: the trunk steps
+// through epi_regs_act (the 64-row kernel's bytes), the sigma step adds the sigma head's chains, the view step forms the
+// rgb head and writes the raw rows; the head sums follow head_dot_*, so the outputs are the 64-row kernel's bits.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBar128 = 4;   // named barriers kBar128 + g (1 and 3 are the 64-row kernel's)
+
+// The view step's epilogue (one N = 128 half in `d`): the rgb head (head_dot_*) of rows r0 and r0 + 8 (bias_t, wrgb_t
+// = the step's bias and rgb weights + 2(t%4)).  Lane t%4 = i + 2 sh sums row r0 + 8i's blocks in column share sh; lane i
+// adds the other share and writes row r0 + 8i of `raw`.
+__device__ __forceinline__ void view_epilogue128(const float (&d)[64], const float* bias_t, const float* wrgb_t,
+                                                 const float* consts, const MlpProgram& prog, const float* sig_row,
+                                                 float* raw, int CH, int64_t s_r0, int64_t S, int r0, int lane) {
+  const int lt = lane & 3, i_mine = lt & 1, sh_mine = lt >> 1;
+  float c[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float2 b = *reinterpret_cast<const float2*>(bias_t + 8 * j);
+    const float v00 = relu_nan(d[4 * j + 0] + b.x), v01 = relu_nan(d[4 * j + 1] + b.y);
+    const float v10 = relu_nan(d[4 * j + 2] + b.x), v11 = relu_nan(d[4 * j + 3] + b.y);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const float2 w = *reinterpret_cast<const float2*>(wrgb_t + k * 128 + 8 * j);
+      const float b0 = head_dot_block_quad(head_dot_pair(v00, w.x, v01, w.y));
+      const float b1 = head_dot_block_quad(head_dot_pair(v10, w.x, v11, w.y));
+      if (sh_mine == (j < 8 ? 0 : 1)) c[k] = head_dot_add_block(c[k], i_mine ? b1 : b0);
+    }
+  }
+  float o[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float other = __shfl_xor_sync(0xffffffffu, c[k], 2);   // the same row's other share
+    o[k] = head_dot_total(c[k], other, consts[prog.rgb_bias_off + k]);
+  }
+  const int64_t s = s_r0 + 8 * i_mine;
+  if (sh_mine == 0 && s < S) {
+    const float o3 = __fadd_rn(sig_row[r0 + 8 * i_mine], consts[prog.sigma_bias_off]);
+    float* dst = raw + s * CH;
+    if (CH == 4) {
+      *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o3);
+    } else {
+      dst[0] = o[0]; dst[1] = o[1]; dst[2] = o[2]; dst[3] = o3;
+    }
+  }
+}
+
+template <int PASSES, int FMT>
+__global__ void __launch_bounds__(kMlp128Threads, 1) mlp_rows128_kernel(const __grid_constant__ MlpLaunch L) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const MlpParams& p = L.p;
+  const MlpProgram& prog = L.prog;
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  const int n_iter = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kSmem128Bars);
+  const uint32_t bar_full = smem_u32(&bars[0]);              // [kSlots128] weight slot landed
+  const uint32_t bar_empty = smem_u32(&bars[kSlots128]);     // [kSlots128] released by all 8 consumer warps
+  const uint32_t ring_s = smem_u32(smem + kSmem128Ring);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kSlots128; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 2 * kConsumerThreads / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    // =============================================================== weight stream (one elected thread)
+    setmaxnreg_dec<24>();
+    if ((threadIdx.x >> 5) == 2 * kConsumerThreads / 32 && elect_one())
+      stream_weights<PASSES, kSlots128>(p, prog, n_iter, ring_s, bar_full, bar_empty);
+    return;   // nothing waits for the other warps of the warpgroup
+  }
+  // =============================================================== consumer warpgroup wg
+  setmaxnreg_inc<240>();
+  const int tid = threadIdx.x & (kConsumerThreads - 1), w = tid >> 5, bar = kBar128 + wg;
+  uint8_t* blk = smem + kSmem128Blk + wg * kBlk128Bytes;
+  // the operand columns [256, 512) are at blk: addresses formed from kColOpBase (mma_slot, epi_regs_act) are taken
+  // from `op`, which lies the head columns' 32 K-cores before it (still inside the map: blk >= 48 KB)
+  static_assert(kSmem128Blk >= (kColAHi - kColOpBase) / 4 * kOpKCoreBytes, "op base inside shared memory");
+  uint8_t* op = blk + kBlk128Op - (kColAHi - kColOpBase) / 4 * kOpKCoreBytes;
+  uint8_t* op_t = op + (w * 16 + (lane >> 2)) * 16 + (lane & 3) * 4;   // this thread's word of a register epilogue
+  const uint32_t op_s = smem_u32(op), emb_s = smem_u32(blk + kBlk128Emb), dir_s = smem_u32(blk + kBlk128Dir);
+  float* sig_row = reinterpret_cast<float*>(smem + kSmem128Sig) + kRows * wg;   // the warpgroup's rows
+  const int r0 = w * 16 + (lane >> 2);
+  const float* consts = p.consts;
+  RingPos rp{0u, -1};
+  uint32_t vmax = 0;
+  float acc0[64], acc1[64];
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {   // (n_iter is not kept live here)
+    const int64_t s_base = (int64_t)tile * kRows128 + kRows * wg;
+    if (kStreamOnly || s_base >= p.S) {
+      // no sample of this warpgroup in the tile: take the weight slots, compute nothing
+#pragma unroll 1
+      for (int si = 0; si < prog.n_stages; ++si) {
+#pragma unroll 1
+        for (int j = 0; j < stage_slots(prog.st[si]); ++j, ++rp.gs) {
+          mbar_wait(bar_full + 8 * ring_slot<kSlots128>(rp.gs), ring_phase<kSlots128>(rp.gs));
+          release_slot<kSlots128>(bar_empty, (int)ring_slot<kSlots128>(rp.gs), lane == 0);
+        }
+      }
+      continue;
+    }
+    tile_prologue<PASSES, FMT, false>(p, prog, blk + kBlk128Emb, blk + kBlk128Dir, tid, bar, s_base, vmax);
+    int si = 0;
+    for (int st = 0; st < prog.n_steps; ++st) {
+      const EpiDesc ed = prog.ep[st];
+      si = step_mmas<PASSES, FMT, kSlots128>(acc0, acc1, prog, ed, si, ring_s, bar_full, bar_empty, emb_s, dir_s, op_s,
+                                             rp, lane == 0);
+      const float* bias_t = consts + ed.bias_off + 2 * (lane & 3);
+      const float* aux_t = consts + ed.aux_off + 2 * (lane & 3);
+      if (ed.kind == EPI_VIEW_RGB) {
+        view_epilogue128(acc0, bias_t, aux_t, consts, prog, sig_row, p.raw, p.CH, s_base + r0, p.S, r0, lane);
+      } else if (kAblNoTrunkEpi && !ed.sigma) {
+        named_bar_sync(bar, kConsumerThreads);
+        named_bar_sync(bar, kConsumerThreads);
+      } else if (ed.sigma) {
+        float sg = 0.f;   // lane t%4 = i + 2 sh: row r0 + 8i, column share sh
+        named_bar_sync(bar, kConsumerThreads);   // every warp's MMAs of the step have retired: its input is dead
+        epi_regs_act_sig<PASSES, FMT, 0, true>(acc0, bias_t, aux_t, op_t, vmax, sg);
+        epi_regs_act_sig<PASSES, FMT, 1, true>(acc1, bias_t, aux_t, op_t, vmax, sg);
+        fence_proxy_async_smem();                // the next step's MMAs read what was just stored
+        named_bar_sync(bar, kConsumerThreads);
+        // share 0 + share 1: lane t%4 = i < 2 keeps row r0 + 8i (and reads it back in the view epilogue)
+        const float sg_other = __shfl_xor_sync(0xffffffffu, sg, 2);
+        if ((lane & 3) < 2) sig_row[r0 + 8 * (lane & 1)] = __fadd_rn(sg, sg_other);
+      } else {
+        trunk_epilogue<PASSES, FMT>(acc0, acc1, bias_t, op_t, vmax, bar);
+      }
+    }
+  }
+  if (p.status != nullptr && ((vmax & 0xFFFFu) >= inf_bits16<FMT>() || (vmax >> 16) >= inf_bits16<FMT>()))
+    atomicOr(p.status, 1u);
+}
+
+template <int PASSES, int FMT>
+static int launch_rows128(const MlpLaunch& L, int dev, int grid, cudaStream_t stream) {
+  const int rc = opt_in_smem((const void*)mlp_rows128_kernel<PASSES, FMT>, kSmem128Total, dev);
+  if (rc != PNR_OK) return rc;
+  mlp_rows128_kernel<PASSES, FMT><<<grid, kMlp128Threads, kSmem128Total, stream>>>(L);
+  PNR_LAUNCH_CHECK("mlp_rows128_kernel");
+  return PNR_OK;
+}
+
 template <int PASSES, int FMT, bool COMP, bool BWD = false>
 static int launch_one(const MlpLaunch& L, int dev, int grid, cudaStream_t stream) {
   constexpr int kSmem = COMP ? kSmemTotalComp : kSmemTotal;
@@ -982,15 +1211,35 @@ static int launch_one(const MlpLaunch& L, int dev, int grid, cudaStream_t stream
   return PNR_OK;
 }
 
-// Launches on the CURRENT device (the caller has made the context's device current).  mode 1: the
-// compositing-epilogue variant; the launch's rays_per_cta is set here (whole rays per CTA, so that every CTA's range
-// starts on a 32-sample boundary).  mode 2: L.prog is a backward program (x3 precisions only).
-int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream) {
+// Launches on the CURRENT device (the caller has made the context's device current).  mode 0: raw rows, on the
+// 128-row kernel when `rows` is 128, or 0 and the program passes mlp_rows128_ok, else on the 64-row kernel (`rows` 64);
+// rows = 128 for a program that fails mlp_rows128_ok is refused.  mode 1: the compositing-epilogue variant; the
+// launch's rays_per_cta is set here (whole rays per CTA, so that every CTA's range starts on a 32-sample boundary).
+// mode 2: L.prog is a backward program (x3 precisions only).  Modes 1 and 2 run on the 64-row kernel whatever `rows`.
+int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream, int rows) {
   const bool composite = mode == kMlpComposite;
   int dev = 0;
   const int rc = current_device("launch_mlp", &dev);
   if (rc != PNR_OK) return rc;
   const int sms = num_sms(dev);
+  const bool ok = mlp_rows128_ok(L.prog);
+  L.p.head_blocks = ok ? 1 : 0;   // such a program sums its heads as the 128-row kernel does, whichever kernel runs it
+  if (mode == kMlpForward && rows != 64) {
+    if (rows == 128 && !ok)
+      return set_error(PNR_ERR_UNSUPPORTED, "launch_mlp: this network's program does not run on the 128-row kernel "
+                                            "(a 256-wide network without heads does)");
+    if (ok) {
+      const int64_t tiles = (L.p.S + kRows128 - 1) / kRows128;
+      PNR_CHECK_ARG(tiles < ((int64_t)1 << 31), "launch_mlp: too many samples");
+      L.p.num_tiles = (int32_t)tiles;
+      const int grid = L.p.num_tiles < sms ? L.p.num_tiles : sms;
+      if (grid <= 0) return PNR_OK;
+      if (fmt == kFmtF16) return passes == 3 ? launch_rows128<3, kFmtF16>(L, dev, grid, stream)
+                                             : launch_rows128<1, kFmtF16>(L, dev, grid, stream);
+      return passes == 3 ? launch_rows128<3, kFmtBF16>(L, dev, grid, stream)
+                         : launch_rows128<1, kFmtBF16>(L, dev, grid, stream);
+    }
+  }
   const int64_t tiles = (L.p.S + kRows - 1) / kRows;
   PNR_CHECK_ARG(tiles < ((int64_t)1 << 31), "launch_mlp: too many samples");
   L.p.num_tiles = (int32_t)tiles;

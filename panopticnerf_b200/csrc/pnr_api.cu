@@ -23,7 +23,7 @@ int set_error(int code, const char* fmt, ...) {
 }
 void count_launch(int n) { g_launches += n; }
 
-int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream);  // mlp_wgmma.cu
+int launch_mlp(MlpLaunch& L, int passes, int fmt, int mode, cudaStream_t stream, int rows = 0);  // mlp_wgmma.cu
 
 }  // namespace pnr
 
@@ -64,6 +64,7 @@ struct pnr_ctx {
   PackedProgram prog[kNumPrograms];
   uint32_t* d_status = nullptr; // sticky range-check word of the fused MLP (bit 0: activation out of operand range)
   const float* hash_table = nullptr;   // hash-grid contexts: the caller's table (pnr_bind_hashgrid_table), not owned
+  int32_t mlp_rows = 0;   // raw-row launches: 0 = the tile the program allows, 64 or 128 (pnr_set_mlp_rows)
   uint32_t hash_res[kHashMaxLevels] = {};
   float* d_V = nullptr;   // V of the load or of the last pnr_update_weights: what programs are packed from on the device
   std::vector<int64_t> v_off, shapes;   // V's layout (Builder::v_off); the shapes given to pnr_load_weights
@@ -914,7 +915,22 @@ extern "C" int pnr_mlp_forward(pnr_ctx* ctx, const float* pts, const float* view
     return rc;
   L->p.CH = 4 + ctx->cfg.num_classes + ctx->cfg.num_instances;
   L->p.raw = raw;
-  return launch_mlp(*L, ctx->passes, ctx->fmt, kMlpForward, (cudaStream_t)stream);
+  return launch_mlp(*L, ctx->passes, ctx->fmt, kMlpForward, (cudaStream_t)stream, ctx->mlp_rows);
+}
+
+extern "C" int pnr_set_mlp_rows(pnr_ctx* ctx, int32_t rows) {
+  PNR_CHECK_ARG(ctx, "pnr_set_mlp_rows: null context");
+  PNR_CHECK_ARG(rows == 0 || rows == 64 || rows == 128, "pnr_set_mlp_rows: rows=%d not in {0, 64, 128}", rows);
+  ctx->mlp_rows = rows;
+  return PNR_OK;
+}
+
+extern "C" int pnr_program_tile_rows(const void* program, size_t program_bytes, int32_t* rows) {
+  PNR_CHECK_ARG(program && rows, "pnr_program_tile_rows: null pointer");
+  PNR_CHECK_ARG(program_bytes == sizeof(MlpProgram), "pnr_program_tile_rows: %zu bytes, a program has %zu",
+                program_bytes, sizeof(MlpProgram));
+  *rows = mlp_rows128_ok(*static_cast<const MlpProgram*>(program)) ? kRows128 : kRows;
+  return PNR_OK;
 }
 
 extern "C" int pnr_mlp_composite(pnr_ctx* ctx, const float* rays, const float* z, int64_t R, int32_t N,

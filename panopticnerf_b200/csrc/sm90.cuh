@@ -107,6 +107,14 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ---------------------------------------------------------------- register reallocation between warpgroups
+// Every warp of the warpgroup executes it.  A raise waits until lowered warpgroups have returned enough registers to the
+// CTA's pool, so the sums of the two must fit the registers the kernel was launched with.
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ---------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor, K-major, no swizzle ("interleaved" 8 x 16-byte core matrices, each stored as 128
 // contiguous bytes).  lbo_bytes: distance between the core matrices adjacent in K (one K16 step reads two of them);
