@@ -9,11 +9,10 @@ import pytest
 import torch
 
 import panopticnerf_b200 as PN
-from oracle import reference_losses as OL
-from oracle import reference_renderer as O
 import oracle_instance as OI
 from panopticnerf_b200 import _capi, synthetic as S
 from panopticnerf_b200.lib.train import NetworkWrapper, make_network_wrapper
+from test_gpu_train_chain import record_d_raw, run_chain  # noqa: F401 (record_d_raw: a fixture)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -184,71 +183,22 @@ def test_render_train_without_grad_equals_the_staged_render():
         assert torch.equal(got[k], ref[k]), k
 
 
-def _oracle_net(cfg, net):
-    onet = O.Network(cfg).double()
-    onet.load_state_dict({k: v.detach().cpu().double() for k, v in net.state_dict().items()})
-    return onet
-
-
-def _oracle_chain(cfg, b, out, onet, onet_f, w, thr):
-    """The float64 oracle of one iteration on the depths the GPU sampled: the coarse pass on z_vals_0 (tagged as the
-    oracle tags them), the fine pass on z_vals, and the five terms."""
-    rays = b["rays"].double()
-    o, d = rays[:, :3], rays[:, 3:]
-    kw = dict(num_classes=cfg.num_classes, num_instances=cfg.num_instances, box_sem=b["box_sem"], box_inst=b["box_inst"])
-    box = [out[k].cpu() for k in ("box_id", "t_in", "t_out")]
-    z0, z1 = out["z_vals_0"].cpu(), out["z_vals"].cpu()
-    sb0 = O.tag_samples(z0, *box)
-    assert torch.equal(out["sample_box"].cpu(), O.tag_samples(z1, *box))
-    query = O.Renderer._query
-    o0 = O.raw2outputs(query(None, onet, o, d, z0.double()), z0.double(), d, sample_box=sb0, **kw)
-    o1 = O.raw2outputs(query(None, onet_f, o, d, z1.double()), z1.double(), d, sample_box=out["sample_box"].cpu(), **kw)
-    total, terms = OL.losses(o1["rgb_map"], o0["rgb_map"], o1["depth_map"], o1["semantic_map"], o1["fixed_semantic_map"],
-                             b["rgb"].double(), b["depth"].double(), b["pseudo_label"], None, w[:4])
-    inst, _, label, n = OI.instance_loss(o1["instance_map"], o1["fixed_instance_map"], thr)
-    return total + w[4] * inst, terms, inst, label, n
-
-
-def _cos_norm(a, b):
-    a, b = a.detach().cpu().double().reshape(-1), b.reshape(-1)
-    return float((a * b).sum() / (a.norm() * b.norm())), float(a.norm() / b.norm())
-
-
 @pytest.mark.parametrize("shared", [False, True])
-def test_one_iteration_matches_the_oracle_chain(shared):
-    """cfg3-shaped networks, 64 + 128 samples, primitives, fixed maps and all five terms: the total within 1e-4 and every
-    parameter's gradient by direction and size (cosine >= 0.999, norm within 1 %), as the single-pass chain test."""
+def test_one_iteration_matches_the_oracle_chain(shared, record_d_raw):
+    """cfg3-shaped networks, 64 + 128 samples, primitives, fixed maps and all five terms against the float64 oracle
+    chain pinned to the iteration's own decisions (tests/test_gpu_train_chain.run_chain): maps, total and terms,
+    d_raw of both passes and every parameter's gradient element by element; labels and count exact."""
     cfg = _cfg()
-    net = S.init_network_weights(PN.make_network(cfg), seed=21)
-    fine = None if shared else S.init_network_weights(PN.make_network(cfg), seed=22)
-    onet = _oracle_net(cfg, net)
-    onet_f = onet if shared else _oracle_net(cfg, fine)
-    net = net.to(DEV)
-    fine = fine.to(DEV) if fine is not None else None
-    wrapper = NetworkWrapper(cfg, net, fine)
+    net = S.init_network_weights(PN.make_network(cfg), seed=21).to(DEV)
+    fine = None if shared else S.init_network_weights(PN.make_network(cfg), seed=22).to(DEV)
     b = _batch(cfg, 160, seed=7, step=8)
-    output, loss, stats, image_stats = wrapper(_dev(b))
-    loss.backward()
-    w = wrapper.weights
-    tot_ref, terms_ref, inst_ref, label, n = _oracle_chain(cfg, b, output, onet, onet_f, w, wrapper.inst_min_weight)
-    tot_ref.backward()
-    assert n >= 20 and int(stats["n_inst"]) == n
-    assert torch.equal(output["inst_label"].cpu().long(), label)
-    assert float(loss.detach()) == pytest.approx(float(tot_ref.detach()), rel=1e-4)
-    assert float(stats["inst_loss"]) == pytest.approx(float(inst_ref.detach()), rel=1e-4)
-    assert float(stats["rgb_loss"]) == pytest.approx(float(terms_ref[0].detach()), rel=1e-4)
-    assert image_stats == {} and set(stats) >= {"loss", "rgb_loss", "depth_loss", "sem_loss", "fix_loss", "inst_loss",
-                                                "psnr", "n_inst"}
-    pairs = [(net, onet)] + ([] if shared else [(fine, onet_f)])
-    fine_net = net if shared else fine
-    assert float(fine_net.instance_linears[1].weight.grad.norm()) > 0.0
-    for mine, ref in pairs:
-        for (name, p), (_, q) in zip(mine.named_parameters(), ref.named_parameters()):
-            if float(q.grad.norm()) == 0.0:       # the heads of a separate coarse network: only its colour is supervised
-                assert mine is not fine_net and float(p.grad.norm()) == 0.0, name
-                continue
-            cos, ratio = _cos_norm(p.grad, q.grad)
-            assert cos >= 0.999 and abs(ratio - 1.0) < 1e-2, f"{name}: cosine {cos:.6f}, norm ratio {ratio:.4f}"
+    mine, ref, ob, pins, output = run_chain(cfg, net, fine, b, record_d_raw, f"wrapper shared={shared}")
+    label = OI.instance_labels(ref["maps"]["fine"]["fixed_instance_map"].cpu(), 0.5)
+    n = int((label >= 0).sum())
+    assert n >= 20 and torch.equal(output["inst_label"].cpu().long(), label)
+    assert float((net if shared else fine).instance_linears[1].weight.grad.norm()) > 0.0
+    if not shared:      # only its colour is supervised: the coarse network's heads get exactly nothing
+        assert float(net.instance_linears[1].weight.grad.abs().max()) == 0.0
 
 
 def _train(cfg, net, fine, steps, lr, seed):
