@@ -325,6 +325,57 @@ typedef struct pnr_project_depth_args {
 size_t pnr_project_depth_workspace_bytes(int64_t P, int32_t occlusion_radius);
 int pnr_project_depth(const pnr_project_depth_args* args, void* stream);
 
+/* Depth targets from a rectified stereo pair by semi-global matching (DESIGN 3.4).  Rules (chosen here: the
+ * reference's stereo preprocessing is not public), per pair of H x W RGB8 images (left = the frame's pixels in the
+ * frame store, right = right[i]), D disparities; all integer until step 7:
+ *   1. Grey: g = (4899 R + 9617 G + 1868 B + 8192) >> 14.
+ *   2. Census: a 9 x 7 window (9 wide, 7 high) in raster order, centre excluded, 62 bits; bit k = g(q_k) < g(p);
+ *      coordinates outside the image clamped to the nearest edge pixel.
+ *   3. Cost: C(x, y, d) = popcount(census_L(x, y) ^ census_R(x - d, y)) for x - d >= 0, else 63; d in [0, D).
+ *   4. Aggregation over the 8 directions r in {(+-1, 0), (0, +-1), (+-1, +-1)}:
+ *      L_r(p, d) = C(p, d) + min(L_r(p-r, d), L_r(p-r, d-1) + P1, L_r(p-r, d+1) + P1, m_r(p-r) + P2) - m_r(p-r),
+ *      m_r = min_k L_r(., k), out-of-range d +- 1 terms absent, L_r = C where p - r is outside the image.
+ *      L_r <= 63 + P2, so S(p, d) = sum_r L_r(p, d) <= 8 (63 + 2048) fits in u16.
+ *   5. Winner d* = argmin_d S, lowest d on ties.  Invalid if some d with |d - d*| > 1 has S(d) (100 - U) <
+ *      S(d*) 100 (uniqueness), or unless x - d* >= 0 and |d* - d_R(x - d*)| <= 1 (left-right check), with
+ *      d_R(x') = argmin_d S(x' + d, y, d) over x' + d < W, lowest d on ties.
+ *   6. Subpixel, in sixteenths: for 0 < d* < D - 1, den = max(S(d*-1) + S(d*+1) - 2 S(d*), 1),
+ *      d16 = 16 d* + ((S(d*-1) - S(d*+1)) 16 + den) / (2 den) with C's division (toward zero); else d16 = 16 d*;
+ *      an invalid pixel has d16 = -1.
+ *   7. Depth t = B16 / fp32(d16), one IEEE fp32 division (B16 = fp32(16 (P_rect_00[0,3] - P_rect_01[0,3])) = 16 fx b,
+ *      composed in float64 by the caller), kept when d16 > 0 and min_depth < t <= max_depth, else 0 (no target).
+ *      t is z in rectified camera 0, the units of the pinhole's rays.
+ * Inputs: the frame store rgb8 [P, 3] u8 and pix_offset [F+1] i64 (device), the host table frames [n] of the call's
+ * frames (each of H x W pixels), right [n, H, W, 3] u8 (device).  Outputs (at least one): depth [P] f32 (the store's;
+ * only the pixels of the named frames are rewritten) and disparity [n, H, W] i16 (d16).  A frame whose device
+ * pix_offset range is not H W pixels inside [0, P] is not read and not written (its disparity is -1).  The call is a
+ * fixed sequence of launches on `stream` with the frame table in the kernels' parameters: no host copy, allocation
+ * or synchronisation, so it can be captured in a CUDA graph.
+ * workspace: pnr_stereo_workspace_bytes(n, H, W, D) bytes of device scratch, 16-byte aligned, laid out as four
+ * sections, each starting on a 16-byte boundary (N = n H W): census_L [N] u64, census_R [N] u64, S [N, D] u16,
+ * d_R [N] i16.  0 for arguments outside the accepted ranges.
+ * Refused before any launch (PNR_ERR_ARG, by name): n < 1, H or W outside [1, 65535], D not in {32, 64, .., 256},
+ * P1 / P2 outside 0 <= P1 <= P2 <= 2048, U outside [0, 99], F < 1, P < 1, a frames[i] outside [0, F), a null rgb8,
+ * pix_offset, right or frames, both outputs null, with depth: B16 not finite and > 0, min_depth not finite and > 0,
+ * max_depth not finite and > min_depth; a short or misaligned workspace. */
+typedef struct pnr_stereo_args {
+  const uint8_t* rgb8;          /* [P, 3] device: the frame store's colours                                    */
+  const int64_t* pix_offset;    /* [F+1] device                                                                */
+  int64_t P;
+  int32_t F;
+  const int32_t* frames;        /* [n] host: the store's frame of each pair                                    */
+  int32_t n, H, W;
+  const uint8_t* right;         /* [n, H, W, 3] device                                                         */
+  int32_t D, P1, P2, U;
+  float B16, min_depth, max_depth;
+  float* depth;                 /* [P] device, nullable                                                        */
+  int16_t* disparity;           /* [n, H, W] device, nullable                                                  */
+  void* workspace;
+  size_t workspace_bytes;
+} pnr_stereo_args;
+size_t pnr_stereo_workspace_bytes(int32_t n, int32_t H, int32_t W, int32_t D);
+int pnr_stereo_depth(const pnr_stereo_args* args, void* stream);
+
 /* a7: standalone positional encoding, out [n, 3+6L]. */
 int pnr_encode(const float* x, int64_t n, int32_t L, float* out, void* stream);
 

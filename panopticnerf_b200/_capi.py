@@ -125,6 +125,15 @@ class PnrProjectDepthArgs(C.Structure):
                 ("workspace_bytes", C.c_size_t)]
 
 
+class PnrStereoArgs(C.Structure):
+    """pnr_stereo_args of include/pnr.h (same field order); frames is a host pointer."""
+    _fields_ = [("rgb8", C.c_void_p), ("pix_offset", C.c_void_p), ("P", C.c_int64), ("F", C.c_int32),
+                ("frames", C.c_void_p), ("n", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("right", C.c_void_p),
+                ("D", C.c_int32), ("P1", C.c_int32), ("P2", C.c_int32), ("U", C.c_int32), ("B16", C.c_float),
+                ("min_depth", C.c_float), ("max_depth", C.c_float), ("depth", C.c_void_p), ("disparity", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 SAMPLE_MODE = {"uniform": 0, "intervals": 1}
 COMM_ID_BYTES = 128
 
@@ -152,6 +161,8 @@ SIGNATURES = {
     "pnr_sample_ray_batch": (C.c_int, [C.POINTER(PnrRayBatchArgs), _vp]),
     "pnr_project_depth_workspace_bytes": (C.c_size_t, [_i64, _i32]),
     "pnr_project_depth": (C.c_int, [C.POINTER(PnrProjectDepthArgs), _vp]),
+    "pnr_stereo_workspace_bytes": (C.c_size_t, [_i32, _i32, _i32, _i32]),
+    "pnr_stereo_depth": (C.c_int, [C.POINTER(PnrStereoArgs), _vp]),
     "pnr_encode": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_forward": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp]),
     "pnr_mlp_composite": (C.c_int, [_vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i32,

@@ -83,10 +83,12 @@ def camera_poses(root, seq: str, camera: str):
 
 
 def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00", pseudo_dir=None, depth_dir=None,
-                sem_to_train: Optional[Dict[int, int]] = None, device="cuda", lidar=False) -> FrameSet:
+                sem_to_train: Optional[Dict[int, int]] = None, device="cuda", lidar=False, stereo=False) -> FrameSet:
     """The frames `frames` of sequence `seq` seen by `camera`, on `device` (module docstring: layout and formats).
     lidar: False, True or a dict of `lidar.lidar_depth` options - the depth table from the sequence's Velodyne scans
-    instead of depth_dir's PNGs (the two are refused together)."""
+    instead of depth_dir's PNGs (the two are refused together).
+    stereo: False, True or a dict of `stereo.stereo_depth` options - the depth table from the image_00 / image_01
+    pair by semi-global matching (refused together with depth_dir or lidar)."""
     if camera not in CAMERAS:
         raise ValueError(f"load_frames: camera {camera!r}; one of {CAMERAS}")
     want_lidar = lidar is not False and lidar is not None   # {} is on, with the defaults
@@ -96,6 +98,14 @@ def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00",
             raise ValueError("load_frames: lidar and depth_dir both give the depth table; pass one of them")
         if lidar is not True and (not isinstance(lidar, dict) or set(lidar) - set(LIDAR_OPTIONS)):
             raise ValueError(f"load_frames: lidar={lidar!r}; False, True or a dict with keys from {LIDAR_OPTIONS}")
+    want_stereo = stereo is not False and stereo is not None   # {} is on, with the defaults
+    if want_stereo:
+        from .stereo import STEREO_OPTIONS
+        if depth_dir is not None or want_lidar:
+            raise ValueError("load_frames: stereo and " + ("lidar" if want_lidar else "depth_dir") + " both give the "
+                             "depth table; pass one of them")
+        if stereo is not True and (not isinstance(stereo, dict) or set(stereo) - set(STEREO_OPTIONS)):
+            raise ValueError(f"load_frames: stereo={stereo!r}; False, True or a dict with keys from {STEREO_OPTIONS}")
     root = Path(root)
     frames = [int(f) for f in frames]
     if not frames:
@@ -132,6 +142,9 @@ def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00",
     if want_lidar:
         from .lidar import lidar_depth
         lidar_depth(fs, root, seq, **({} if lidar is True else lidar))
+    if want_stereo:
+        from .stereo import stereo_depth
+        stereo_depth(fs, root, seq, **({} if stereo is True else stereo))
     return fs
 
 
