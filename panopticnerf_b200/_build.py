@@ -80,6 +80,17 @@ def _compile(lib: Path, extra_flags, verbose: bool, objdir: Path) -> Path:
     return lib
 
 
+def build_host_emu() -> Path:
+    """g++ tests/host_emu.cpp -> build/host_emu.so: the host build of csrc/ray_math.h and csrc/stereo_math.h that the
+    CPU tests hold against the oracles.  -ffp-contract=off keeps every fp32 operation rounded on its own, as the
+    kernels' __f*_rn intrinsics do."""
+    out = PKG.parent / "build" / "host_emu.so"
+    out.parent.mkdir(exist_ok=True)
+    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
+                           str(PKG.parent / "tests" / "host_emu.cpp")])
+    return out
+
+
 if __name__ == "__main__":
     import sys
     print(build(force=True, verbose=True))

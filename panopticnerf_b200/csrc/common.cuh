@@ -78,6 +78,23 @@ inline int current_device(const char* what, int* out) {
   return PNR_OK;
 }
 
+// The camera table of a frame-set call (pnr_sample_ray_batch, pnr_project_depth; fn names it): 1..MAX cameras, each a
+// pinhole (0) or fisheye (2) of H, W in [1, 2^size_bits) (size_bits = 31: any positive int32).
+inline int check_cameras(const char* fn, const pnr_ray_camera* cams, int32_t n, int size_bits) {
+  PNR_CHECK_ARG(n >= 1 && n <= PNR_RAY_BATCH_MAX_CAMERAS, "%s: num_cameras=%d outside [1,%d]", fn, n,
+                PNR_RAY_BATCH_MAX_CAMERAS);
+  for (int k = 0; k < n; ++k) {
+    const pnr_ray_camera& c = cams[k];
+    PNR_CHECK_ARG(c.model != 1, "%s: camera %d is equirect (model 1): its rays are device-only (sincosf), so frame "
+                  "sets take pinhole (0) and fisheye (2) cameras", fn, k);
+    PNR_CHECK_ARG(c.model == 0 || c.model == 2, "%s: camera %d model %d (0 pinhole, 2 fisheye)", fn, k, c.model);
+    PNR_CHECK_ARG(c.H >= 1 && c.W >= 1 && (int64_t)c.H < (int64_t(1) << size_bits) &&
+                  (int64_t)c.W < (int64_t(1) << size_bits),
+                  "%s: camera %d size H=%d W=%d outside [1, 2^%d)", fn, k, c.H, c.W, size_bits);
+  }
+  return PNR_OK;
+}
+
 // Lets `kernel` use `bytes` (> 48 KB) of dynamic shared memory on device `dev`.  The opt-in is a per-device function
 // attribute: it is set once per (kernel, device).
 inline int opt_in_smem(const void* kernel, int bytes, int dev) {

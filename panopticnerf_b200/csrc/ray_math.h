@@ -1,6 +1,6 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
-// kernels (ray_kernels.cu, rays_kernel, ray_batch_kernel and the depth kernels in stream_kernels.cu) and host builds used
-// by the CPU tests (tests/host_emu.cpp, tests/host_emu_lidar.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
+// kernels (ray_kernels.cu, rays_kernel, ray_batch_kernel and the depth kernels in stream_kernels.cu) and the host build
+// used by the CPU tests (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
 // here (staging, shuffles, sorts); the rules they apply per ray - the per-primitive intersection step, range clamps,
 // sample depths, output slots, camera directions, batch draws - are the functions below, called by both builds.  One
 // piece stays written out in stratified_kernel and again in host_emu.cpp: the interval test (pnr_tag's rule), because
@@ -601,7 +601,7 @@ PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, i
 // ---------------------------------------------------------------------------------------------- LiDAR depth targets
 // pnr_project_depth (include/pnr.h; DESIGN 3.4): a scan's points projected into a frame, the nearest per pixel.  The
 // projections are the inverses of pnr_pinhole_dir / pnr_fisheye_dir; depth_kernels in stream_kernels.cu and the host
-// build (tests/host_emu_lidar.cpp) call the routines below.
+// build (tests/host_emu.cpp) call the routines below.
 
 PNR_HD uint32_t pnr_float_bits(float x) {
 #if defined(__CUDA_ARCH__)

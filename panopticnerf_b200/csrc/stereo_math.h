@@ -1,7 +1,7 @@
 // stereo_math.h — the per-pixel and per-step rules of pnr_stereo_depth (include/pnr.h, DESIGN 3.4): grey, census,
 // matching cost, one step of a semi-global aggregation path over packed u16 pairs, the left-right minimum and the
 // per-pixel selection.  Shared by the kernels (stereo_kernels.cu) and the host build the CPU tests hold against the
-// numpy oracle (tests/host_emu_stereo.cpp); the kernels keep only layout here (staging, shuffles, the path walk).
+// numpy oracle (tests/host_emu.cpp); the kernels keep only layout here (staging, shuffles, the path walk).
 // Everything is integer arithmetic until the one fp32 division of the depth, so both builds give the same bits.
 #pragma once
 #include <stdint.h>

@@ -119,13 +119,20 @@ struct DepthPair {
   int64_t p0, n;   // the scan's points [p0, p0 + n)
   int32_t frame;
 };
-struct DepthScatterParams {
-  const float4* points;
+// The frame store as both depth kernels read it: frame f's camera and clamped pixel range (pnr_depth_frame)
+struct DepthStore {
   const int32_t* frame_cam;
   const int64_t* pix_offset;
   int64_t P;
   pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
   int32_t num_cameras;
+  __device__ __forceinline__ const pnr_ray_camera& frame(int f, int64_t* lo, int64_t* hi) const {
+    return cams[pnr_depth_frame(frame_cam, pix_offset, num_cameras, P, f, lo, hi)];
+  }
+};
+struct DepthScatterParams {
+  const float4* points;
+  DepthStore store;
   float min_depth, max_depth;
   uint32_t* zbuf;
   DepthPair pairs[kDepthPairsPerLaunch];
@@ -134,8 +141,7 @@ struct DepthScatterParams {
 __global__ void __launch_bounds__(kDepthThreads) depth_scatter_kernel(const __grid_constant__ DepthScatterParams p) {
   const DepthPair& q = p.pairs[blockIdx.y];
   int64_t lo, hi;
-  const int cam = pnr_depth_frame(p.frame_cam, p.pix_offset, p.num_cameras, p.P, q.frame, &lo, &hi);
-  const pnr_ray_camera& c = p.cams[cam];
+  const pnr_ray_camera& c = p.store.frame(q.frame, &lo, &hi);
   const float4* pts = p.points + q.p0;
   for (int64_t i = (int64_t)blockIdx.x * kDepthThreads + threadIdx.x; i < q.n;
        i += (int64_t)gridDim.x * kDepthThreads) {
@@ -150,11 +156,7 @@ __global__ void __launch_bounds__(kDepthThreads) depth_scatter_kernel(const __gr
 // kFill: zbuf = +Inf over the frames' pixels; otherwise depth = pnr_depth_pixel of the z-buffer (r = 0: finalise, in
 // place when zbuf aliases depth; r > 0: the filter, from the workspace's z-buffer)
 struct DepthFrameParams {
-  const int32_t* frame_cam;
-  const int64_t* pix_offset;
-  int64_t P;
-  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
-  int32_t num_cameras;
+  DepthStore store;
   uint32_t* zbuf;
   float* depth;
   int32_t radius;
@@ -164,8 +166,7 @@ struct DepthFrameParams {
 template <bool kFill>
 __global__ void __launch_bounds__(kDepthThreads) depth_frames_kernel(const __grid_constant__ DepthFrameParams p) {
   int64_t lo, hi;
-  const int cam = pnr_depth_frame(p.frame_cam, p.pix_offset, p.num_cameras, p.P, p.frames[blockIdx.y], &lo, &hi);
-  const pnr_ray_camera& c = p.cams[cam];
+  const pnr_ray_camera& c = p.store.frame(p.frames[blockIdx.y], &lo, &hi);
   const int64_t n = hi - lo;
   for (int64_t q = (int64_t)blockIdx.x * kDepthThreads + threadIdx.x; q < n; q += (int64_t)gridDim.x * kDepthThreads) {
     if (kFill)
@@ -649,17 +650,8 @@ extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream
                 32 * kCompMaxPerLane);
   PNR_CHECK_ARG(a.Ni >= 0 && a.Ni <= 32 * kCompMaxPerLane - a.N, "pnr_sample_ray_batch: Ni=%d outside [0,%d] (N + Ni <= %d)",
                 a.Ni, 32 * kCompMaxPerLane - a.N, 32 * kCompMaxPerLane);
-  PNR_CHECK_ARG(a.num_cameras >= 1 && a.num_cameras <= PNR_RAY_BATCH_MAX_CAMERAS,
-                "pnr_sample_ray_batch: num_cameras=%d outside [1,%d]", a.num_cameras, PNR_RAY_BATCH_MAX_CAMERAS);
-  for (int k = 0; k < a.num_cameras; ++k) {
-    const pnr_ray_camera& c = a.cams[k];
-    if (c.model == 1)
-      return set_error(PNR_ERR_ARG, "pnr_sample_ray_batch: camera %d is equirect (model 1): its rays are device-only "
-                       "(sincosf), so batches take pinhole (0) and fisheye (2) cameras", k);
-    PNR_CHECK_ARG(c.model == 0 || c.model == 2, "pnr_sample_ray_batch: camera %d model %d (0 pinhole, 2 fisheye)", k,
-                  c.model);
-    PNR_CHECK_ARG(c.H >= 1 && c.W >= 1, "pnr_sample_ray_batch: camera %d size H=%d W=%d < 1", k, c.H, c.W);
-  }
+  int rc = check_cameras("pnr_sample_ray_batch", a.cams, a.num_cameras, 31);
+  if (rc != PNR_OK) return rc;
   PNR_CHECK_ARG(a.c2w && a.frame_cam && a.pix_offset && a.rgb8,
                 "pnr_sample_ray_batch: null frame-set pointer (c2w, frame_cam, pix_offset and rgb8 are required)");
   PNR_CHECK_ARG(a.rays && a.rgb && a.u, "pnr_sample_ray_batch: null output pointer (rays, rgb and u are required)");
@@ -667,7 +659,7 @@ extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream
   const int64_t n = a.r1 - a.r0;
   if (n == 0) return PNR_OK;
   int dev = 0;
-  int rc = current_device("pnr_sample_ray_batch", &dev);
+  rc = current_device("pnr_sample_ray_batch", &dev);
   if (rc != PNR_OK) return rc;
   const int64_t want = (n + kRayBatchThreads - 1) / kRayBatchThreads, cap = (int64_t)num_sms(dev) * 8;
   const int64_t blocks = want < cap ? want : cap;
@@ -694,18 +686,8 @@ extern "C" int pnr_project_depth(const pnr_project_depth_args* args, void* strea
   PNR_CHECK_ARG(a.Q >= 0, "pnr_project_depth: Q=%d < 0", a.Q);
   PNR_CHECK_ARG(a.S >= 0, "pnr_project_depth: S=%d < 0", a.S);
   PNR_CHECK_ARG(a.Npts >= 0, "pnr_project_depth: Npts=%lld < 0", (long long)a.Npts);
-  PNR_CHECK_ARG(a.num_cameras >= 1 && a.num_cameras <= PNR_RAY_BATCH_MAX_CAMERAS,
-                "pnr_project_depth: num_cameras=%d outside [1,%d]", a.num_cameras, PNR_RAY_BATCH_MAX_CAMERAS);
-  for (int k = 0; k < a.num_cameras; ++k) {
-    const pnr_ray_camera& c = a.cams[k];
-    if (c.model == 1)
-      return set_error(PNR_ERR_ARG, "pnr_project_depth: camera %d is equirect (model 1); depth targets take pinhole "
-                       "(0) and fisheye (2) cameras, as training batches do", k);
-    PNR_CHECK_ARG(c.model == 0 || c.model == 2, "pnr_project_depth: camera %d model %d (0 pinhole, 2 fisheye)", k,
-                  c.model);
-    PNR_CHECK_ARG(c.H >= 1 && c.W >= 1 && c.H < (1 << 24) && c.W < (1 << 24),
-                  "pnr_project_depth: camera %d size H=%d W=%d outside [1, 2^24)", k, c.H, c.W);
-  }
+  int rc = check_cameras("pnr_project_depth", a.cams, a.num_cameras, 24);
+  if (rc != PNR_OK) return rc;
   PNR_CHECK_ARG(isfinite(a.min_depth) && a.min_depth > 0.f, "pnr_project_depth: min_depth=%g is not finite and > 0",
                 (double)a.min_depth);
   PNR_CHECK_ARG(isfinite(a.max_depth) && a.max_depth > a.min_depth,
@@ -742,7 +724,7 @@ extern "C" int pnr_project_depth(const pnr_project_depth_args* args, void* strea
                 a.workspace_bytes, a.workspace, need);
   if (a.Q == 0) return PNR_OK;
   int dev = 0;
-  int rc = current_device("pnr_project_depth", &dev);
+  rc = current_device("pnr_project_depth", &dev);
   if (rc != PNR_OK) return rc;
   const int sms = num_sms(dev);
   const cudaStream_t st = (cudaStream_t)stream;
@@ -753,14 +735,16 @@ extern "C" int pnr_project_depth(const pnr_project_depth_args* args, void* strea
   int64_t max_hw = 1;
   for (int k = 0; k < a.num_cameras; ++k) max_hw = std::max(max_hw, (int64_t)a.cams[k].H * a.cams[k].W);
   uint32_t* zbuf = filter ? (uint32_t*)a.workspace : (uint32_t*)a.depth;
+  DepthStore store;
+  store.frame_cam = a.frame_cam; store.pix_offset = a.pix_offset; store.P = a.P;
+  for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k) store.cams[k] = a.cams[k < a.num_cameras ? k : 0];
+  store.num_cameras = a.num_cameras;
 
   // the frame passes: kFill over zbuf, then (after the scatter) the final depth
   auto frame_pass = [&](bool fill) -> int {
     std::unique_ptr<DepthFrameParams> hold(new DepthFrameParams());   // 8 KB, copied by each launch
     DepthFrameParams& fp = *hold;
-    fp.frame_cam = a.frame_cam; fp.pix_offset = a.pix_offset; fp.P = a.P;
-    for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k) fp.cams[k] = a.cams[k < a.num_cameras ? k : 0];
-    fp.num_cameras = a.num_cameras; fp.zbuf = zbuf; fp.depth = a.depth;
+    fp.store = store; fp.zbuf = zbuf; fp.depth = a.depth;
     fp.radius = a.occlusion_radius; fp.margin = a.occlusion_margin;
     for (size_t f0 = 0; f0 < frames.size(); f0 += kDepthFramesPerLaunch) {
       const int nf = (int)std::min<size_t>(kDepthFramesPerLaunch, frames.size() - f0);
@@ -779,9 +763,8 @@ extern "C" int pnr_project_depth(const pnr_project_depth_args* args, void* strea
 
   std::unique_ptr<DepthScatterParams> hold(new DepthScatterParams());   // 18 KB, copied by each launch
   DepthScatterParams& sp = *hold;
-  sp.points = (const float4*)a.points; sp.frame_cam = a.frame_cam; sp.pix_offset = a.pix_offset; sp.P = a.P;
-  for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k) sp.cams[k] = a.cams[k < a.num_cameras ? k : 0];
-  sp.num_cameras = a.num_cameras; sp.min_depth = a.min_depth; sp.max_depth = a.max_depth; sp.zbuf = zbuf;
+  sp.points = (const float4*)a.points; sp.store = store;
+  sp.min_depth = a.min_depth; sp.max_depth = a.max_depth; sp.zbuf = zbuf;
   int np = 0;
   int64_t max_n = 0;
   auto flush = [&]() -> int {

@@ -91,21 +91,20 @@ def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00",
     pair by semi-global matching (refused together with depth_dir or lidar)."""
     if camera not in CAMERAS:
         raise ValueError(f"load_frames: camera {camera!r}; one of {CAMERAS}")
-    want_lidar = lidar is not False and lidar is not None   # {} is on, with the defaults
-    if want_lidar:
-        from .lidar import LIDAR_OPTIONS
-        if depth_dir is not None:
-            raise ValueError("load_frames: lidar and depth_dir both give the depth table; pass one of them")
-        if lidar is not True and (not isinstance(lidar, dict) or set(lidar) - set(LIDAR_OPTIONS)):
-            raise ValueError(f"load_frames: lidar={lidar!r}; False, True or a dict with keys from {LIDAR_OPTIONS}")
-    want_stereo = stereo is not False and stereo is not None   # {} is on, with the defaults
-    if want_stereo:
-        from .stereo import STEREO_OPTIONS
-        if depth_dir is not None or want_lidar:
-            raise ValueError("load_frames: stereo and " + ("lidar" if want_lidar else "depth_dir") + " both give the "
-                             "depth table; pass one of them")
-        if stereo is not True and (not isinstance(stereo, dict) or set(stereo) - set(STEREO_OPTIONS)):
-            raise ValueError(f"load_frames: stereo={stereo!r}; False, True or a dict with keys from {STEREO_OPTIONS}")
+    from .lidar import LIDAR_OPTIONS, lidar_depth
+    from .stereo import STEREO_OPTIONS, stereo_depth
+    # the sources of the depth table, at most one per call: (name, value, option keys, fill).  depth_dir's PNGs are read
+    # with the images; lidar / stereo are on unless False or None ({} is on, with the defaults).
+    source = None
+    for name, value, keys, fill in (("depth_dir", depth_dir, None, None), ("lidar", lidar, LIDAR_OPTIONS, lidar_depth),
+                                    ("stereo", stereo, STEREO_OPTIONS, stereo_depth)):
+        if value is None or (keys is not None and value is False):
+            continue
+        if source is not None:
+            raise ValueError(f"load_frames: {name} and {source[0]} both give the depth table; pass one of them")
+        if keys is not None and value is not True and (not isinstance(value, dict) or set(value) - set(keys)):
+            raise ValueError(f"load_frames: {name}={value!r}; False, True or a dict with keys from {keys}")
+        source = (name, value, fill)
     root = Path(root)
     frames = [int(f) for f in frames]
     if not frames:
@@ -139,13 +138,30 @@ def load_frames(root, seq: str, frames: Iterable[int], camera: str = "image_00",
     fs = FrameSet.from_images([cam], [0] * len(frames), np.stack(c2w).astype(np.float32), rgb,
                               lab if pseudo_dir is not None else None, dep if depth_dir is not None else None,
                               [(camera, f) for f in frames], device)
-    if want_lidar:
-        from .lidar import lidar_depth
-        lidar_depth(fs, root, seq, **({} if lidar is True else lidar))
-    if want_stereo:
-        from .stereo import stereo_depth
-        stereo_depth(fs, root, seq, **({} if stereo is True else stereo))
+    if source is not None and source[2] is not None:
+        source[2](fs, root, seq, **({} if source[1] is True else source[1]))
     return fs
+
+
+def check_depth_range(what: str, min_depth, max_depth) -> None:
+    """The depth limits of a depth source (`what` names it): min_depth finite and > 0, max_depth finite and above it."""
+    if not (np.isfinite(min_depth) and min_depth > 0):
+        raise ValueError(f"{what}: min_depth={min_depth}; finite and > 0")
+    if not (np.isfinite(max_depth) and max_depth > min_depth):
+        raise ValueError(f"{what}: max_depth={max_depth}; finite and > min_depth={min_depth}")
+
+
+def check_names(frames: FrameSet, what: str) -> None:
+    """A depth source finds each frame of the set by its (camera, frame id) in frames.names."""
+    if len(frames.names) != frames.num_frames:
+        raise ValueError(f"{what}: the set names {len(frames.names)} of its {frames.num_frames} frames; each frame needs "
+                         "its (camera, frame id)")
+
+
+def ensure_depth(frames: FrameSet) -> None:
+    """Allocate frames.depth (zero: no depth) when the set has none."""
+    if frames.depth is None:
+        frames.depth = torch.zeros(frames.num_pixels, dtype=torch.float32, device=frames.rgb8.device)
 
 
 __all__ = ["CAMERAS", "camera_of", "camera_poses", "load_frames"]

@@ -25,9 +25,9 @@ import numpy as np
 import torch
 
 from .... import _capi
-from ..ray_batch import CAMERA_MODEL, FrameSet
+from ..ray_batch import FrameSet, fill_frame_store
 from .calib import _floats, load_cam_to_pose, load_poses
-from .frames import CAMERAS, camera_poses
+from .frames import CAMERAS, camera_poses, check_depth_range, check_names, ensure_depth
 
 DEFAULT_MIN_DEPTH = 0.1          # metres
 DEFAULT_MAX_DEPTH = 80.0         # metres: the Velodyne HDL-64E's usable range
@@ -86,16 +86,7 @@ def project_depth(frames: FrameSet, points: torch.Tensor, scan_offset, pair_fram
     a.points, a.Npts = _capi.ptr(points, torch.float32, "points"), int(points.shape[0])
     a.scan_offset, a.S = so.ctypes.data, so.size - 1
     a.pair_frame, a.pair_scan, a.pair_M, a.Q = pf.ctypes.data, ps.ctypes.data, pm.ctypes.data, pf.size
-    a.frame_cam = _capi.ptr(frames.frame_cam, torch.int32, "frame_cam")
-    a.pix_offset = _capi.ptr(frames.pix_offset, torch.int64, "pix_offset")
-    a.F, a.P = frames.num_frames, frames.num_pixels
-    if len(frames.cameras) > _capi.RAY_BATCH_MAX_CAMERAS:
-        raise ValueError(f"project_depth: {len(frames.cameras)} cameras > {_capi.RAY_BATCH_MAX_CAMERAS}")
-    for k, cam in enumerate(frames.cameras):
-        a.cams[k].model, a.cams[k].H, a.cams[k].W = CAMERA_MODEL[cam.model], cam.H, cam.W
-        for i, x in enumerate(cam.intr):
-            a.cams[k].intr[i] = x
-    a.num_cameras = len(frames.cameras)
+    fill_frame_store(a, frames, "project_depth")
     a.min_depth, a.max_depth = float(min_depth), float(max_depth)
     a.occlusion_radius, a.occlusion_margin = int(occlusion_radius), float(occlusion_margin)
     a.depth = _capi.ptr(frames.depth, torch.float32, "depth")
@@ -110,10 +101,7 @@ def project_depth(frames: FrameSet, points: torch.Tensor, scan_offset, pair_fram
 def _check_options(lidar_window, min_depth, max_depth, occlusion_radius, occlusion_margin, chunk_frames):
     if int(lidar_window) != lidar_window or lidar_window < 0:
         raise ValueError(f"lidar_depth: lidar_window={lidar_window}; an integer >= 0")
-    if not (np.isfinite(min_depth) and min_depth > 0):
-        raise ValueError(f"lidar_depth: min_depth={min_depth}; finite and > 0")
-    if not (np.isfinite(max_depth) and max_depth > min_depth):
-        raise ValueError(f"lidar_depth: max_depth={max_depth}; finite and > min_depth={min_depth}")
+    check_depth_range("lidar_depth", min_depth, max_depth)
     if int(occlusion_radius) != occlusion_radius or not 0 <= occlusion_radius <= 8:
         raise ValueError(f"lidar_depth: occlusion_radius={occlusion_radius}; an integer in [0, 8]")
     if occlusion_radius > 0 and not 0 < occlusion_margin < 1:
@@ -174,13 +162,10 @@ def lidar_depth(frames: FrameSet, root, seq: str, lidar_window: int = 0, min_dep
     `load_frames` and `concat_frame_sets` leave them.  chunk_frames frames go to the device per call, with the scans
     their windows need, so the device holds at most chunk_frames + 2 w scans at a time.  Returns `frames`."""
     _check_options(lidar_window, min_depth, max_depth, occlusion_radius, occlusion_margin, chunk_frames)
-    F = frames.num_frames
-    if len(frames.names) != F:
-        raise ValueError(f"lidar_depth: the set names {len(frames.names)} of its {F} frames; each frame needs its "
-                         "(camera, frame id)")
+    check_names(frames, "lidar_depth")
     pairs = frame_scans(frames.names, root, seq, lidar_window)
-    if frames.depth is None:
-        frames.depth = torch.zeros(frames.num_pixels, dtype=torch.float32, device=frames.rgb8.device)
+    ensure_depth(frames)
+    F = frames.num_frames
     for f0 in range(0, F, int(chunk_frames)):
         chunk = range(f0, min(F, f0 + int(chunk_frames)))
         scans = sorted({s for f in chunk for s, _ in pairs[f]})

@@ -23,6 +23,7 @@ import torch
 from .... import _capi
 from ..ray_batch import FrameSet
 from .calib import load_perspective
+from .frames import check_depth_range, check_names, ensure_depth
 
 DEFAULT_DISPARITIES = 128
 DEFAULT_P1 = 10
@@ -117,16 +118,10 @@ def stereo_depth(frames: FrameSet, root, seq: str, num_disparities: int = DEFAUL
     `frames`."""
     import cv2
     _check_sgm("stereo_depth", num_disparities, P1, P2, uniqueness)
-    if not (np.isfinite(min_depth) and min_depth > 0):
-        raise ValueError(f"stereo_depth: min_depth={min_depth}; finite and > 0")
-    if not (np.isfinite(max_depth) and max_depth > min_depth):
-        raise ValueError(f"stereo_depth: max_depth={max_depth}; finite and > min_depth={min_depth}")
+    check_depth_range("stereo_depth", min_depth, max_depth)
     if not _is_int(chunk_frames) or chunk_frames < 1:
         raise ValueError(f"stereo_depth: chunk_frames={chunk_frames}; an integer >= 1")
-    F = frames.num_frames
-    if len(frames.names) != F:
-        raise ValueError(f"stereo_depth: the set names {len(frames.names)} of its {F} frames; each frame needs its "
-                         "(camera, frame id)")
+    check_names(frames, "stereo_depth")
     left = [(f, int(fid)) for f, (cam, fid) in enumerate(frames.names) if cam == "image_00"]
     if not left:
         raise ValueError("stereo_depth: the set has no image_00 frames; stereo depth comes from the image_00 / "
@@ -150,8 +145,7 @@ def stereo_depth(frames: FrameSet, root, seq: str, num_disparities: int = DEFAUL
     for (_, fid), p in zip(left, paths):   # all present before anything is written
         if not p.is_file():
             raise FileNotFoundError(f"{p}: missing right image (image_01) of frame {fid}")
-    if frames.depth is None:
-        frames.depth = torch.zeros(frames.num_pixels, dtype=torch.float32, device=dev)
+    ensure_depth(frames)
     for c0 in range(0, len(left), int(chunk_frames)):
         chunk = range(c0, min(len(left), c0 + int(chunk_frames)))
         rgb = []

@@ -137,6 +137,21 @@ def concat_frame_sets(*sets: FrameSet) -> FrameSet:
                     table("depth", 0.0, torch.float32), [n for s in sets for n in s.names])
 
 
+def fill_frame_store(a, frames: FrameSet, what: str) -> None:
+    """Write the frame store of `frames` (frame_cam, pix_offset, F, P) and its camera table (cams, num_cameras) into
+    the C arguments `a` of `what` (pnr_ray_batch_args or pnr_project_depth_args)."""
+    a.frame_cam = _capi.ptr(frames.frame_cam, torch.int32, "frame_cam")
+    a.pix_offset = _capi.ptr(frames.pix_offset, torch.int64, "pix_offset")
+    a.F, a.P = frames.num_frames, frames.num_pixels
+    if len(frames.cameras) > _capi.RAY_BATCH_MAX_CAMERAS:
+        raise ValueError(f"{what}: {len(frames.cameras)} cameras > {_capi.RAY_BATCH_MAX_CAMERAS}")
+    for k, cam in enumerate(frames.cameras):
+        a.cams[k].model, a.cams[k].H, a.cams[k].W = CAMERA_MODEL[cam.model], cam.H, cam.W
+        for i, x in enumerate(cam.intr):
+            a.cams[k].intr[i] = x
+    a.num_cameras = len(frames.cameras)
+
+
 def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N: int, Ni: int = 0,
                      want_pixel: bool = False, want_frame: bool = False) -> Dict[str, torch.Tensor]:
     """Rays r0 .. r1-1 of the batch (seed, step): one pnr_sample_ray_batch launch on the frames' device.  Returns
@@ -160,19 +175,10 @@ def sample_ray_batch(frames: FrameSet, seed: int, step: int, r0: int, r1: int, N
         out["frame"] = e(max(n, 0), dtype=torch.int32)
     a = _capi.PnrRayBatchArgs()
     a.c2w = _capi.ptr(frames.c2w, torch.float32, "c2w")
-    a.frame_cam = _capi.ptr(frames.frame_cam, torch.int32, "frame_cam")
-    a.pix_offset = _capi.ptr(frames.pix_offset, torch.int64, "pix_offset")
-    a.F, a.P = frames.num_frames, frames.num_pixels
+    fill_frame_store(a, frames, "sample_ray_batch")
     a.rgb8 = _capi.ptr(frames.rgb8, torch.uint8, "rgb8")
     a.label = _capi.ptr(frames.label, torch.int16, "label")
     a.depth = _capi.ptr(frames.depth, torch.float32, "depth")
-    if len(frames.cameras) > _capi.RAY_BATCH_MAX_CAMERAS:
-        raise ValueError(f"sample_ray_batch: {len(frames.cameras)} cameras > {_capi.RAY_BATCH_MAX_CAMERAS}")
-    for k, cam in enumerate(frames.cameras):
-        a.cams[k].model, a.cams[k].H, a.cams[k].W = CAMERA_MODEL[cam.model], cam.H, cam.W
-        for i, x in enumerate(cam.intr):
-            a.cams[k].intr[i] = x
-    a.num_cameras = len(frames.cameras)
     a.seed, a.step, a.r0, a.r1, a.N, a.Ni = int(seed), int(step), int(r0), int(r1), int(N), int(Ni)
     a.rays, a.rgb, a.u = _capi.ptr(out["rays"]), _capi.ptr(out["rgb"]), _capi.ptr(out["u"])
     a.u_fine = _capi.ptr(out.get("u_fine"))

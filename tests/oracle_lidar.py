@@ -1,30 +1,14 @@
 """numpy float32 oracle of pnr_project_depth (include/pnr.h, DESIGN 3.4): the same operation order as
 pnr_project_point / pnr_depth_pixel of ray_math.h, every operation a rounded float32 one (numpy does not contract to
-FMA; its sqrt and division are correctly rounded), and helpers to call the host build (tests/host_emu_lidar.cpp)."""
+FMA; its sqrt and division are correctly rounded), and helpers to call the host build (tests/host_emu.cpp)."""
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 
 from panopticnerf_b200 import _capi
 
-ROOT = Path(__file__).resolve().parent.parent
 f32 = np.float32
-
-
-def host_build():
-    """Compile tests/host_emu_lidar.cpp (as tests/host_emu.py compiles host_emu.cpp) and load it."""
-    out = ROOT / "build" / "host_emu_lidar.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu_lidar.cpp")])
-    lib = C.CDLL(str(out))
-    lib.emu_project_point.argtypes = [C.POINTER(_capi.PnrRayCamera), C.c_void_p, C.c_float, C.c_float, C.c_float,
-                                      C.c_float, C.c_float, C.POINTER(C.c_int64), C.POINTER(C.c_float)]
-    lib.emu_project_point.restype = C.c_int
-    lib.emu_project_depth.argtypes = [C.POINTER(_capi.PnrProjectDepthArgs)]
-    return lib
 
 
 def camera_struct(cam):

@@ -1,15 +1,12 @@
 """numpy oracle of pnr_stereo_depth (include/pnr.h, DESIGN 3.4): a restatement of the semi-global matching rule in
 integers - grey, census, cost, the eight path recursions (vectorised over the axis across the path and over d), the
 winner, uniqueness, left-right check and subpixel with C's division written out - and the one float32 division of the
-depth.  Also the host build of stereo_math.h (tests/host_emu_stereo.cpp), scenes with a known disparity, and a
+depth.  Also helpers to call the host build of stereo_math.h (tests/host_emu.cpp), scenes with a known disparity, and a
 sequence in the KITTI-360 layout with the stereo pair."""
-import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
 f32 = np.float32
 BIG = 1 << 20                      # an absent d +- 1 term
 DIRECTIONS = ((1, 0), (-1, 0), (0, 1), (0, -1), (1, 1), (-1, -1), (1, -1), (-1, 1))
@@ -142,20 +139,6 @@ def sgm(left, right, D=128, P1=10, P2=120, U=10, want_S=False):
 
 
 # ---------------------------------------------------------------------------------------------------- host build
-def host_build():
-    """Compile tests/host_emu_stereo.cpp (as tests/host_emu.py compiles host_emu.cpp) and load it."""
-    out = ROOT / "build" / "host_emu_stereo.so"
-    out.parent.mkdir(exist_ok=True)
-    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
-                           str(ROOT / "tests" / "host_emu_stereo.cpp")])
-    lib = C.CDLL(str(out))
-    lib.emu_stereo.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 6 + [C.c_float] * 3 + [C.c_void_p] * 3
-    lib.emu_stereo.restype = None
-    lib.emu_select.argtypes = [C.c_void_p] + [C.c_int] * 4 + [C.c_void_p]
-    lib.emu_select.restype = None
-    return lib
-
-
 def host_select(lib, S, U):
     """The host build's selection over S [H, W, D] -> d16 [H, W] i16."""
     S = np.ascontiguousarray(S, np.uint16)

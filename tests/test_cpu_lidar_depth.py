@@ -22,41 +22,36 @@ f32 = np.float32
 TINY_FISHEYE = (2, 6, 7, (3.0, 2.5, 3.1, 2.4, 1.2, 0.05, 0.02))
 
 
-@pytest.fixture(scope="module")
-def lemu():
-    return O.host_build()
-
-
 def _same(a, b):
     return np.asarray(a).tobytes() == np.asarray(b).tobytes()
 
 
-def _check_points(lemu, cam, M, p, mind, maxd):
+def _check_points(emu, cam, M, p, mind, maxd):
     want = O.project_points(cam, M, p, mind, maxd)
-    got = O.host_point(lemu, cam, M, p, mind, maxd)
+    got = O.host_point(emu, cam, M, p, mind, maxd)
     for g, w, k in zip(got, want, ("ok", "pix", "t")):
         assert _same(g, w), k
     return got
 
 
 @pytest.mark.parametrize("cam", [O.PINHOLE, O.FISHEYE, TINY_FISHEYE], ids=["pinhole", "fisheye", "tiny_fisheye"])
-def test_point_equals_the_oracle_on_random_points(cam, lemu):
+def test_point_equals_the_oracle_on_random_points(cam, emu):
     rng = np.random.default_rng(cam[1])
     for trial in range(4):
         M = np.concatenate([O.rotation(rng.uniform(-0.3, 0.3, 3)), rng.uniform(-2, 2, (3, 1))], 1)
         p = np.stack([rng.uniform(-40, 40, 3000), rng.uniform(-10, 10, 3000), rng.uniform(-20, 80, 3000)], 1)
-        ok, _, _ = _check_points(lemu, cam, M, p, 0.1, 80.0)
+        ok, _, _ = _check_points(emu, cam, M, p, 0.1, 80.0)
         assert 0 < ok.sum() < len(p)
 
 
-def test_point_at_the_pixel_half_boundaries(lemu):
+def test_point_at_the_pixel_half_boundaries(emu):
     # fx = 2, cx = 0.5, z = 1: uf = (2 x) / 1 + 0.5 is exact, so x = k / 2 puts the point on uf = k + 0.5
     cam = (0, 4, 9, (2.0, 2.0, 0.5, 0.5))
     M = np.concatenate([np.eye(3), np.zeros((3, 1))], 1)
     k = np.arange(-1, 9, dtype=f32)
     xs = np.concatenate([k / 2, np.nextafter(k / 2, f32(-np.inf)), np.nextafter(k / 2, f32(np.inf))])
     p = np.stack([xs, np.full_like(xs, 0.5), np.ones_like(xs)], 1)
-    ok, pix, _ = _check_points(lemu, cam, M, p, 0.5, 2.0)
+    ok, pix, _ = _check_points(emu, cam, M, p, 0.5, 2.0)
     n = len(k)
     # exactly on k + 0.5: fp32(k + 0.5 + 0.5) = k + 1 -> pixel u = k + 1 (kept while < W = 9)
     on = (k + 1 >= 0) & (k + 1 < 9)
@@ -66,19 +61,19 @@ def test_point_at_the_pixel_half_boundaries(lemu):
     assert ok[n:].any()
 
 
-def test_point_at_the_depth_limits_and_behind_the_camera(lemu):
+def test_point_at_the_depth_limits_and_behind_the_camera(emu):
     cam = (0, 8, 8, (4.0, 4.0, 3.5, 3.5))
     M = np.concatenate([np.eye(3), np.zeros((3, 1))], 1)
     mind, maxd = f32(0.25), f32(50.0)
     zs = [mind, np.nextafter(mind, f32(1)), np.nextafter(mind, f32(0)), maxd, np.nextafter(maxd, f32(0)),
           np.nextafter(maxd, f32(100)), f32(0), f32(-1), f32(-0.0), f32(10)]
     p = np.stack([np.zeros(len(zs), f32), np.zeros(len(zs), f32), np.array(zs, f32)], 1)
-    ok, _, t = _check_points(lemu, cam, M, p, mind, maxd)
+    ok, _, t = _check_points(emu, cam, M, p, mind, maxd)
     assert ok.tolist() == [False, True, False, True, True, False, False, False, False, True]
     assert t[1] == zs[1] and t[3] == maxd
 
 
-def test_point_at_the_fisheye_mirror_limit(lemu):
+def test_point_at_the_fisheye_mirror_limit(emu):
     # p = (4, 0, -3): n = 5 exactly, x_s.z = fp32(-3 / 5); xi = -x_s.z gives x_s.z + xi = 0 (refused), one ulp more
     # projects
     zs = f32(-3) / f32(5)
@@ -86,20 +81,20 @@ def test_point_at_the_fisheye_mirror_limit(lemu):
     p = np.array([[4, 0, -3], [40, 0, -30]], f32)
     for xi, want in ((-zs, False), (np.nextafter(-zs, f32(1)), True), (np.nextafter(-zs, f32(0)), False)):
         cam = (2, 4000, 4000, (1e-6, 1e-6, 2000.0, 2000.0, float(xi), 0.0, 0.0))
-        ok, _, t = _check_points(lemu, cam, M, p, 0.1, 80.0)
+        ok, _, t = _check_points(emu, cam, M, p, 0.1, 80.0)
         assert ok.tolist() == [want, want]
         if want:
             assert t[0] == 5.0 and t[1] == 50.0
 
 
 @pytest.mark.parametrize("cam", [O.PINHOLE, O.FISHEYE], ids=["pinhole", "fisheye"])
-def test_point_with_nan_and_inf_coordinates(cam, lemu):
+def test_point_with_nan_and_inf_coordinates(cam, emu):
     rng = np.random.default_rng(3)
     M = np.concatenate([O.rotation(rng.uniform(-0.2, 0.2, 3)), rng.uniform(-1, 1, (3, 1))], 1)
     bad = [np.nan, np.inf, -np.inf]
     p = np.array([[b if i == j else 1.0 for j in range(3)] for i in range(3) for b in bad] +
                  [[1.0, 1.0, 10.0]], f32)
-    ok, _, _ = _check_points(lemu, cam, M, p, 0.1, 80.0)
+    ok, _, _ = _check_points(emu, cam, M, p, 0.1, 80.0)
     assert not ok[:-1].any() and ok[-1]
 
 
@@ -113,14 +108,14 @@ def _rays(emu, cam, c2w):
     return rays
 
 
-def test_round_trip_pinhole_is_exact(emu, lemu):
+def test_round_trip_pinhole_is_exact(emu):
     cam = (0, 47, 61, (52.5, 51.0, 30.2, 23.7))
     I = np.concatenate([np.eye(3), np.zeros((3, 1))], 1)
     rays = _rays(emu, cam, I)
     rng = np.random.default_rng(0)
     t = rng.uniform(0.2, 79.0, len(rays)).astype(f32)
     p = rays[:, 3:] * t[:, None]
-    ok, pix, tt = _check_points(lemu, cam, I, p, 0.1, 80.0)
+    ok, pix, tt = _check_points(emu, cam, I, p, 0.1, 80.0)
     assert ok.all()
     assert np.array_equal(pix, np.arange(len(rays)))
     assert np.array_equal(tt, t)
@@ -132,7 +127,7 @@ def test_round_trip_pinhole_is_exact(emu, lemu):
 FISHEYE_ROUND_TRIP_PX = 2e-3
 
 
-def test_round_trip_fisheye_within_the_newton_bound(emu, lemu):
+def test_round_trip_fisheye_within_the_newton_bound(emu):
     model, H, W, intr = O.FISHEYE
     sub = (2, 140, 140, (intr[0] / 10, intr[1] / 10, intr[2] / 10, intr[3] / 10) + tuple(intr[4:]))
     I = np.concatenate([np.eye(3), np.zeros((3, 1))], 1)
@@ -143,7 +138,7 @@ def test_round_trip_fisheye_within_the_newton_bound(emu, lemu):
     t = rng.uniform(0.5, 70.0, len(rays)).astype(f32)
     p = (rays[:, 3:] * t[:, None])[inner]
     ok, pix, tt, uf, vf = O.project_points(sub, I, p, 0.1, 80.0, want_uv=True)
-    _check_points(lemu, sub, I, p, 0.1, 80.0)
+    _check_points(emu, sub, I, p, 0.1, 80.0)
     assert ok.all()
     err = np.maximum(np.abs(uf - u[inner]), np.abs(vf - v[inner]))
     assert err.max() < FISHEYE_ROUND_TRIP_PX, err.max()
@@ -152,7 +147,7 @@ def test_round_trip_fisheye_within_the_newton_bound(emu, lemu):
 
 
 @pytest.mark.parametrize("radius", [0, 1, 8])
-def test_zbuffer_equals_the_oracle(radius, lemu):
+def test_zbuffer_equals_the_oracle(radius, emu):
     rng = np.random.default_rng(10 + radius)
     cams = [(0, 9, 13, (6.0, 6.0, 6.3, 4.1)), TINY_FISHEYE, (0, 1, 1, (1.0, 1.0, 0.0, 0.0))]
     fc, po, pts, so, pf, ps, pm = O.random_scene(rng, cams, F=7, S=4, n_lo=20, n_hi=4000, pairs_per_frame=3)
@@ -163,7 +158,7 @@ def test_zbuffer_equals_the_oracle(radius, lemu):
     depth_in = rng.uniform(1, 2, int(po[-1])).astype(f32)
     named = set(pf.tolist())
     want = O.zbuffer(cams, fc, po, pts, so, pf, ps, pm, 0.1, 60.0, radius, 0.05, depth_in=depth_in)
-    got = O.host_zbuffer(lemu, cams, fc, po, pts, so, pf, ps, pm, 0.1, 60.0, radius, 0.05, depth_in=depth_in)
+    got = O.host_zbuffer(emu, cams, fc, po, pts, so, pf, ps, pm, 0.1, 60.0, radius, 0.05, depth_in=depth_in)
     assert _same(got, want)
     plain = O.zbuffer(cams, fc, po, pts, so, pf, ps, pm, 0.1, 60.0, 0, 0.05)
     assert (plain > 0).sum() > 20 and (want > 0).any()
@@ -176,13 +171,13 @@ def test_zbuffer_equals_the_oracle(radius, lemu):
         assert np.all((want == 0) | (want == plain))       # and changed nothing else
 
 
-def test_zbuffer_with_all_points_on_one_pixel_and_a_wall(lemu):
+def test_zbuffer_with_all_points_on_one_pixel_and_a_wall(emu):
     cams = [(0, 5, 6, (4.0, 4.0, 2.5, 2.0))]
     I = np.concatenate([np.eye(3), np.zeros((3, 1))], 1).astype(f32).reshape(1, 12)
     rng = np.random.default_rng(5)
     z = rng.uniform(1, 50, 1000).astype(f32)
     pts = np.stack([np.zeros_like(z), np.zeros_like(z), z, z], 1)
-    got = O.host_zbuffer(lemu, cams, [0], [0, 30], pts, [0, 1000], [0], [0], I, 0.1, 80.0)
+    got = O.host_zbuffer(emu, cams, [0], [0, 30], pts, [0, 1000], [0], [0], I, 0.1, 80.0)
     want = np.zeros(30, f32)
     want[2 * 6 + 3] = z.min()      # uf = (4 * 0) / z + 2.5 -> u = floor(3.0) = 3; vf = 2 -> v = 2
     assert _same(got, want)
@@ -213,7 +208,7 @@ def test_load_cam_to_velo_and_its_refusal(tmp_path):
         L.load_cam_to_velo(tmp_path / "d.txt")
 
 
-def test_the_transform_chain_puts_a_world_point_on_its_pixel(tmp_path, lemu):
+def test_the_transform_chain_puts_a_world_point_on_its_pixel(tmp_path, emu):
     seq = O.write_sequence(tmp_path, [5, 6])
     # a world point 12 m in front of camera 0 at frame 5, on pixel (u, v) = (9, 17) (z = 12: x = (9 - 15.5) 12 / 20)
     u, v, z = 9, 17, 12.0
@@ -225,7 +220,7 @@ def test_the_transform_chain_puts_a_world_point_on_its_pixel(tmp_path, lemu):
     assert [s for s, _ in rows[0]] == [5, 6]            # scan 4 has no pose or file: skipped
     M = dict(rows[0])[6]
     cam = (0, 24, 32, (20.0, 20.0, 15.5, 11.5))
-    ok, pix, t = O.host_point(lemu, cam, M, pv[None, :3], 0.1, 80.0)
+    ok, pix, t = O.host_point(emu, cam, M, pv[None, :3], 0.1, 80.0)
     assert ok[0] and pix[0] == v * 32 + u and abs(t[0] - z) < 1e-4
     # a fisheye frame: its pose is poses.txt @ cam_to_pose["image_02"]
     rows = L.frame_scans([("image_02", 6)], tmp_path, seq["seq"])

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import oracle_stereo as O
+from host_emu import emu  # noqa: F401  (session fixture: the host build of ray_math.h and stereo_math.h)
 from panopticnerf_b200 import _capi
 from panopticnerf_b200.lib.datasets.kitti360 import load_frames
 from panopticnerf_b200.lib.datasets.kitti360 import stereo as ST
@@ -19,11 +20,6 @@ from panopticnerf_b200.lib.datasets.ray_batch import Camera, FrameSet
 
 ROOT = Path(__file__).resolve().parent.parent
 f32 = np.float32
-
-
-@pytest.fixture(scope="module")
-def semu():
-    return O.host_build()
 
 
 # ---------------------------------------------------------------------------------------------------- the oracle
@@ -50,7 +46,7 @@ def test_path_costs_stay_within_63_plus_P2(P1, P2):
     assert S.max() < 1 << 16
 
 
-def test_a_flat_image_matches_everything_at_zero(semu):
+def test_a_flat_image_matches_everything_at_zero(emu):
     img = np.full((12, 20, 3), 77, np.uint8)
     cen = O.census(O.grey(img))
     C_ = O.costs(cen, cen, 32)
@@ -60,7 +56,7 @@ def test_a_flat_image_matches_everything_at_zero(semu):
     assert not S[..., 0].any()
     assert not d16.any()
     assert not O.depth_of(d16, 1000.0, 0.1, 40.0).any()
-    hd, hdep = O.host_sgm(semu, img, img, 32, b16=1000.0)
+    hd, hdep = O.host_sgm(emu, img, img, 32, b16=1000.0)
     assert not hd.any() and not hdep.any()
 
 
@@ -68,17 +64,17 @@ def _row_volume(vec, W):
     return np.tile(np.asarray(vec, np.int64), (1, W, 1))
 
 
-def test_ties_pick_the_lowest_disparity(semu):
+def test_ties_pick_the_lowest_disparity(emu):
     # S(d) = 5 min(|d - 3|, |d - 4|): a tie between d = 3 and 4 everywhere; d* = 3 and d_R = 3 (also the lowest),
     # subpixel: lo = 5, hi = 0, den = 5, (5 16 + 5) / 10 = 8 -> d16 = 56 where x >= 3
     d = np.arange(32)
     S = _row_volume(5 * np.minimum(np.abs(d - 3), np.abs(d - 4)), 10)
     got = O.select(S, 0)
     assert got[0].tolist() == [-1, -1, -1] + [56] * 7
-    assert np.array_equal(O.host_select(semu, S, 0), got)
+    assert np.array_equal(O.host_select(emu, S, 0), got)
 
 
-def test_uniqueness_at_equality_and_one_unit_past(semu):
+def test_uniqueness_at_equality_and_one_unit_past(emu):
     # d* = 2 with S = 90; with U = 10 a far d with S(d) 90 < 90 100 refuses: S(d) = 100 is the equality (kept),
     # S(d) = 99 one unit past (refused)
     for far, want in ((100, 32), (99, -1)):
@@ -89,14 +85,14 @@ def test_uniqueness_at_equality_and_one_unit_past(semu):
         S = _row_volume(vec, 6)
         got = O.select(S, 10)
         assert got[0, 2:].tolist() == [want] * 4, (far, got)
-        assert np.array_equal(O.host_select(semu, S, 10), got)
+        assert np.array_equal(O.host_select(emu, S, 10), got)
     # d* +- 1 never counts against uniqueness
     vec = np.full(32, 500)
     vec[2], vec[3], vec[1] = 90, 90, 95
     assert O.select(_row_volume(vec, 6), 10)[0, 5] >= 0
 
 
-def test_subpixel_truncates_negative_numerators_toward_zero(semu):
+def test_subpixel_truncates_negative_numerators_toward_zero(emu):
     # S(d*-1) = 10, S(d*) = 4, S(d*+1) = 30: den = 32, numerator (10 - 30) 16 + 32 = -288, -288 / 64 = -4.5 -> -4
     # (floor division would give -5); d* = 5 -> d16 = 76
     vec = np.full(32, 900)
@@ -104,24 +100,24 @@ def test_subpixel_truncates_negative_numerators_toward_zero(semu):
     S = _row_volume(vec, 8)
     got = O.select(S, 10)
     assert got[0, 5:].tolist() == [76, 76, 76]
-    assert np.array_equal(O.host_select(semu, S, 10), got)
+    assert np.array_equal(O.host_select(emu, S, 10), got)
     # positive numerator: S(d*-1) = 30, S(d*+1) = 10: (20 16 + 32) / 64 = 5 (5.5 truncated)
     vec[4:7] = [30, 4, 10]
     assert O.select(_row_volume(vec, 8), 10)[0, 5] == 85
 
 
 # ---------------------------------------------------------------------------------------------------- scenes
-def test_random_dots_at_a_constant_disparity(semu):
+def test_random_dots_at_a_constant_disparity(emu):
     rng = np.random.default_rng(1)
     d0 = 9
     left, right = O.random_dots(rng, 40, 120, d0)
     d16 = O.sgm(left, right, 64)
-    assert np.array_equal(O.host_sgm(semu, left, right, 64)[0], d16)
+    assert np.array_equal(O.host_sgm(emu, left, right, 64)[0], d16)
     inner = d16[3:-3, d0 + 4:-4]                    # away from the clamped census border and the unmatched band
     assert (np.rint(inner / 16) == d0).mean() >= 0.99
 
 
-def test_a_fronto_parallel_plane_reads_its_depth(semu):
+def test_a_fronto_parallel_plane_reads_its_depth(emu):
     # fx b / Z = 6 exactly: the plane's texture cells are one pixel wide at Z, so each right pixel sees the left
     # pixel six to its right.  Strong smoothness (P1 = 200, P2 = 2048) keeps the parabola's two sides even, so the
     # subpixel rule lands within one sixteenth of 96.
@@ -129,7 +125,7 @@ def test_a_fronto_parallel_plane_reads_its_depth(semu):
     Z = fx * b / d0
     left, right = O.render_pair(H, W, fx, 59.5, 19.5, b, [(Z, None, 3)])
     b16 = float(f32(16 * fx * b))
-    d16, depth = O.host_sgm(semu, left, right, 64, 200, 2048, 10, b16, 0.1, 40.0)
+    d16, depth = O.host_sgm(emu, left, right, 64, 200, 2048, 10, b16, 0.1, 40.0)
     assert np.array_equal(d16, O.sgm(left, right, 64, 200, 2048, 10))
     inner = (slice(3, -3), slice(d0 + 4, -4))
     assert (d16[inner] >= 0).all()
@@ -138,14 +134,14 @@ def test_a_fronto_parallel_plane_reads_its_depth(semu):
     assert np.array_equal(depth, O.depth_of(d16, b16, 0.1, 40.0))
 
 
-def test_the_band_a_near_square_occludes_fails_the_left_right_check(semu):
+def test_the_band_a_near_square_occludes_fails_the_left_right_check(emu):
     # far plane at disparity 4, a square at disparity 12 over left columns [50, 80): the far plane's pixels of left
     # columns [42, 50) are hidden from the right camera by the square.  U = 0 turns uniqueness off, so what refuses
     # them is the left-right check.
     H, W, fx, b = 48, 128, 40.0, 0.6
     left, right = O.render_pair(H, W, fx, 63.5, 23.5, b, [(fx * b / 4, None, 1), (fx * b / 12, (50, 80, 10, 38), 2)])
     d16 = O.sgm(left, right, 32, 10, 120, 0)
-    assert np.array_equal(O.host_sgm(semu, left, right, 32, 10, 120, 0)[0], d16)
+    assert np.array_equal(O.host_sgm(emu, left, right, 32, 10, 120, 0)[0], d16)
     band = d16[14:34, 43:49]
     assert (band < 0).mean() >= 0.9
     assert (np.abs(d16[14:34, 54:76].astype(int) - 192) <= 8).mean() >= 0.95
@@ -161,14 +157,14 @@ CASES = [(H, W, D, *PENALTIES[k % 3], UNIQUENESS[(k // 3) % 3])
 
 
 @pytest.mark.parametrize("H,W,D,P1,P2,U", CASES)
-def test_host_build_equals_the_oracle(H, W, D, P1, P2, U, semu):
+def test_host_build_equals_the_oracle(H, W, D, P1, P2, U, emu):
     rng = np.random.default_rng(H * 1000 + W * 10 + D)
     left, right = O.random_dots(rng, H, W, min(5, W - 1))
     if H > 1:   # smooth parts too, where ties and flat costs occur
         left[: H // 3] //= 64
         right[: H // 3] //= 64
     b16 = float(f32(16 * 552.554 * 0.6))
-    d16, depth, S = O.host_sgm(semu, left, right, D, P1, P2, U, b16, 1.0, 40.0, want_S=True)
+    d16, depth, S = O.host_sgm(emu, left, right, D, P1, P2, U, b16, 1.0, 40.0, want_S=True)
     want, wS = O.sgm(left, right, D, P1, P2, U, want_S=True)
     assert np.array_equal(S.astype(np.int32), wS)
     assert np.array_equal(d16, want)

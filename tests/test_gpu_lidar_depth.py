@@ -9,6 +9,7 @@ import pytest
 import torch
 
 import oracle_lidar as O
+from host_emu import emu  # noqa: F401  (session fixture: the host build of ray_math.h and stereo_math.h)
 import panopticnerf_b200 as PN
 from panopticnerf_b200 import _capi, synthetic as S
 from panopticnerf_b200.lib.datasets.kitti360 import lidar as L
@@ -18,11 +19,6 @@ DEV = "cuda:0"
 f32 = np.float32
 SMALL_PINHOLE = (0, 48, 64, (40.0, 40.0, 31.7, 23.2))
 SMALL_FISHEYE = (2, 50, 50, (47.8, 47.7, 25.6, 25.2, 2.2134, 0.01647, 1.6035))
-
-
-@pytest.fixture(scope="module")
-def lemu():
-    return O.host_build()
 
 
 def prepare(cams, fc, po, pts, so, pf, ps, pm, mind, maxd, radius=0, margin=0.1, depth=None):
@@ -64,12 +60,12 @@ CASES = [(1, 1, (1, 1), 1, 0), (3, 2, (0, 5000), 2, 0), (40, 12, (100, 30000), 4
 
 
 @pytest.mark.parametrize("F,S_,npts,ppf,radius", CASES)
-def test_kernel_equals_the_host_build(F, S_, npts, ppf, radius, lemu):
+def test_kernel_equals_the_host_build(F, S_, npts, ppf, radius, emu):
     rng = np.random.default_rng(F * 7 + radius)
     cams = [SMALL_PINHOLE, SMALL_FISHEYE, (0, 1, 1, (1.0, 1.0, 0.0, 0.0))]
     scene = O.random_scene(rng, cams, F, S_, npts[0], npts[1], pairs_per_frame=ppf)
     got, _ = device_call(cams, *scene, 0.1, 60.0, radius, 0.07)
-    want = O.host_zbuffer(lemu, cams, *scene, 0.1, 60.0, radius, 0.07)
+    want = O.host_zbuffer(emu, cams, *scene, 0.1, 60.0, radius, 0.07)
     assert _bytes(got) == want.tobytes()
     if F >= 3:
         assert (want > 0).sum() > 10
@@ -77,7 +73,7 @@ def test_kernel_equals_the_host_build(F, S_, npts, ppf, radius, lemu):
         assert models == {0, 2} or F < 40
 
 
-def test_kernel_at_2_24_plus_3_points_on_one_pixel_and_spread(lemu):
+def test_kernel_at_2_24_plus_3_points_on_one_pixel_and_spread(emu):
     rng = np.random.default_rng(24)
     n = (1 << 24) + 3
     cams = [SMALL_PINHOLE]
@@ -91,12 +87,12 @@ def test_kernel_at_2_24_plus_3_points_on_one_pixel_and_spread(lemu):
     po = np.array([0, 48 * 64, 2 * 48 * 64], np.int64)
     args = (cams, [0, 0], po, pts, [0, n], [0, 1], [0, 0], np.concatenate([M, M * 1.0]))
     got, _ = device_call(*args, 0.1, 60.0)
-    want = O.host_zbuffer(lemu, *args, 0.1, 60.0)
+    want = O.host_zbuffer(emu, *args, 0.1, 60.0)
     assert _bytes(got) == want.tobytes()
     assert (want > 0).sum() > 1000
 
 
-def test_order_split_repeat_and_graph_replay_give_the_same_bytes(lemu):
+def test_order_split_repeat_and_graph_replay_give_the_same_bytes(emu):
     rng = np.random.default_rng(77)
     cams = [SMALL_PINHOLE, SMALL_FISHEYE]
     fc, po, pts, so, pf, ps, pm = O.random_scene(rng, cams, 50, 10, 2000, 40000, pairs_per_frame=5)
@@ -188,7 +184,7 @@ def test_a_wall_at_10_m_and_a_nearer_occluder(cam):
         assert (np.abs(d[inner] - 6.0) < 0.17).all()
 
 
-def test_two_to_the_31_plus_3_pixels(lemu):
+def test_two_to_the_31_plus_3_pixels(emu):
     big = (0, 8192, 16384, (8000.0, 8000.0, 8191.5, 4095.5))
     tiny = (0, 1, 3, (1.0, 1.0, 1.0, 0.0))
     P = 16 * (1 << 27) + 3
@@ -205,7 +201,7 @@ def test_two_to_the_31_plus_3_pixels(lemu):
     depth = torch.full((P,), -1.0, dtype=torch.float32, device=DEV)
     device_call(cams, fc, po, pts, [0, n], [15, 16], [0, 0], np.concatenate([I, I]), 0.1, 60.0, depth=depth)
     for f, cam in ((15, big), (16, tiny)):
-        want = O.host_zbuffer(lemu, [cam], [0], [0, cam[1] * cam[2]], pts, [0, n], [0], [0], I, 0.1, 60.0)
+        want = O.host_zbuffer(emu, [cam], [0], [0, cam[1] * cam[2]], pts, [0, n], [0], [0], I, 0.1, 60.0)
         assert _bytes(depth[int(po[f]):int(po[f + 1])]) == want.tobytes(), f
     assert bool((depth[-3:] > 0).all())
     assert bool((depth[int(po[14]):int(po[15])] == -1).all()) and bool((depth[:1 << 20] == -1).all())
