@@ -35,10 +35,12 @@ enum { PNR_OK = 0, PNR_ERR_ARG = -1, PNR_ERR_CUDA = -2, PNR_ERR_STATE = -3, PNR_
 
 /* MLP arithmetic mode: element format of the tensor-core operands (accumulation is always fp32).
  * The x3 modes split every operand x = hi + lo in that format and issue A_hi*B_hi + A_lo*B_hi + A_hi*B_lo. */
-enum { PNR_PREC_BF16X3 = 0, /* ~2^-17 per product, fp32 exponent range; ~1e-4 end to end (marginal)       */
-       PNR_PREC_BF16 = 1,   /* 1 pass, ~1e-2 end to end: fast mode, outside the tolerance                 */
-       PNR_PREC_FP16X3 = 2, /* ~2^-21 per product, needs |activation| < 65504; meets 1e-4 with margin     */
-       PNR_PREC_FP16 = 3    /* 1 pass, ~1e-3 end to end: fast mode, outside the tolerance                 */ };
+enum { PNR_PREC_BF16X3 = 0, /* operand split to 2^-17 |x|, fp32 exponent range; ~1e-4 end to end (marginal) */
+       PNR_PREC_BF16 = 1,   /* 1 pass, 2^-8 |x|; ~1e-2 end to end: fast mode, outside the tolerance         */
+       PNR_PREC_FP16X3 = 2, /* operand split to max(2^-23 |x|, 2^-25), needs |activation| < 65504; meets
+                               1e-4 with margin at O(1) operands.  The 2^-25 floor (fp16 subnormals) leaves an
+                               operand of 1e-4 only ~2^-12 relative, like one fp16 part                    */
+       PNR_PREC_FP16 = 3    /* 1 pass, max(2^-11 |x|, 2^-25); ~1e-3 end to end: fast mode, outside the tolerance */ };
 
 typedef struct pnr_ctx pnr_ctx;
 

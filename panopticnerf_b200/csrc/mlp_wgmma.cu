@@ -23,9 +23,11 @@
 // operand columns, K steps) and the epilogue table.
 //
 // Precision: operands are 16-bit (fp16 or bf16), accumulation fp32.  The "x3" modes compute every product
-// as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo with x = hi + lo split in the operand format: ~2^-21 relative
-// per product for fp16x3 (default; what the 1e-4 parity tolerance needs with margin), ~2^-17 for
-// bf16x3 (fp32 exponent range).  The 1-pass modes keep the first term only (fast, out of tolerance).
+// as A_hi*B_hi + A_lo*B_hi + A_hi*B_lo with x = hi + lo split in the operand format (split_x2): the split leaves
+// max(2^-23 |x|, 2^-25) of an operand in fp16x3 (default; what the 1e-4 parity tolerance needs with margin) and
+// 2^-17 |x| in bf16x3 (fp32 exponent range).  The fp16 floor is the subnormal spacing: an operand of 1e-4 (an early
+// hash-grid feature, say) is carried to ~2^-12 relative only, like one fp16 part.  The 1-pass modes keep the first
+// term only, max(2^-11 |x|, 2^-25) and 2^-8 |x| of an operand (fast, out of tolerance).
 // Range check: a value written into an operand (the embeddings included) whose hi part rounds to inf (fp16 modes:
 // |x| >= 65520) or that is NaN sets bit 0 of the context's sticky status word (pnr_status): overflow is reported, never
 // silent.  The ReLU keeps a NaN, as torch.relu does, so a NaN input or parameter reaches the outputs as well.

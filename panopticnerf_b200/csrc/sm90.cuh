@@ -174,8 +174,11 @@ __device__ __forceinline__ void mma_run_halves(float (&d0)[64], float (&d1)[64],
 
 // ---------------------------------------------------------------- 16-bit hi/lo split
 // x = hi + lo + residual, both parts rounded to nearest even in the operand format:
-//   bf16 (8-bit significand):  residual <= 2^-18 |x|, fp32 exponent range (never overflows)
-//   fp16 (11-bit significand): residual <= 2^-22 |x|, requires |x| < 65504
+//   bf16 (8-bit significand):  residual <= 2^-17 |x|, fp32 exponent range (never overflows)
+//   fp16 (11-bit significand): residual <= max(2^-23 |x|, 2^-25), requires |x| < 65504
+// The fp16 floor is half the subnormal spacing 2^-24: lo is subnormal once |x - hi| < 2^-14 (|x| below ~2^-3), so a
+// small operand keeps 2^-25 absolute - a 1e-4 value only ~2^-12 relative, like one fp16 part.  bf16 has no such floor
+// at the magnitudes a network holds.  (tests/test_cpu_operand_split.py)
 // Two values are packed per 32-bit word with the lower K index in the low half (K-major A operand).
 template <int FMT>
 __device__ __forceinline__ void split_x2(float x0, float x1, uint32_t& hi, uint32_t& lo) {

@@ -89,13 +89,18 @@ def split16(x: np.ndarray, bf16: bool):
     return hi.double().numpy(), lo.double().numpy()
 
 
-def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = False, grad_in=None):
+def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = False, grad_in=None, emb_x=None):
     """What the kernel computes for these samples, from the packed program.  Default: exact activations, float64
     (tests the program).  operand_precision=True also rounds the A operands like the tensor cores see them:
-    fp32 activations split into 16-bit hi (+ lo in the x3 modes), products hi*Whi (+ lo*Whi + hi*Wlo)."""
+    fp32 activations split into 16-bit hi (+ lo in the x3 modes), products hi*Whi (+ lo*Whi + hi*Wlo).
+    emb_x [S, E]: the embedding operand in place of gamma(pts) (a hash-grid network's h(x))."""
     S_ = pts.shape[0]
     bf16 = cfg.precision.startswith("bf16")
-    emb = np.zeros((S_, 64)); emb[:, :3 + 6 * cfg.xyz_res] = O.embed(pts, cfg.xyz_res).double().numpy()
+    emb = np.zeros((S_, 64))
+    if emb_x is None:
+        emb[:, :3 + 6 * cfg.xyz_res] = O.embed(pts, cfg.xyz_res).double().numpy()
+    else:
+        emb[:, :emb_x.shape[1]] = emb_x
     dirs = np.zeros((S_, 32)); dirs[:, :3 + 6 * cfg.view_res] = O.embed(viewdirs, cfg.view_res).double().numpy()
     act = {COL_A_HI: np.zeros((S_, 256)), COL_HEAD_HI: np.zeros((S_, 128))}
     acc = np.zeros((S_, 256))
