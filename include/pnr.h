@@ -547,7 +547,10 @@ int pnr_composite_backward(const float* raw, const float* z, const float* rays, 
  * transposed weight stream on the tensor cores, gradients split hi/lo like activations.  Samples are given as pts
  * [R*N,3] or as (rays [R,6], z [R,N]).  x3 precisions only; D <= 9.  grad_scale: a power of two applied to grad_h on
  * load and removed from everything the kernel writes (exact): pick it so that max |grad_h| * grad_scale is a few
- * hundred, or the fp16 operand parts of small gradients go subnormal (1.0 when grad_h is already O(1)). */
+ * hundred, or the fp16 operand parts of small gradients go subnormal (absolute floor 2^-25 / grad_scale; 1.0 when
+ * grad_h is already O(1)).  The same scale carries every intermediate dZ_j, which can grow well past max |grad_h|
+ * (a layer with small weights feeding one with large ones): one whose scaled value reaches 65520 in fp16x3 sets
+ * PNR_STATUS_RANGE; rerun with a smaller grad_scale. */
 int pnr_mlp_backward_trunk(pnr_ctx* ctx, const float* pts, const float* rays, const float* z, int64_t R, int32_t N,
                            const float* grad_h, float grad_scale, float* grad_emb, int32_t ld_emb, float* stash,
                            uint32_t* stash_absmax, void* stream);

@@ -37,7 +37,23 @@ layer as the local term |W| k.
 
 Encoder inputs.  h(x): exact (the fp32 oracle encoder is bit-identical to the kernel's).  gamma(x): p itself is exact;
 each sin / cos of the exact fp32 argument p 2^k is within CUDA's documented 2 ulp of sincosf.  gamma(d) in rays mode
-also carries the error of d / |d| formed in the kernel (`VIEWDIR_REL`)."""
+also carries the error of d / |d| formed in the kernel (`VIEWDIR_REL`).
+
+BACKWARD (`backward_bound`: pnr_mlp_backward_trunk, the stash it writes and d(trunk input)), pinned to the kernel's D
+ReLU masks M_i, so there are no kink terms: every slope is the mask's exact 0 or 1.  The kernel works in units scaled by
+grad_scale = gs (a power of two: the scaling and the stash's unscaling are exact), and so does the model:
+  Last layer.  g_{D-1} = gs dZ_{D-1} = M_{D-1} (gs grad_h), exact.
+  Step l.  acc = g_l W_l^T over the h columns of layer l's input (and, at layer 0 and the skip layer, over its embedded
+  columns), with W_l packed transposed from the same fp32 weights: a tensor-core layer with K = W and no bias add.  Its
+  local error is the split term of both operands, evaluated at the SCALED magnitude |g_l| + E (so the fp16 floor
+  2^-25 is 2^-25 / gs after unscaling), plus c 2^-23 |g_l| |W_l| with c = passes x W / 16 (no bias add).  Then
+  g_{l-1} = M_{l-1} acc: the error propagates through the pinned mask, the signs of W kept in the source matrices.
+  d(trunk input).  The skip layer writes its embedded columns first; layer 0 adds its own to them: one fp32
+  rounding of the sum, 2^-23 (|ref| + E).  Everything the kernel writes is divided by gs at the end.
+With acc=False (the replay accumulates exactly) the accumulation terms and the rounding of the sum drop out.
+A split whose fp16 lo part rounds toward zero still passes, in the forward as in the backward (the backward checked on
+the replay, every regime and grad_h regime): twice the floor stays within bounds that count every error at its worst
+sign."""
 from __future__ import annotations
 
 import torch
@@ -89,13 +105,15 @@ def _times(W, A):
 def linear(segs, b, precision, acc, delta, name, dW=None):
     """One tensor-core layer.  segs: (W [N, K], h_ref [S, K], Err of h, bound E of h) per K segment of the operand
     (the skip layer's [gamma(x) | h], the view layer's [h | gamma(d)]).  dW: the kernel's own error of the first
-    segment's weights (the fold).  Registers the layer's local bound as source `name` in delta; returns (pre-activation
-    reference, its Err)."""
+    segment's weights (the fold).  b None: no bias add (a backward step).  Registers the layer's local bound as source
+    `name` in delta; returns (pre-activation reference, its Err)."""
+    c = 1 if b is not None else 0
+    if b is None:
+        b = segs[0][1].new_zeros(segs[0][0].shape[0])
     ref = b[None].clone()
     local = torch.zeros_like(ref.expand(segs[0][1].shape[0], -1)).clone()
     absh = torch.zeros_like(local)
     terms = {}
-    c = 1
     for i, (W, h, err, E) in enumerate(segs):
         aW = W.abs() if (dW is None or i) else W.abs() + dW
         a = h.abs() + E                                    # |h| of the kernel's operand
@@ -117,9 +135,9 @@ def linear(segs, b, precision, acc, delta, name, dW=None):
     return ref, Err(terms, torch.zeros_like(local))
 
 
-def relu(ref, err, delta):
+def relu(ref, err, delta, E=None):
     """ReLU of the reference and of the error: exact slopes where |ref| > E, a kink bound k = E elsewhere."""
-    E = err.bound(delta)
+    E = err.bound(delta) if E is None else E
     kink = ref.abs() <= E
     m = torch.where(kink, 0.5, (ref > E).to(ref.dtype))
     terms = {s: (A * m if A.dim() == 2 else A * m[..., None]) for s, A in err.terms.items()}
@@ -169,18 +187,32 @@ def forward_bound(net, precision, ex, e_ex, ed, e_ed, acc=True, chunk=1024):
     return tuple(torch.cat(t, 0) for t in zip(*parts))
 
 
-def _forward_bound(net, precision, ex, e_ex, ed, e_ed, acc):
+def _trunk(net, precision, ex, e_ex, acc, delta):
+    """The trunk's forward layers: (h, its Err, its bound E, [(pre_i, E_pre_i, H_i, E_H_i)] per layer i): the reference
+    pre-activation, the bound of the kernel's pre-activation, the reference activation relu(pre_i) and the bound of
+    the kernel's activation.  Registers source "x" (the trunk input's error e_ex) in delta."""
     skip, dev = len(net.pts_linears) // 2, ex.device
-    delta = {"x": e_ex, "d": e_ed}
-    zero = torch.zeros_like
-    x_err, d_err = Err({"x": torch.ones_like(ex)}, zero(ex)), Err({"d": torch.ones_like(ed)}, zero(ed))
+    delta["x"] = e_ex
+    x_err = Err({"x": torch.ones_like(ex)}, torch.zeros_like(ex))
     h, err, E = ex, x_err, e_ex
+    layers = []
     for i, lin in enumerate(net.pts_linears):
         W, b = _p(lin, dev)
         segs = ([(W, h, err, E)] if i != skip + 1 else
                 [(W[:, :ex.shape[1]], ex, x_err, e_ex), (W[:, ex.shape[1]:], h, err, E)])
-        h, err = relu(*linear(segs, b, precision, acc, delta, f"L{i}"), delta)
+        pre, pre_err = linear(segs, b, precision, acc, delta, f"L{i}")
+        E_pre = pre_err.bound(delta)
+        h, err = relu(pre, pre_err, delta, E_pre)
         E = err.bound(delta)
+        layers.append((pre, E_pre, h, E))
+    return h, err, E, layers
+
+
+def _forward_bound(net, precision, ex, e_ex, ed, e_ed, acc):
+    dev = ex.device
+    delta = {"d": e_ed}
+    d_err = Err({"d": torch.ones_like(ed)}, torch.zeros_like(ed))
+    h, err, E, _ = _trunk(net, precision, ex, e_ex, acc, delta)
     sig, sig_err = dot_head(*_p(net.alpha_linear, dev), h, err, E, acc, delta, "sigma")
     # view layer: [W_view_h W_feat | W_view_d] [h | gamma(d)] + W_view_h b_feat + b_view, the fold rounded to fp32 from
     # a double sum: 2^-24 of |W_view_h| |W_feat| for the rounding, the double sum's error far below the other 2^-24
@@ -202,6 +234,97 @@ def _forward_bound(net, precision, ex, e_ex, ed, e_ed, acc):
             outs.append(logit)
             bounds.append(l_err.bound(delta))
     return torch.cat(outs, 1), torch.cat(bounds, 1), h, E
+
+
+def backward_bound(net, precision, ex, e_ex, grad_h, grad_scale, masks, acc=True, chunk=1024):
+    """The trunk backward (pnr_mlp_backward_trunk) pinned to the kernel's ReLU masks (masks[i] [S, W], 0 / 1: layer
+    i's pattern; the last one gates grad_h).  Returns a dict of float64 tensors on ex's device:
+        pre, E_pre, H, E_H: per trunk layer, the forward side (_trunk): reference pre-activation and activation, and
+                            the bounds of the kernel's (what the stash's H_i slots and the masks are checked against);
+        dZ, B_dZ:           per trunk layer j, the reference gradient w.r.t. its pre-activation and the bound of the
+                            kernel's (the stash's dZ_j slots);
+        d_in, B_in:         d(trunk input) [S, E] and its bound.
+    The model: BACKWARD in the module docstring."""
+    out = {}
+    for i in range(0, ex.shape[0], chunk):
+        sl = slice(i, i + chunk)
+        part = _backward_bound(net, precision, ex[sl], e_ex[sl], grad_h[sl], grad_scale, [m[sl] for m in masks], acc)
+        for k, v in part.items():
+            out.setdefault(k, []).append(v)
+    return {k: ([torch.cat(t, 0) for t in zip(*v)] if isinstance(v[0], list) else torch.cat(v, 0)) for k, v in out.items()}
+
+
+def _masked(err, M):
+    return Err({s: (A * M if A.dim() == 2 else A * M[..., None]) for s, A in err.terms.items()}, err.k * M)
+
+
+def _backward_bound(net, precision, ex, e_ex, grad_h, gs, masks, acc):
+    D, skip, dev = len(net.pts_linears), len(net.pts_linears) // 2, ex.device
+    Ex = ex.shape[1]
+    _, _, _, layers = _trunk(net, precision, ex, e_ex, acc, {})
+    delta = {}
+    M = [m.to(dev, torch.float64) for m in masks]
+    # scaled units throughout (the kernel's operands): g_{D-1} = M_{D-1} grad_h gs, exact
+    g = M[D - 1] * grad_h.to(dev, torch.float64) * gs
+    err = Err({}, torch.zeros_like(g))
+    E = torch.zeros_like(g)
+    dZ, B = [None] * D, [None] * D
+    dZ[D - 1], B[D - 1] = g / gs, E.clone()
+    parts = []                       # the d(trunk input) contributions: the skip layer's first, then layer 0's
+    for l in range(D - 1, -1, -1):
+        W = _p(net.pts_linears[l], dev)[0]
+        if l == 0 or l == skip + 1:
+            parts.append(linear([(W[:, :Ex].T, g, err, E)], None, precision, acc, delta, f"g{l}x"))
+        if l == 0:
+            break
+        ref, e = linear([(W[:, Ex:].T if l == skip + 1 else W.T, g, err, E)], None, precision, acc, delta, f"g{l}")
+        g, err = ref * M[l - 1], _masked(e, M[l - 1])
+        E = err.bound(delta)
+        dZ[l - 1], B[l - 1] = g / gs, E / gs
+    ref, err = parts[0]
+    if len(parts) == 2:              # layer 0's contribution added to the skip layer's: one fp32 rounding of the sum
+        ref1, err1 = parts[1]
+        ref = ref + ref1
+        terms = dict(err.terms)
+        for s, A in err1.terms.items():
+            terms[s] = terms[s] + A if s in terms else A
+        err = Err(terms, err.k + err1.k)
+        if acc:
+            delta["sum"] = U * (ref.abs() + err.bound(delta))
+            err.terms["sum"] = torch.ones_like(ref)
+    return {"pre": [t[0] for t in layers], "E_pre": [t[1] for t in layers], "H": [t[2] for t in layers],
+            "E_H": [t[3] for t in layers], "dZ": dZ, "B_dZ": B, "d_in": ref / gs, "B_in": err.bound(delta) / gs}
+
+
+# ------------------------------------------------------------------------------------------------ pnr_wgrad
+WGRAD_U = {"fp16x3": 2.0 ** -11, "bf16x3": 2.0 ** -8}    # unit roundoff of one 16-bit operand part
+WGRAD_RUN_SLABS = 16                                    # slabs of 64 samples per run of pnr_wgrad's register accumulators
+
+
+def wgrad_slabs_per_cta(S, No, sms):
+    """(64-sample slabs per CTA, CTAs per column block) of one pnr_wgrad call on a device with `sms` SMs."""
+    mh = 2 if No > 128 else 1
+    slabs = -(-S // 64)
+    G = max(1, min(slabs, max(sms // mh, 1)))
+    return -(-slabs // G), G
+
+
+def wgrad_tau(prec, S, No, sms):
+    """tau of one pnr_wgrad call (tests/test_gpu_train_limits.py): the operand split, 3 products x 4 k-steps per slab
+    accumulated in one run, and the round-to-nearest adds of the runs and of the CTAs' partials."""
+    per_cta, G = wgrad_slabs_per_cta(S, No, sms)
+    runs = -(-per_cta // WGRAD_RUN_SLABS)
+    return 3 * WGRAD_U[prec] ** 2 + 12 * min(per_cta, WGRAD_RUN_SLABS) * 2.0 ** -23 + 4 * (runs + G) ** 0.5 * 2.0 ** -24
+
+
+def wgrad_bound(A, ab, cx, S, No, prec, sc, sms):
+    """pnr_wgrad's per-element bound of dW = dZ^T X and db = column sums of dZ, from the operands it was given:
+    A = |dZ|^T |X|, ab = column sums of |dZ|, cx = column sums of |X|; sc = the dz_scale it ran with (1: none).
+    dW: tau A + floor, the floor 2^-24 (cx / sc + ab) in fp16x3 where a 16-bit part can be subnormal; db: 2^-24 (S + 64) ab."""
+    bW = wgrad_tau(prec, S, No, sms) * A
+    if prec == "fp16x3":
+        bW = bW + 2.0 ** -24 * (cx[None, :] / sc + ab[:, None])
+    return bW, 2.0 ** -24 * (S + 64) * ab
 
 
 # ------------------------------------------------------------------------------------------------ regimes

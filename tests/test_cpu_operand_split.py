@@ -21,11 +21,11 @@ import numpy as np
 import pytest
 import torch
 
-from oracle_bound import encoding, forward_bound, twin, view_encoding
+from oracle_bound import backward_bound, encoding, forward_bound, twin, view_encoding
 from oracle_hashgrid import SCENE_AABB, hash_cfg, oracle_like
 from panopticnerf_b200 import make_cfg, make_network, synthetic as S
 from test_cpu_hashgrid_network import build
-from test_cpu_program import F_WAIT_E0, replay, split16, to_f32
+from test_cpu_program import F_WAIT_E0, PROGRAM_BACKWARD, REPLAY_DEFECTS, replay, split16, to_f32
 
 # (relative, floor) of r (both parts) and of r1 (hi alone)
 RESIDUAL = {"fp16": ((2.0 ** -23, 2.0 ** -25), (2.0 ** -11, 2.0 ** -25)), "bf16": ((2.0 ** -17, 0.0), (2.0 ** -8, 0.0))}
@@ -223,3 +223,97 @@ def test_bound_holds_and_is_tight_on_the_replay(regime, precision):
     print(f"{regime[0]} k={k} {precision}: worst |err|/B = {worst:.3g}")
     assert worst <= 1.0, f"{regime[0]} {precision}: an element outside the bound ({worst:.3g})"
     assert worst >= TIGHT, f"{regime[0]} {precision}: the bound is loose ({worst:.3g})"
+
+
+# ------------------------------------------------------------------------------------------------ backward bound vs replay
+GRADS = ("unit", "tiny-unscaled", "spread")
+
+
+def default_grad_scale(grad_h):
+    """The power of two Network.backward_trunk picks: max |grad_h| * grad_scale ~ 256."""
+    m = float(grad_h.abs().max())
+    return 2.0 ** max(-100, min(100, round(math.log2(256.0 / m))))
+
+
+def grad_regime(name, n, W, seed):
+    """(grad_h [n, W], grad_scale).  unit: O(1) at the default scale; tiny-unscaled: 2^-20 O(1) with grad_scale = 1, so
+    the fp16 parts of every gradient are subnormal; spread: columns over 2^-12 .. 2^4, default scale.  No entry is 0:
+    a nonzero dZ_{D-1} is then exactly the last layer's mask."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(n, W, generator=g)
+    x = torch.where(x == 0, torch.ones_like(x), x)
+    if name == "tiny-unscaled":
+        return x * 2.0 ** -20, 1.0
+    if name == "spread":
+        x = x * torch.exp2(torch.linspace(-12.0, 4.0, W))[torch.randperm(W, generator=g)]
+    return x, default_grad_scale(x)
+
+
+def fp16_safe_scale(b, gs):
+    """The largest power of two <= gs that keeps every float64 dZ_j (j < D-1: the loaded one is at most ~256) times
+    the scale below 2^14, inside the fp16 range check with room to spare."""
+    m = max(float(d.abs().max()) for d in b["dZ"])
+    return min(gs, 2.0 ** math.floor(math.log2(2.0 ** 14 / m))) if m > 0 else gs
+
+
+def stash_masks(H, dZ_last):
+    """The kernel's D ReLU masks from its stash: H_i > 0 for i < D-1, dZ_{D-1} != 0 for the last layer."""
+    return [(h > 0).double() for h in H] + [(dZ_last != 0).double()]
+
+
+def backward_ratios(b, dZ, d_in):
+    """Worst |err| / B per dZ_j and of d(trunk input)."""
+    out = {f"dZ{j}": float(ratio(dZ[j], b["dZ"][j], b["B_dZ"][j]).max()) for j in range(len(dZ))}
+    out["d_in"] = float(ratio(d_in, b["d_in"], b["B_in"]).max())
+    return out
+
+
+def _replay_backward(cfg, net, regime, pts, ex, grad_h, gs, defect=None):
+    prog, w16, consts = build(cfg, net, flags=PROGRAM_BACKWARD)
+    stash = {}
+    d_in, _ = replay(prog, w16, consts, cfg, pts, torch.zeros_like(pts), operand_precision=True,
+                     grad_in=grad_h.double().numpy(), emb_x=ex.numpy() if regime[1] is not None else None,
+                     grad_scale=gs, stash=stash, defect=defect)
+    D = cfg.D
+    H = [torch.from_numpy(stash[i]) for i in range(D - 1)]
+    dZ = [torch.from_numpy(stash[2 * D - 2 - j]) for j in range(D)]
+    return torch.from_numpy(d_in)[:, :ex.shape[1]], H, dZ
+
+
+def _backward_case(precision, regime, grad, n=512, defect=None):
+    cfg, net = make_regime(precision, regime, W=128)
+    pts, _ = regime_points(regime, n, seed=5)
+    ex, e_ex = trunk_input(cfg, net, pts)
+    net, k = apply_twin(net, regime, ex)
+    grad_h, gs = grad_regime(grad, n, cfg.W, seed=7)
+    d_in, H, dZ = _replay_backward(cfg, net, regime, pts, ex, grad_h, gs, defect)
+    masks = stash_masks(H, dZ[-1])
+    b = backward_bound(net, precision, ex, e_ex, grad_h, gs, masks, acc=False)
+    if precision == "fp16x3" and fp16_safe_scale(b, gs) < gs:      # the kernel would flag this scale: rerun below it
+        gs = fp16_safe_scale(b, gs)
+        d_in, H, dZ = _replay_backward(cfg, net, regime, pts, ex, grad_h, gs, defect)
+        b = backward_bound(net, precision, ex, e_ex, grad_h, gs, masks, acc=False)
+    return backward_ratios(b, dZ, d_in), f"{regime[0]} k={k} {precision} {grad} gs=2^{int(math.log2(gs))}"
+
+
+@pytest.mark.parametrize("grad", GRADS)
+@pytest.mark.parametrize("precision", ["fp16x3", "bf16x3"])
+@pytest.mark.parametrize("regime", REGIMES, ids=[r[0] for r in REGIMES])
+def test_backward_bound_holds_and_is_tight_on_the_replay(regime, precision, grad):
+    """oracle_bound.backward_bound against the backward program's replay (operands rounded as the tensor cores see
+    them, exact accumulation), pinned to the masks of the replay's own stash: every dZ_j slot and every element of
+    d(trunk input) within B, and the worst at least TIGHT of B."""
+    worst, name = _backward_case(precision, regime, grad)
+    print(f"{name}: " + " ".join(f"{g}={v:.3g}" for g, v in worst.items()))
+    assert max(worst.values()) <= 1.0, f"{name}: an element outside the bound {worst}"
+    assert max(worst.values()) >= TIGHT, f"{name}: the bound is loose {worst}"
+
+
+@pytest.mark.parametrize("precision", ["fp16x3", "bf16x3"])
+@pytest.mark.parametrize("defect", REPLAY_DEFECTS)
+def test_backward_bound_rejects_a_defective_kernel(defect, precision):
+    """Each deliberate defect of the replay (a 1-pass gradient operand, a mask one layer off, grad_scale left in the
+    dZ_0 slot, the skip layer's d(input) overwritten by layer 0's) takes some element outside the bound."""
+    worst, name = _backward_case(precision, REGIMES[0], "unit", defect=defect)
+    print(f"{defect} {name}: " + " ".join(f"{g}={v:.3g}" for g, v in worst.items()))
+    assert max(worst.values()) > 1.0, f"{defect} {name}: the bound does not see it {worst}"

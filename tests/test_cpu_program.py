@@ -89,11 +89,22 @@ def split16(x: np.ndarray, bf16: bool):
     return hi.double().numpy(), lo.double().numpy()
 
 
-def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = False, grad_in=None, emb_x=None):
+REPLAY_DEFECTS = ("grad_hi_only", "mask_of_next_layer", "scale_left_in_dz0", "skip_overwritten")
+
+
+def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = False, grad_in=None, emb_x=None,
+           grad_scale: float = 1.0, stash=None, defect=None):
     """What the kernel computes for these samples, from the packed program.  Default: exact activations, float64
     (tests the program).  operand_precision=True also rounds the A operands like the tensor cores see them:
     fp32 activations split into 16-bit hi (+ lo in the x3 modes), products hi*Whi (+ lo*Whi + hi*Wlo).
-    emb_x [S, E]: the embedding operand in place of gamma(pts) (a hash-grid network's h(x))."""
+    emb_x [S, E]: the embedding operand in place of gamma(pts) (a hash-grid network's h(x)).
+    Backward programs: grad_in is multiplied by grad_scale as it is loaded and every gradient written is divided by it
+    (pnr_mlp_backward_trunk); `stash` (a dict) receives every stash slot the program writes, keyed by slot
+    (EpiDesc.out_off1 - 1): H_i in slot i < D-1, dZ_j in slot 2D-2-j.
+    defect: one of REPLAY_DEFECTS, a kernel made wrong on purpose, for the tests that check a bound rejects it: the
+    gradient operands keep only their hi part; dZ_0 gated by layer 1's mask instead of layer 0's; dZ_0 stashed
+    without the division by grad_scale; layer 0's d(input) overwriting the skip layer's instead of adding to it."""
+    assert defect is None or defect in REPLAY_DEFECTS
     S_ = pts.shape[0]
     bf16 = cfg.precision.startswith("bf16")
     emb = np.zeros((S_, 64))
@@ -105,7 +116,7 @@ def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = Fals
     act = {COL_A_HI: np.zeros((S_, 256)), COL_HEAD_HI: np.zeros((S_, 128))}
     acc = np.zeros((S_, 256))
     CH = 4 + cfg.num_classes + cfg.num_instances
-    out = np.zeros((S_, CH if grad_in is None else 3 + 6 * cfg.xyz_res))
+    out = np.zeros((S_, CH if grad_in is None else 3 + 6 * cfg.xyz_res if emb_x is None else emb_x.shape[1]))
     sig = np.zeros(S_)
     masks = {}                       # backward programs: ReLU sign pattern per slot
     step = -1
@@ -147,6 +158,8 @@ def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = Fals
                 acc[:, sd.acc_col:sd.acc_col + n] = 0.0
             if operand_precision:
                 a_hi, a_lo = split16(A, bf16)
+                if defect == "grad_hi_only" and s >= cfg.D:      # the backward steps: A is a gradient
+                    a_lo = np.zeros_like(a_lo)
                 prod = a_hi @ W.T
                 if prog.passes == 3:
                     prod = prod + a_lo @ W.T + a_hi @ Wlo.T
@@ -164,18 +177,27 @@ def replay(prog, w16, consts, cfg, pts, viewdirs, operand_precision: bool = Fals
         v = acc[:, ed.acc_col:ed.acc_col + n] + consts[ed.bias_off:ed.bias_off + n][None]
         if ed.kind == EPI_MASK_TO_A:         # gradient w.r.t. a hidden layer's output, gated by its sign pattern
             v = acc[:, ed.acc_col:ed.acc_col + n]
-            act[ed.dst_col][:, :n] = np.where(masks[ed.n_valid - 1][:, :n], v, 0.0) if ed.n_valid else v
+            slot = ed.n_valid if (defect == "mask_of_next_layer" and ed.n_valid == 1) else ed.n_valid - 1
+            act[ed.dst_col][:, :n] = np.where(masks[slot][:, :n], v, 0.0) if ed.n_valid else v
+            if stash is not None and ed.out_off1:
+                keep = defect == "scale_left_in_dz0" and ed.n_valid == 1
+                stash[ed.out_off1 - 1] = act[ed.dst_col][:, :n] / (1.0 if keep else grad_scale)
         elif ed.kind == EPI_LOADG_TO_A:      # last forward layer: the incoming gradient gated by its own pattern
-            act[ed.dst_col][:, :n] = np.where(v > 0.0, grad_in[:, :n], 0.0)
+            act[ed.dst_col][:, :n] = np.where(v > 0.0, grad_in[:, :n] * grad_scale, 0.0)
+            if stash is not None and ed.out_off1:
+                stash[ed.out_off1 - 1] = act[ed.dst_col][:, :n] / grad_scale
         elif ed.kind == EPI_GRAD_OUT:
-            v = acc[:, ed.acc_col:ed.acc_col + ed.n_valid]
-            out[:, ed.out_off:ed.out_off + ed.n_valid] = v + (out[:, ed.out_off:ed.out_off + ed.n_valid] if ed.n_valid1 else 0.0)
+            v = acc[:, ed.acc_col:ed.acc_col + ed.n_valid] / grad_scale
+            add = ed.n_valid1 and defect != "skip_overwritten"
+            out[:, ed.out_off:ed.out_off + ed.n_valid] = v + (out[:, ed.out_off:ed.out_off + ed.n_valid] if add else 0.0)
         elif ed.kind == EPI_RELU_TO_A:
             v = np.maximum(v, 0.0)
             if ed.sigma:
                 sig = v @ consts[ed.aux_off:ed.aux_off + n].astype(np.float64)
             if grad_in is not None and ed.n_valid:
                 masks[ed.n_valid - 1] = v > 0.0
+            if stash is not None and ed.out_off1:
+                stash[ed.out_off1 - 1] = v.copy()
             act[ed.dst_col][:, :n] = v
         elif ed.kind == EPI_VIEW_RGB:
             v = np.maximum(v, 0.0)

@@ -21,6 +21,7 @@ import math
 import pytest
 import torch
 
+from oracle_bound import WGRAD_RUN_SLABS, WGRAD_U, wgrad_bound
 from panopticnerf_b200 import _capi
 from panopticnerf_b200.lib.train.mlp_backward import _pow2_scale
 
@@ -28,8 +29,8 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 F64 = torch.float64
 CHUNK = 1 << 18
-U = {"fp16x3": 2.0 ** -11, "bf16x3": 2.0 ** -8}       # unit roundoff of one 16-bit operand part
-RUN_SLABS = 16                                        # pnr_wgrad: slabs of 64 samples per run of the register accumulators
+U = WGRAD_U                                            # unit roundoff of one 16-bit operand part
+RUN_SLABS = WGRAD_RUN_SLABS                           # pnr_wgrad: slabs of 64 samples per run of the register accumulators
 CONTRACT = {"fp16x3": 2e-5, "bf16x3": 1e-4}           # pnr_wgrad's dW: max error / RMS of the result
 
 
@@ -96,29 +97,13 @@ def _ref_wgrad(dz, x):
     return R, A, rb, ab, cx
 
 
-def _slabs_per_cta(S, No):
-    mh = 2 if No > 128 else 1
-    slabs = -(-S // 64)
-    G = max(1, min(slabs, max(_sms() // mh, 1)))
-    return -(-slabs // G), G
-
-
-def _wgrad_tau(prec, S, No):
-    """tau of the module docstring for one pnr_wgrad call: 3 products x 4 k-steps per slab accumulate in one run."""
-    per_cta, G = _slabs_per_cta(S, No)
-    runs = -(-per_cta // RUN_SLABS)
-    return 3 * U[prec] ** 2 + 12 * min(per_cta, RUN_SLABS) * 2.0 ** -23 + 4 * math.sqrt(runs + G) * 2.0 ** -24
-
-
 def _check_wgrad(W, b, ref, S, prec, sc, what, contract=True):
-    """Every element of dW and db within its bound; dW within the path's contract of the RMS, db within 1e-4."""
+    """Every element of dW and db within its bound (oracle_bound.wgrad_bound); dW within the path's contract of the
+    RMS, db within 1e-4."""
     R, A, rb, ab, cx = ref
-    tau = _wgrad_tau(prec, S, R.shape[0])
-    floor = 0.0
-    if prec == "fp16x3":
-        floor = 2.0 ** -24 * (cx[None, :] / sc + ab[:, None])
-    r = _ratio((W.double() - R).abs(), tau * A + floor)
-    rbias = _ratio((b.double() - rb).abs(), 2.0 ** -24 * (S + 64) * ab) if b is not None else 0.0
+    bW, bb = wgrad_bound(A, ab, cx, S, R.shape[0], prec, sc, _sms())
+    r = _ratio((W.double() - R).abs(), bW)
+    rbias = _ratio((b.double() - rb).abs(), bb) if b is not None else 0.0
     _report(f"{what} dW", r)
     _report(f"{what} db", rbias)
     if contract:
