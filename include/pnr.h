@@ -264,6 +264,73 @@ typedef struct pnr_ray_batch_args {
 } pnr_ray_batch_args;
 int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream);
 
+/* Weighted draws (DESIGN 3.4): pnr_sample_ray_batch with the pixel drawn through a per-pixel weight table weight [P]
+ * u16 (pnr_pixel_weights) and its group sums weight_cum [ceil(P/32)] u64 (pnr_pixel_cdf), with T = weight_total and
+ * weight_nonzero (the count of non-zero weights) passed by value.  Block 0 gives x = mulhi64(w0 << 32 | w1, T) and the
+ * pixel is the smallest p with S(p) > x, S(p) = sum_{q <= p} weight[q]: an upper-bound search of weight_cum for the
+ * group of 32 pixels, then a scan of its weights.  A pixel of weight 0 is never drawn, and a table of all ones draws
+ * p = x, the unweighted pixel, so every output equals pnr_sample_ray_batch's bit for bit.  The frame, ray, targets and
+ * jitter follow from p as there.  importance [r1 - r0] f32 (nullable) = fp32(T / (weight_nonzero weight[p])) in
+ * double, one division rounded once: its mean under the draw is 1.
+ * Refused before any launch (PNR_ERR_ARG, by name): everything pnr_sample_ray_batch refuses; a null w, weight or
+ * weight_cum, weight_total = 0, weight_nonzero outside [1, P], weight_total outside [weight_nonzero,
+ * 65535 weight_nonzero]. */
+typedef struct pnr_ray_batch_weights {
+  const uint16_t* weight;       /* [P] u16 device                                                                */
+  const uint64_t* weight_cum;   /* [ceil(P/32)] u64 device (pnr_pixel_cdf's cum)                                 */
+  uint64_t weight_total;        /* T = the sum of the weights (pnr_pixel_cdf's totals[0])                        */
+  int64_t weight_nonzero;       /* the count of non-zero weights (totals[1])                                     */
+  float* importance;            /* [r1 - r0] f32 device, nullable: T / (weight_nonzero weight[p])                */
+} pnr_ray_batch_weights;
+int pnr_sample_ray_batch_weighted(const pnr_ray_batch_args* args, const pnr_ray_batch_weights* w, void* stream);
+
+/* Per-pixel weights of a frame set for weighted draws (DESIGN 3.4).  Rule (chosen here), per pixel q of frame f,
+ * slot = 1 + label for a label in [0, C), else 0 (-1 and any other value; every pixel without a label table):
+ *   x = (scale * frame_factor[f]) * class_factor[slot] in fp32, each product rounded, no FMA (a NULL table reads 1);
+ *   weight = 0 when the camera's mask is 0 at q, when x is NaN or x <= 0; 65535 when x >= 65535 (+Inf included);
+ *   otherwise x rounded to the nearest integer, ties to even (0.5 -> 0, 1.5 -> 2, 65534.5 -> 65534).
+ * Inputs: the frame table as pnr_ray_batch_args (frame_cam [F], pix_offset [F+1], P, cams; a malformed device table is
+ * clamped, never read or written outside, and a frame's pixels past its camera's H W are given weight 0), label [P]
+ * i16 (nullable), frame_factor [F] f32 and class_factor [C+1] f32 (nullable), mask[k] [H_k W_k] u8 of camera k
+ * (nullable; non-zero = keep), all on the device.  Output weight [P] u16: the pixels of the frames of the table are
+ * written, every other byte is left as it is.  No host copy or synchronisation: the call can be captured.
+ * Refused before any launch (PNR_ERR_ARG, by name): F < 1 or >= 2^31 - 1, P < 1, C outside [0, 32767], num_cameras
+ * outside [1, PNR_RAY_BATCH_MAX_CAMERAS], a camera model other than 0 / 2 or H, W outside [1, 2^31), a null
+ * frame_cam, pix_offset or weight, scale not finite and > 0. */
+typedef struct pnr_pixel_weights_args {
+  const int32_t* frame_cam;     /* [F] device                                                                    */
+  const int64_t* pix_offset;    /* [F+1] device                                                                  */
+  int32_t F;
+  int64_t P;
+  pnr_ray_camera cams[PNR_RAY_BATCH_MAX_CAMERAS];
+  int32_t num_cameras;
+  const int16_t* label;         /* [P] device, nullable                                                          */
+  int32_t C;                    /* classes: class_factor has C + 1 entries (slot 0 = outside [0, C))             */
+  const float* frame_factor;    /* [F] device, nullable = 1                                                      */
+  const float* class_factor;    /* [C+1] device, nullable = 1                                                    */
+  const uint8_t* mask[PNR_RAY_BATCH_MAX_CAMERAS];   /* [H*W] device per camera, nullable = keep every pixel     */
+  float scale;
+  uint16_t* weight;             /* [P] device                                                                    */
+} pnr_pixel_weights_args;
+int pnr_pixel_weights(const pnr_pixel_weights_args* args, void* stream);
+
+/* Class histogram of a label table: counts [C+1] u64 (device), slot 0 = labels outside [0, C) (-1 included), slot
+ * 1 + c = class c.  Integer sums: exact and independent of the order of the pixels.  counts is overwritten (zeroed
+ * on the stream first).  Refused (PNR_ERR_ARG, by name): P < 1, C outside [0, 8191], a null label or counts. */
+int pnr_label_counts(const int16_t* label, int64_t P, int32_t C, uint64_t* counts, void* stream);
+
+/* Exact prefix sum of a weight table in groups of 32 pixels: cum[g] = sum_{q < min(P, 32 (g+1))} weight[q] u64, for
+ * g < ceil(P/32), and totals[2] u64 = {T = the sum of all weights, the count of non-zero weights}, all on the device.
+ * Integer addition: every schedule gives the same bits.  Reduce-then-scan: per tile of 2^15 pixels its sum, one
+ * block's scan of the tile sums, then per tile the group sums scanned on top of its prefix (the weights are read
+ * twice).  No host copy or synchronisation: the call can be captured.  workspace: pnr_pixel_cdf_workspace_bytes(P)
+ * bytes of device scratch, 16-byte aligned (two u64 per tile); 0 for P outside [1, 2^47).
+ * Refused (PNR_ERR_ARG, by name): P outside [1, 2^47), a null or misaligned (16 bytes) weight, a null cum or totals,
+ * a short or misaligned workspace. */
+size_t pnr_pixel_cdf_workspace_bytes(int64_t P);
+int pnr_pixel_cdf(const uint16_t* weight, int64_t P, uint64_t* cum, uint64_t* totals, void* workspace,
+                  size_t workspace_bytes, void* stream);
+
 /* Depth targets from LiDAR scans (DESIGN 3.4): the points of scan s, projected into frame f of a frame set, leave per
  * pixel the nearest depth, written into that set's depth table.  Rules (chosen here: the reference's preprocessing
  * is not public):

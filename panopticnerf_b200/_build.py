@@ -14,7 +14,8 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libpnr.so"
-SOURCES = ["pnr_api.cu", "ray_kernels.cu", "stream_kernels.cu", "mlp_wgmma.cu", "render.cu", "comm.cu", "panoptic_kernels.cu", "wgrad_wgmma.cu", "linear_wgmma.cu", "eval_kernels.cu", "optim_kernels.cu", "stereo_kernels.cu"]
+SOURCES = ["pnr_api.cu", "ray_kernels.cu", "stream_kernels.cu", "mlp_wgmma.cu", "render.cu", "comm.cu", "panoptic_kernels.cu", "wgrad_wgmma.cu", "linear_wgmma.cu", "eval_kernels.cu", "optim_kernels.cu", "stereo_kernels.cu",
+           "weight_kernels.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC"] + os.environ.get("PNR_NVCC_FLAGS", "").split()
 
@@ -88,6 +89,16 @@ def build_host_emu() -> Path:
     out.parent.mkdir(exist_ok=True)
     subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
                            str(PKG.parent / "tests" / "host_emu.cpp")])
+    return out
+
+
+def build_host_emu_weights() -> Path:
+    """g++ tests/host_emu_weights.cpp -> build/host_emu_weights.so: the host build of the weighted-draw routines of
+    csrc/ray_math.h, with build_host_emu's flags."""
+    out = PKG.parent / "build" / "host_emu_weights.so"
+    out.parent.mkdir(exist_ok=True)
+    subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", str(out),
+                           str(PKG.parent / "tests" / "host_emu_weights.cpp")])
     return out
 
 

@@ -114,6 +114,20 @@ class PnrRayBatchArgs(C.Structure):
                [(k, C.c_void_p) for k in ("rays", "rgb", "depth_out", "pseudo_label", "u", "u_fine", "pixel", "frame")]
 
 
+class PnrRayBatchWeights(C.Structure):
+    """pnr_ray_batch_weights of include/pnr.h (same field order)."""
+    _fields_ = [("weight", C.c_void_p), ("weight_cum", C.c_void_p), ("weight_total", C.c_uint64),
+                ("weight_nonzero", C.c_int64), ("importance", C.c_void_p)]
+
+
+class PnrPixelWeightsArgs(C.Structure):
+    """pnr_pixel_weights_args of include/pnr.h (same field order)."""
+    _fields_ = [("frame_cam", C.c_void_p), ("pix_offset", C.c_void_p), ("F", C.c_int32), ("P", C.c_int64),
+                ("cams", PnrRayCamera * RAY_BATCH_MAX_CAMERAS), ("num_cameras", C.c_int32), ("label", C.c_void_p),
+                ("C", C.c_int32), ("frame_factor", C.c_void_p), ("class_factor", C.c_void_p),
+                ("mask", C.c_void_p * RAY_BATCH_MAX_CAMERAS), ("scale", C.c_float), ("weight", C.c_void_p)]
+
+
 class PnrProjectDepthArgs(C.Structure):
     """pnr_project_depth_args of include/pnr.h (same field order); scan_offset and the pair tables are host pointers."""
     _fields_ = [("points", C.c_void_p), ("Npts", C.c_int64), ("scan_offset", C.c_void_p), ("S", C.c_int32),
@@ -159,6 +173,11 @@ SIGNATURES = {
     "pnr_tag_samples": (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
     "pnr_generate_rays": (C.c_int, [_i32, _i32, _i32, _i32, _i32, C.POINTER(_f32), C.POINTER(_f32), _vp, _vp]),
     "pnr_sample_ray_batch": (C.c_int, [C.POINTER(PnrRayBatchArgs), _vp]),
+    "pnr_sample_ray_batch_weighted": (C.c_int, [C.POINTER(PnrRayBatchArgs), C.POINTER(PnrRayBatchWeights), _vp]),
+    "pnr_pixel_weights": (C.c_int, [C.POINTER(PnrPixelWeightsArgs), _vp]),
+    "pnr_label_counts": (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
+    "pnr_pixel_cdf_workspace_bytes": (C.c_size_t, [_i64]),
+    "pnr_pixel_cdf": (C.c_int, [_vp, _i64, _vp, _vp, _vp, C.c_size_t, _vp]),
     "pnr_project_depth_workspace_bytes": (C.c_size_t, [_i64, _i32]),
     "pnr_project_depth": (C.c_int, [C.POINTER(PnrProjectDepthArgs), _vp]),
     "pnr_stereo_workspace_bytes": (C.c_size_t, [_i32, _i32, _i32, _i32]),

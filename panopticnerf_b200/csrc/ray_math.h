@@ -1,6 +1,8 @@
 // ray_math.h — per-ray arithmetic with a fully specified fp32 operation order, shared by the CUDA
-// kernels (ray_kernels.cu, rays_kernel, ray_batch_kernel and the depth kernels in stream_kernels.cu) and the host build
-// used by the CPU tests (tests/host_emu.cpp) to prove the order matches the oracle bit for bit without a GPU.  The kernels keep only layout
+// kernels (ray_kernels.cu, rays_kernel, ray_batch_kernel and the depth kernels in stream_kernels.cu, the weight kernels
+// in weight_kernels.cu) and the host build
+// used by the CPU tests (tests/host_emu.cpp; the weighted draws' routines in tests/host_emu_weights.cpp) to prove the
+// order matches the oracle bit for bit without a GPU.  The kernels keep only layout
 // here (staging, shuffles, sorts); the rules they apply per ray - the per-primitive intersection step, range clamps,
 // sample depths, output slots, camera directions, batch draws - are the functions below, called by both builds.  One
 // piece stays written out in stratified_kernel and again in host_emu.cpp: the interval test (pnr_tag's rule), because
@@ -30,6 +32,7 @@
 #define PNR_DADD(a, b) __dadd_rn((a), (b))
 #define PNR_DSUB(a, b) __dsub_rn((a), (b))
 #define PNR_DMUL(a, b) __dmul_rn((a), (b))
+#define PNR_DDIV(a, b) __ddiv_rn((a), (b))
 #define PNR_SQRT(a) __fsqrt_rn((a))
 #define PNR_LDG(p) __ldg((p))
 #else
@@ -40,6 +43,7 @@
 #define PNR_DADD(a, b) ((a) + (b))
 #define PNR_DSUB(a, b) ((a) - (b))
 #define PNR_DMUL(a, b) ((a) * (b))
+#define PNR_DDIV(a, b) ((a) / (b))
 #define PNR_SQRT(a) sqrtf((a))
 #define PNR_LDG(p) (*(p))
 #endif
@@ -553,12 +557,82 @@ PNR_HD int pnr_frame_of(const int64_t* off, int F, int64_t p) {
 // an 8-bit colour channel -> [0, 1], as torch's u8.float() / 255 on the CPU (true division)
 PNR_HD float pnr_u8_unit(uint8_t b) { return PNR_DIV((float)b, 255.0f); }
 
+// ---------------------------------------------------------------------------------------------- weighted draws
+// pnr_pixel_weights / pnr_pixel_cdf / pnr_sample_ray_batch_weighted (include/pnr.h; DESIGN 3.4).
+
+#define PNR_WEIGHT_GROUP 32         // pixels per entry of the weight table's prefix sum
+#define PNR_WEIGHT_MAX 65535.0f
+
+// the class-factor slot of a label: 1 + label for a label in [0, C), else 0 (-1 and every other value)
+PNR_HD int pnr_weight_slot(int16_t label, int C) { return (label >= 0 && label < C) ? 1 + label : 0; }
+// one pixel's weight: x = (scale * frame_factor) * class_factor in fp32, each product rounded; 0 when masked, NaN or
+// x <= 0; 65535 when x >= 65535 (+Inf too); otherwise x rounded to the nearest integer, ties to even (adding and
+// subtracting 2^23 rounds a float in [0, 2^23) to an integer in the current mode, round-to-nearest-even)
+PNR_HD uint16_t pnr_pixel_weight(bool keep, float scale, float frame_factor, float class_factor) {
+  if (!keep) return 0;
+  const float x = PNR_MUL(PNR_MUL(scale, frame_factor), class_factor);
+  if (!(x > 0.f)) return 0;
+  if (x >= PNR_WEIGHT_MAX) return 65535;
+  return (uint16_t)PNR_SUB(PNR_ADD(x, 8388608.0f), 8388608.0f);
+}
+// pixel q of frame f (camera cam, of n clamped pixels starting at lo) under the rule above.  A camera mask covers the
+// camera's H W pixels; a pixel past them (a malformed table) is not kept.
+PNR_HD uint16_t pnr_weight_of_pixel(const pnr_pixel_weights_args& a, int f, int cam, int64_t lo, int64_t q) {
+  const uint8_t* mask = a.mask[0];
+#pragma unroll
+  for (int k = 1; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k)
+    if (k == cam) mask = a.mask[k];
+  int64_t HW = 0;
+#pragma unroll
+  for (int k = 0; k < PNR_RAY_BATCH_MAX_CAMERAS; ++k)
+    if (k == cam) HW = (int64_t)a.cams[k].H * a.cams[k].W;
+  const bool keep = q < HW && (mask == nullptr || mask[q] != 0);
+  const float ff = a.frame_factor ? a.frame_factor[f] : 1.0f;
+  const int slot = a.label ? pnr_weight_slot(a.label[lo + q], a.C) : 0;
+  const float cf = a.class_factor ? a.class_factor[slot] : 1.0f;
+  return pnr_pixel_weight(keep, a.scale, ff, cf);
+}
+// the weighted pick: the smallest p with S(p) > x, S the inclusive prefix sum of weight [P], through its group sums
+// cum [ceil(P / 32)] (cum[g] = S(min(P, 32 (g + 1)) - 1)): an upper-bound search of cum for the group, then a scan of
+// its (at most 32) weights.  Tables that disagree with x are clamped: the result always lies in [0, P).
+PNR_HD int64_t pnr_weighted_pixel(const uint16_t* weight, const uint64_t* cum, int64_t P, uint64_t x) {
+  const int64_t G = (P + PNR_WEIGHT_GROUP - 1) / PNR_WEIGHT_GROUP;
+  int64_t lo = 0, hi = G;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (PNR_LDG(cum + mid) <= x) lo = mid + 1; else hi = mid;
+  }
+  const int64_t g = lo < G ? lo : G - 1;
+  uint64_t s = g > 0 ? PNR_LDG(cum + g - 1) : 0;
+  const int64_t q0 = g * PNR_WEIGHT_GROUP, q1 = q0 + PNR_WEIGHT_GROUP < P ? q0 + PNR_WEIGHT_GROUP : P;
+  for (int64_t q = q0; q < q1; ++q) {
+    s += PNR_LDG(weight + q);
+    if (s > x) return q;
+  }
+  return q1 - 1;
+}
+// the reweighting factor of a drawn pixel of weight w: T / (nonzero w), one double division, rounded to fp32 once
+PNR_HD float pnr_importance(uint64_t T, int64_t nonzero, uint16_t w) {
+  return (float)PNR_DDIV((double)T, PNR_DMUL((double)nonzero, (double)w));
+}
+
 // Row r - a.r0 of every output of pnr_sample_ray_batch for the global ray r (off: a.pix_offset or a copy of it).
-PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, int64_t r) {
+// kWeighted: the pixel drawn through the weight table *wt (pnr_sample_ray_batch_weighted; the caller has checked it).
+template <bool kWeighted = false>
+PNR_HD void pnr_ray_batch_row(const pnr_ray_batch_args& a, const int64_t* off, int64_t r,
+                              const pnr_ray_batch_weights* wt = nullptr) {
   const int64_t row = r - a.r0;
   uint32_t w[4];
   pnr_ray_draw(a.seed, a.step, r, 0u, w);
-  const int64_t p = (int64_t)pnr_mulhi64(((uint64_t)w[0] << 32) | w[1], (uint64_t)a.P);
+  int64_t p;
+  if (kWeighted) {
+    p = pnr_weighted_pixel(wt->weight, wt->weight_cum, a.P,
+                           pnr_mulhi64(((uint64_t)w[0] << 32) | w[1], wt->weight_total));
+    if (wt->importance)
+      wt->importance[row] = pnr_importance(wt->weight_total, wt->weight_nonzero, PNR_LDG(wt->weight + p));
+  } else {
+    p = (int64_t)pnr_mulhi64(((uint64_t)w[0] << 32) | w[1], (uint64_t)a.P);
+  }
   const int f = pnr_frame_of(off, a.F, p);
   int cam = a.frame_cam[f];
   cam = cam < 0 ? 0 : (cam >= a.num_cameras ? a.num_cameras - 1 : cam);

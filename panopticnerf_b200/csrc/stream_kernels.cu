@@ -5,8 +5,8 @@
 //   composite : one warp per ray; lanes stride the sample axis; transmittance is an exclusive
 //               product scan done with warp shuffles; per-class logits are accumulated with lanes
 //               striding the (contiguous) channel axis so every raw row is read once, coalesced.
-//   ray batch : one thread per training ray: a seeded random pixel of a device frame set, its camera ray, targets
-//               and jitter (pnr_ray_batch_row of ray_math.h).
+//   ray batch : one thread per training ray: a seeded random pixel of a device frame set (uniform, or through a
+//               pixel weight table's prefix sums), its camera ray, targets and jitter (pnr_ray_batch_row of ray_math.h).
 //   depth     : LiDAR depth targets: grid-strided over (pair, point), a z-buffer by integer atomicMin, then per pixel
 //               the final depth or the occlusion filter (pnr_project_point / pnr_depth_pixel of ray_math.h).
 #include "common.cuh"
@@ -98,6 +98,22 @@ __global__ void __launch_bounds__(kRayBatchThreads) ray_batch_kernel(const pnr_r
   for (int64_t i = (int64_t)blockIdx.x * kRayBatchThreads + threadIdx.x; i < n;
        i += (int64_t)gridDim.x * kRayBatchThreads)
     pnr_ray_batch_row(a, off, a.r0 + i);
+}
+// the same with the pixel drawn through the weight table (pnr_sample_ray_batch_weighted)
+template <bool kSmemOff>
+__global__ void __launch_bounds__(kRayBatchThreads) ray_batch_weighted_kernel(const pnr_ray_batch_args a,
+                                                                              const __grid_constant__ pnr_ray_batch_weights wt) {
+  extern __shared__ int64_t s_off[];
+  const int64_t* off = a.pix_offset;
+  if (kSmemOff) {
+    for (int i = threadIdx.x; i <= a.F; i += kRayBatchThreads) s_off[i] = a.pix_offset[i];
+    __syncthreads();
+    off = s_off;
+  }
+  const int64_t n = a.r1 - a.r0;
+  for (int64_t i = (int64_t)blockIdx.x * kRayBatchThreads + threadIdx.x; i < n;
+       i += (int64_t)gridDim.x * kRayBatchThreads)
+    pnr_ray_batch_row<true>(a, off, a.r0 + i, &wt);
 }
 
 // ------------------------------------------------------------------------------------ LiDAR depth targets
@@ -638,39 +654,63 @@ extern "C" int pnr_generate_rays(int32_t H, int32_t W, int32_t row0, int32_t row
   return PNR_OK;
 }
 
-extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream) {
-  PNR_CHECK_ARG(args, "pnr_sample_ray_batch: null args");
+// pnr_sample_ray_batch (wt NULL) and pnr_sample_ray_batch_weighted: the checks of both, then one launch
+static int sample_ray_batch(const char* fn, const pnr_ray_batch_args* args, const pnr_ray_batch_weights* wt,
+                            void* stream) {
+  PNR_CHECK_ARG(args, "%s: null args", fn);
   const pnr_ray_batch_args& a = *args;
-  PNR_CHECK_ARG(a.F >= 1 && a.F < INT32_MAX, "pnr_sample_ray_batch: F=%d outside [1, 2^31 - 1)", a.F);
-  PNR_CHECK_ARG(a.P >= 1, "pnr_sample_ray_batch: P=%lld < 1", (long long)a.P);
+  PNR_CHECK_ARG(a.F >= 1 && a.F < INT32_MAX, "%s: F=%d outside [1, 2^31 - 1)", fn, a.F);
+  PNR_CHECK_ARG(a.P >= 1, "%s: P=%lld < 1", fn, (long long)a.P);
   PNR_CHECK_ARG(a.r0 >= 0 && a.r1 >= a.r0 && a.r1 <= (int64_t(1) << 32),
-                "pnr_sample_ray_batch: range r0=%lld r1=%lld is not 0 <= r0 <= r1 <= 2^32", (long long)a.r0,
-                (long long)a.r1);
-  PNR_CHECK_ARG(a.N >= 1 && a.N <= 32 * kCompMaxPerLane, "pnr_sample_ray_batch: N=%d outside [1,%d]", a.N,
-                32 * kCompMaxPerLane);
-  PNR_CHECK_ARG(a.Ni >= 0 && a.Ni <= 32 * kCompMaxPerLane - a.N, "pnr_sample_ray_batch: Ni=%d outside [0,%d] (N + Ni <= %d)",
-                a.Ni, 32 * kCompMaxPerLane - a.N, 32 * kCompMaxPerLane);
-  int rc = check_cameras("pnr_sample_ray_batch", a.cams, a.num_cameras, 31);
+                "%s: range r0=%lld r1=%lld is not 0 <= r0 <= r1 <= 2^32", fn, (long long)a.r0, (long long)a.r1);
+  PNR_CHECK_ARG(a.N >= 1 && a.N <= 32 * kCompMaxPerLane, "%s: N=%d outside [1,%d]", fn, a.N, 32 * kCompMaxPerLane);
+  PNR_CHECK_ARG(a.Ni >= 0 && a.Ni <= 32 * kCompMaxPerLane - a.N, "%s: Ni=%d outside [0,%d] (N + Ni <= %d)", fn, a.Ni,
+                32 * kCompMaxPerLane - a.N, 32 * kCompMaxPerLane);
+  int rc = check_cameras(fn, a.cams, a.num_cameras, 31);
   if (rc != PNR_OK) return rc;
   PNR_CHECK_ARG(a.c2w && a.frame_cam && a.pix_offset && a.rgb8,
-                "pnr_sample_ray_batch: null frame-set pointer (c2w, frame_cam, pix_offset and rgb8 are required)");
-  PNR_CHECK_ARG(a.rays && a.rgb && a.u, "pnr_sample_ray_batch: null output pointer (rays, rgb and u are required)");
-  PNR_CHECK_ARG(a.Ni == 0 || a.u_fine, "pnr_sample_ray_batch: null output pointer u_fine with Ni=%d", a.Ni);
+                "%s: null frame-set pointer (c2w, frame_cam, pix_offset and rgb8 are required)", fn);
+  PNR_CHECK_ARG(a.rays && a.rgb && a.u, "%s: null output pointer (rays, rgb and u are required)", fn);
+  PNR_CHECK_ARG(a.Ni == 0 || a.u_fine, "%s: null output pointer u_fine with Ni=%d", fn, a.Ni);
+  if (wt) {
+    PNR_CHECK_ARG(wt->weight && wt->weight_cum, "%s: null weight table (weight and weight_cum are required)", fn);
+    PNR_CHECK_ARG(wt->weight_total > 0, "%s: weight_total=0: every pixel has weight 0", fn);
+    PNR_CHECK_ARG(wt->weight_nonzero >= 1 && wt->weight_nonzero <= a.P, "%s: weight_nonzero=%lld outside [1, P=%lld]",
+                  fn, (long long)wt->weight_nonzero, (long long)a.P);
+    PNR_CHECK_ARG(wt->weight_total >= (uint64_t)wt->weight_nonzero &&
+                      wt->weight_total / 65535u + (wt->weight_total % 65535u != 0) <= (uint64_t)wt->weight_nonzero,
+                  "%s: weight_total=%llu outside [weight_nonzero, 65535 weight_nonzero] (weight_nonzero=%lld)", fn,
+                  (unsigned long long)wt->weight_total, (long long)wt->weight_nonzero);
+  }
   const int64_t n = a.r1 - a.r0;
   if (n == 0) return PNR_OK;
   int dev = 0;
-  rc = current_device("pnr_sample_ray_batch", &dev);
+  rc = current_device(fn, &dev);
   if (rc != PNR_OK) return rc;
   const int64_t want = (n + kRayBatchThreads - 1) / kRayBatchThreads, cap = (int64_t)num_sms(dev) * 8;
   const int64_t blocks = want < cap ? want : cap;
-  if (a.F + 1 <= kRayBatchSmemOff) {
-    ray_batch_kernel<true><<<(unsigned)blocks, kRayBatchThreads, (size_t)(a.F + 1) * sizeof(int64_t),
-                             (cudaStream_t)stream>>>(a);
+  const size_t smem = (size_t)(a.F + 1) * sizeof(int64_t);
+  const cudaStream_t st = (cudaStream_t)stream;
+  if (wt) {
+    if (a.F + 1 <= kRayBatchSmemOff) ray_batch_weighted_kernel<true><<<(unsigned)blocks, kRayBatchThreads, smem, st>>>(a, *wt);
+    else ray_batch_weighted_kernel<false><<<(unsigned)blocks, kRayBatchThreads, 0, st>>>(a, *wt);
+    PNR_LAUNCH_CHECK("ray_batch_weighted_kernel");
   } else {
-    ray_batch_kernel<false><<<(unsigned)blocks, kRayBatchThreads, 0, (cudaStream_t)stream>>>(a);
+    if (a.F + 1 <= kRayBatchSmemOff) ray_batch_kernel<true><<<(unsigned)blocks, kRayBatchThreads, smem, st>>>(a);
+    else ray_batch_kernel<false><<<(unsigned)blocks, kRayBatchThreads, 0, st>>>(a);
+    PNR_LAUNCH_CHECK("ray_batch_kernel");
   }
-  PNR_LAUNCH_CHECK("ray_batch_kernel");
   return PNR_OK;
+}
+
+extern "C" int pnr_sample_ray_batch(const pnr_ray_batch_args* args, void* stream) {
+  return sample_ray_batch("pnr_sample_ray_batch", args, nullptr, stream);
+}
+
+extern "C" int pnr_sample_ray_batch_weighted(const pnr_ray_batch_args* args, const pnr_ray_batch_weights* w,
+                                             void* stream) {
+  PNR_CHECK_ARG(w, "pnr_sample_ray_batch_weighted: null weights (w)");
+  return sample_ray_batch("pnr_sample_ray_batch_weighted", args, w, stream);
 }
 
 extern "C" size_t pnr_project_depth_workspace_bytes(int64_t P, int32_t occlusion_radius) {

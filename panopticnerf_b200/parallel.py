@@ -41,17 +41,20 @@ TRAIN_RAY_KEYS = ("rays", "near", "far", "u", "u_fine", "noise", "noise_fine", "
                   "pseudo_weight")
 # per-ray keys that only a batch on a sequence table (kitti360.sequence_primitives) carries: sliced with the rays too
 FRAME_RAY_KEYS = ("ray_frame",)
+# per-ray keys that only a weighted batch (RaySampler(weights=...)) carries: sliced with the rays too
+WEIGHTED_RAY_KEYS = ("importance",)
 
 
 def shard_training_batch(batch: Dict[str, torch.Tensor], rank: int, world: int) -> Dict[str, torch.Tensor]:
     """A training batch's shard for data-parallel training: the rays and every per-ray target and random draw
-    (TRAIN_RAY_KEYS, FRAME_RAY_KEYS) are sliced to `shard_range`; scene tensors (primitives, meshes, aabb, a sequence
-    table's frame_boxes) are replicated.  A rank past the last ray gets an empty shard (zero rows)."""
+    (TRAIN_RAY_KEYS, FRAME_RAY_KEYS, WEIGHTED_RAY_KEYS) are sliced to `shard_range`; scene tensors (primitives,
+    meshes, aabb, a sequence table's frame_boxes) are replicated.  A rank past the last ray gets an empty shard (zero
+    rows)."""
     R = batch["rays"].shape[0]
     lo, hi = shard_range(R, rank, world)
     out = {}
     for k, v in batch.items():
-        if (k in TRAIN_RAY_KEYS or k in FRAME_RAY_KEYS) and torch.is_tensor(v):
+        if (k in TRAIN_RAY_KEYS or k in FRAME_RAY_KEYS or k in WEIGHTED_RAY_KEYS) and torch.is_tensor(v):
             if v.dim() < 1 or v.shape[0] != R:
                 raise ValueError(f"shard_training_batch: {k} has shape {tuple(v.shape)}, expected a leading dim of R={R}")
             out[k] = v[lo:hi].contiguous()
